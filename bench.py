@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA kernels through the C-ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port)
+    python bench.py --steps K --dump-outputs DIR             # also write the last timed step's outputs as DIR/*.npy
 
 A "step" is one training step's worth of the hot path over one batch of 1024 synthetic quadruples:
 both directions (train.py:136-137) x both RGCN layers (Aggregator.py:136-137) over the batched history
@@ -17,7 +18,7 @@ graphs, i.e. 4 fused-layer passes = 2*(E_subj + E_obj) edge-messages (SURVEY.md 
               host cores, bounded sample
 
 L2 hygiene: the timed steps rotate over a pool of distinct pre-built batches whose combined footprint
-(graph arrays + layer outputs) exceeds 2x the 126 MB L2 ("l2": "rotating-pool" in config).
+(graph arrays + layer outputs) exceeds 2x the 50 MB L2 of an H100 ("l2": "rotating-pool" in config).
 """
 import argparse
 import json
@@ -93,6 +94,8 @@ def parse():
                          "as the line's value")
     ap.add_argument('--no-train', action='store_true', help='skip the training-step region of the default line')
     ap.add_argument('--dropout', type=float, default=0.0, help='dropout of the training-step region (reference default 0.5)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32)')
     return ap.parse_args()
 
 
@@ -112,7 +115,7 @@ def _cpu_quota():
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe).  NVML is
+    """SM clock and throttle reasons sampled DURING the timed region.  NVML is
     polled in-process every few ms (a fresh `nvidia-smi -lms` takes longer to start than the timed region
     lasts); falls back to one nvidia-smi query if pynvml is unavailable."""
 
@@ -183,18 +186,18 @@ def measured_peak_gbs():
             return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet: 3.35 TB/s HBM3, not measured)'
 
 
 def measured_peak_tf32():
-    """Dense TF32 tensor peak = half the measured bf16 cuBLAS throughput (MEASURED_PEAKS.json), else half the nominal 2.25 PF."""
+    """Dense TF32 tensor peak = half the measured bf16 cuBLAS throughput (MEASURED_PEAKS.json), else the H100 SXM data sheet."""
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         try:
             return float(json.load(open(p))['bf16_tflops']) / 2, 'measured (MEASURED_PEAKS.json bf16_tflops / 2: TF32 runs at half the bf16 rate)'
         except Exception:
             pass
-    return 1125.0, 'fallback (nominal 2.25 PFLOP/s bf16 / 2)'
+    return 495.0, 'fallback (H100 SXM data sheet: 495 TFLOP/s dense TF32, not measured)'
 
 
 def ncu_traffic():
@@ -350,6 +353,23 @@ def train_region(args, tkg, pool, global_emb, dev, world, torch, dist):
                     '-> gradient all-reduce -> clip_grad_norm_(1.0) -> Adam(lr 1e-3, wd 1e-5); phase times are max over ranks'}
 
 
+DUMP_SAMPLE_ROWS = 8192
+
+
+def dump_outputs(out_dir, e, np):
+    """The arrays one timed step hands its caller, for both directions: `h2_<dir>` = layer-2 output (the read-out rows that
+    feed the GRU, [S, 200]) in full, `h1_<dir>` = layer-1 output ([N, 200], 27 MB per direction at the ICEWS18 shape) on a
+    fixed seeded sample of DUMP_SAMPLE_ROWS rows whose indices are `h1_<dir>_rows`.  float32; about 15 MB in all."""
+    os.makedirs(out_dir, exist_ok=True)
+    for d in e['dirs']:
+        tag = 'obj' if d['reverse'] else 'subj'
+        H1 = d['H1'].float().cpu().numpy()
+        rows = np.sort(np.random.RandomState(0).choice(len(H1), min(len(H1), DUMP_SAMPLE_ROWS), replace=False))
+        np.save(os.path.join(out_dir, 'h1_%s.npy' % tag), H1[rows])
+        np.save(os.path.join(out_dir, 'h1_%s_rows.npy' % tag), rows.astype(np.float64))
+        np.save(os.path.join(out_dir, 'h2_%s.npy' % tag), d['H2'].float().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------------------------------
 def run_ours(args):
     import torch
@@ -454,7 +474,7 @@ def run_ours(args):
 
     def device_step(e, events=None):
         # every step is a new weight generation, as in training (the optimiser changes the weights between steps): the
-        # tcgen05 engine packs each self-loop matrix once per step and both directions use the image
+        # tensor-core engine packs each self-loop matrix once per step and both directions use the image
         step_no[0] += 1
         L.renet_set_weight_generation(step_no[0])
         k = 0
@@ -487,6 +507,8 @@ def run_ours(args):
     launches = _lib.launch_count() - n0
     elapsed_ms = start.elapsed_time(end)
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pool[(args.warmup + args.steps - 1) % len(pool)], np)
     t = torch.tensor([elapsed_ms, float(total_msgs)], device=dev, dtype=torch.float64)
     if world > 1:
         tmax = t.clone(); dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
@@ -526,7 +548,7 @@ def run_ours(args):
 
     mm_achieved = float(np.sum(mm_bytes) / (np.sum(mm_ms) * 1e-3) / 1e9)
     tf32_peak, tf32_src = measured_peak_tf32()
-    roofline_gemm = {'kernel': 'umma_gemm_packed_kernel (layer-1 self-loop product, tcgen05 3xTF32)', 'bound': 'hbm',
+    roofline_gemm = {'kernel': 'umma_gemm_packed_kernel (layer-1 self-loop product, wgmma 3xTF32)', 'bound': 'hbm',
                      'achieved': mm_achieved, 'peak': peak, 'unit': 'GB/s', 'frac': mm_achieved / peak,
                      'avg_launch_us': float(np.mean(mm_ms) * 1e3), 'algorithmic_bytes_per_launch': float(np.mean(mm_bytes)),
                      'tensor_tflops_3xtf32': float(3 * np.sum(mm_flops) / (np.sum(mm_ms) * 1e-3) / 1e12), 'tf32_peak_tflops': tf32_peak,
@@ -536,7 +558,7 @@ def run_ours(args):
     if os.environ.get('RENET_STREAM_TL') == '1' and rank == 0:
         # debug: per-warp time stamps of ONE layer-1 gather launch in the middle of a step (tools/stream_timeline.py explains them)
         WARPS = int(os.environ.get('RENET_STREAM_WARPS', '32'))
-        buf = torch.zeros(148 * WARPS * 8, dtype=torch.int64, device=dev)
+        buf = torch.zeros(132 * WARPS * 8, dtype=torch.int64, device=dev)
         e = pool[(args.warmup + 3) % len(pool)]
         d = e['dirs'][0]
         _lib.check(L.renet_selfloop_gemm(P(ent), P(d['g'].node_ent), P(L1), P(d['H1']), d['g'].N, H_DIM, H_DIM, stream), 'gemm')
@@ -546,9 +568,9 @@ def run_ours(args):
                                            P(d['H1']), d['g'].N, d['g'].E, H_DIM, H_DIM, NUM_BASES, R2, 1, 1, P(hot), hot.numel(), stream), 'gather')
         torch.cuda.synchronize()
         L.renet_debug_stream_timing(None)
-        t = buf.cpu().numpy().reshape(148, WARPS, 8).astype(np.float64)
+        t = buf.cpu().numpy().reshape(132, WARPS, 8).astype(np.float64)
         g0 = t[:, :, 5].min()
-        ph = [(t[:, :, 1] - t[:, :, 0]) / 1965.0, (t[:, :, 2] - t[:, :, 1]) / 1965.0, (t[:, :, 3] - t[:, :, 2]) / 1965.0, (t[:, :, 4] - t[:, :, 3]) / 1965.0]
+        ph = [(t[:, :, 1] - t[:, :, 0]) / 1980.0, (t[:, :, 2] - t[:, :, 1]) / 1980.0, (t[:, :, 3] - t[:, :, 2]) / 1980.0, (t[:, :, 4] - t[:, :, 3]) / 1980.0]
         sys.stderr.write('stream timeline in context: span %.1f us, entry skew %.1f us; medians (us): search %.1f, prologue %.1f, loop %.1f, tail %.1f; '
                          'max loop %.1f\n' % ((t[:, :, 6].max() - g0) / 1e3, (t[:, :, 5].min(1).max() - g0) / 1e3, np.median(ph[0]), np.median(ph[1]),
                                               np.median(ph[2]), np.median(ph[3]), ph[2].max()))
@@ -575,7 +597,7 @@ def run_ours(args):
             S_rows, Q_seq = int(hb.S), int(len(hb.seq_len))
             steps_rows = int(np.sum(hb.seq_len))                       # sum over time steps of the active sequences
             flops = 2.0 * H_DIM * 6 * H_DIM * (S_rows + 2 * Q_seq + len(hb.times) + steps_rows)
-            roofline_gru = {'kernel': 'fused read-out + GRU of one direction: 4 tcgen05 projection GEMMs + gru_recur_kernel (both encoders)',
+            roofline_gru = {'kernel': 'fused read-out + GRU of one direction: 4 wgmma projection GEMMs + gru_recur_kernel (both encoders)',
                             'bound': 'tensor', 'achieved': 3 * flops / (gru_ms * 1e-3) / 1e12, 'peak': tf32_peak, 'unit': 'TFLOP/s',
                             'frac': 3 * flops / (gru_ms * 1e-3) / 1e12 / tf32_peak, 'peak_source': tf32_src, 'ms': gru_ms,
                             'algorithmic_flops': flops, 'rows': S_rows, 'sequences': Q_seq,
@@ -656,7 +678,7 @@ def run_ours(args):
         E2E_DEPTH = 4
         hoststore.reserve_pinned(4 * (E2E_DEPTH + 3))     # every staging buffer the loader can need, pinned up front
         E2E_WORKERS = max(2, min(8, _rank_cpu_budget() - int(os.environ.get('OMP_NUM_THREADS', '1')) - 1))
-        k_e2e = max(4, args.steps)
+        k_e2e = args.steps
         # one full rotation over the pool of batches: the loader, the pinned pool and the caching allocator (whose block
         # sizes depend on the batch) have reached steady state before the clock starts
         w_e2e = max(len(pool) + 1, args.warmup)
@@ -706,7 +728,7 @@ def run_ours(args):
         line = {'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps, 'warmup': args.warmup,
                 'ms_per_step': elapsed_ms / args.steps, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
                 'dtype': 'f32', 'data': 'synthetic',
-                'config': {'workload': WORKLOAD, 'step': '2 directions x 2 RGCN layers (tcgen05 3xTF32 self-loop GEMM + fused gather; layer 2 on the read-out sub-graph); every step is a new weight generation: each self-loop matrix is packed once per step and shared by both directions',
+                'config': {'workload': WORKLOAD, 'step': '2 directions x 2 RGCN layers (wgmma 3xTF32 self-loop GEMM + fused gather; layer 2 on the read-out sub-graph); every step is a new weight generation: each self-loop matrix is packed once per step and shared by both directions',
                            'nodes_per_direction': [d['g'].N for d in g0], 'edges_per_direction': [d['g'].E for d in g0],
                            'edge_msgs_per_step': msgs_per_step[0], 'edge_msgs_executed_per_step': msgs_executed[0],
                            'layer2': 'read-out sub-graph only (identical on every consumed row, Aggregator.py:140); value counts the full E for both layers',
@@ -724,6 +746,8 @@ if __name__ == '__main__':
     if a.timestamps is None:
         a.timestamps = WORKLOADS[a.workload][1]
     WORKLOAD = WORKLOADS[a.workload][2]
+    if a.dump_outputs and (a.workload == 'synth1m' or a.impl == 'reference'):
+        raise SystemExit('bench.py: --dump-outputs covers the CUDA arm of the icews18 and gdelt workloads')
     if a.workload == 'synth1m' and a.impl != 'reference':
         from bench_synth import run_synth1m
         run_synth1m(a, WORKLOAD, METRIC, UNIT, ClockSampler, measured_peak_gbs)

@@ -1,6 +1,6 @@
 """bench.py --workload synth1m: BASELINE.json configs[4] -- a synthetic TKG shard of 1M entities / 500 relations / 250
 timesteps per GPU with mean in-degree 32 (N = 1M nodes, E = 32M directed edges per GPU, weak scaling over GPUs).  The only
-configuration whose feature matrix (800 MB) does not fit the 126 MB L2, i.e. where HBM is the true bound of the gather.
+configuration whose feature matrix (800 MB) does not fit the 50 MB L2, i.e. where HBM is the true bound of the gather.
 Aggregate + GRU only (SURVEY.md section 8(d): the 1M-class decoder is out of scope).
 
 A step = one direction over the shard's batched graph: layer 1 (self-loop GEMM + fused gather over all N / E), layer 2
@@ -206,7 +206,7 @@ def run_synth1m(args, WORKLOAD, METRIC, UNIT, ClockSampler, measured_peak_gbs):
                        'readout_rows': S, 'sequences': Q, 'readout_nodes': U, 'readout_subgraph_edges': E2,
                        'step': 'one direction: layer 1 over the whole shard, layer 2 on the read-out sub-graph, fused read-out + GRUs',
                        'edge_msgs_per_step': 2 * E, 'edge_msgs_executed_per_step': E + E2,
-                       'l2': 'inputs (800 MB of features + 384 MB of CSR per GPU) far exceed the 126 MB L2',
+                       'l2': 'inputs (800 MB of features + 384 MB of CSR per GPU) far exceed the 50 MB L2 of an H100',
                        'parallelism': 'dp%d (independent shards by timestep range, no data-path collective)' % world},
             'clocks': clk, 'e2e': e2e, 'gpu_launches': int(launches),
             'roofline': {'kernel': 'rgcn_gather_d200_kernel (layer 1, whole shard)', 'bound': 'hbm', 'achieved': achieved, 'peak': peak,

@@ -1,5 +1,5 @@
 /*
- * renet_b200.h -- C-ABI of librenet_b200.so: the B200 (sm_100a) kernels behind RE-Net's
+ * renet_b200.h -- C-ABI of librenet_b200.so: the H100 (sm_90a) kernels behind RE-Net's
  * RGCN-aggregate + GRU hot path.
  *
  * The reference (INK-USC/RE-Net) is pure Python and has no FFI of its own; the entry points below
@@ -29,7 +29,7 @@ typedef enum {
   RENET_OK = 0,
   RENET_ERR_INVALID_ARG = -1,   /* bad shape / null pointer / unsupported configuration        */
   RENET_ERR_CUDA = -2,          /* a CUDA runtime call or kernel launch failed                   */
-  RENET_ERR_NO_DEVICE = -3      /* no sm_100 device visible                                      */
+  RENET_ERR_NO_DEVICE = -3      /* no sm_90 device visible                                       */
 } renet_status;
 
 /* Library version (major*10000 + minor*100 + patch). */
@@ -41,12 +41,12 @@ const char* renet_last_error(void);
 int64_t renet_launch_count(void);
 
 /* Dense-GEMM engine used for the self-loop and GRU projections: 0 = FFMA (fp32 CUDA cores),
- * 1 = tcgen05 3xTF32 (tensor cores, fp32-accurate split).  Both are this library's own kernels.
+ * 1 = wgmma 3xTF32 (tensor cores, fp32-accurate split).  Both are this library's own kernels.
  * Process-wide; the initial value comes from the RENET_GEMM environment variable (ffma|umma).
  * renet_set_gemm_engine returns the previous engine. */
 int renet_set_gemm_engine(int engine);
 int renet_get_gemm_engine(void);
-/* Packed-weight cache of the tcgen05 GEMM engine.  The engine consumes weights (self-loop matrices, GRU W_ih / W_hh)
+/* Packed-weight cache of the wgmma GEMM engine.   The engine consumes weights (self-loop matrices, GRU W_ih / W_hh)
  * in a packed shared-memory operand image; packing is a kernel launch per weight per call.  Declaring a weight
  * generation >= 0 promises that every weight passed by pointer is unchanged while the generation is unchanged: packed
  * images are then kept per (device, pointers, shape) and reused, and any change of the generation invalidates all of
@@ -454,7 +454,7 @@ int renet_readout_subgraph(const int32_t* readout, int64_t S, int64_t N,
  * Decoder: logits = X @ W^T + bias followed by cross-entropy (reference model.py:89-91: object prediction, X = [ent[s] |
  * s_h | rel[r]] [B,3h], W = linear.weight [|E|,3h]; model.py:97-100: relation prediction, [B,2h] x [R,2h]).
  *   renet_decoder_ce_fwd : loss_rows[i] = logsumexp_c(logits[i,c]) - logits[i,target[i]], lse[i] = the logsumexp (kept for
- *       backward).  tcgen05 3xTF32 GEMM with a fused epilogue: the [B,|E|] logits never reach memory.
+ *       backward).  wgmma 3xTF32 GEMM with a fused epilogue: the [B,|E|] logits never reach memory.
  *   renet_decoder_ce_bwd : for loss = scale * d_scale[0] * sum_i loss_rows[i] (the reference's mean: scale = 1/B; d_scale =
  *       optional DEVICE scalar, the upstream gradient, so that autograd needs no host read): dX [M,K] written; dW [N,K] and dbias [N] (may be NULL) ACCUMULATED.  The logits are recomputed; the
  *       gradient of the logits (M x N floats, row-major and transposed) lives in the workspace only.

@@ -524,6 +524,45 @@ def gen_renet_eval_global(ns):
     print('renet_eval_global.npz: %d ranks, MRR %.6f MR %.3f Hits@1/3/10 %s' % (len(ranks), res['mrr'], res['mr'], res['hits']))
 
 
+def live_layer_cases():
+    """Inputs of tests/golden/live_layers.npz: four RGCN block layers of RE-Net's shape (200 -> 200, 100 bases of 2x2,
+    self-loop, relu) on random graphs, reproducible without the reference; `rows` is the seeded sample of destinations
+    whose reference outputs are stored (the full outputs would be 690 KB)."""
+    rng = np.random.RandomState(0)
+    cases = []
+    for seed in range(4):
+        N, E, R2 = int(rng.randint(1, 400)), int(rng.randint(1, 3000)), 32
+        src, dst = rng.randint(0, N, E), rng.randint(0, N, E)
+        ty = rng.randint(0, R2, E)
+        v = np.random.RandomState(100 + seed)
+        H = v.standard_normal((N, 200)).astype(np.float32)
+        W = (v.standard_normal((R2, 400)) * 0.1).astype(np.float32)
+        Wl = (v.standard_normal((200, 200)) * 0.07).astype(np.float32)
+        rows = np.sort(v.choice(N, min(N, 8), replace=False))
+        cases.append(dict(N=N, R2=R2, src=src, dst=dst, ty=ty, H=H, W=W, Wl=Wl, rows=rows))
+    return cases
+
+
+def gen_live_layers(ns):
+    import torch.nn.functional as F
+    blob = {}
+    for i, c in enumerate(live_layer_cases()):
+        with ref_loader.cpu_patches():
+            layer = ns.RGCN.RGCNBlockLayer(200, 200, c['R2'], 100, activation=F.relu, self_loop=True, dropout=0.0)
+            with torch.no_grad():
+                layer.weight.copy_(torch.from_numpy(c['W']))
+                layer.loop_weight.copy_(torch.from_numpy(c['Wl']))
+            g = ns.dgl.DGLGraph(); g.add_nodes(c['N']); g.add_edges(c['src'], c['dst'])
+            g.ndata['norm'] = ns.utils.comp_deg_norm(g).view(-1, 1)
+            g.edata['type_s'] = torch.as_tensor(c['ty']); g.edata['type_o'] = torch.as_tensor(c['ty'])
+            g.ndata['h'] = torch.from_numpy(c['H']).clone()
+            layer(g, False)
+        blob['%d/norm' % i] = g.ndata['norm'].view(-1).numpy().astype(np.float32)
+        blob['%d/out_rows' % i] = g.ndata['h'].detach().numpy()[c['rows']].astype(np.float32)
+    np.savez_compressed(os.path.join(OUT, 'live_layers.npz'), **blob)
+    print('live_layers.npz: %d layers' % (len(blob) // 2))
+
+
 if __name__ == '__main__':
     os.makedirs(OUT, exist_ok=True)
     ns = ref_loader.load()
@@ -536,3 +575,4 @@ if __name__ == '__main__':
     gen_aggregator_predict(ns)
     gen_global_tiny(ns)
     gen_renet_eval_global(ns)
+    gen_live_layers(ns)

@@ -169,7 +169,7 @@ def invalidate_packed_weights():
 
 
 class weight_generation:
-    """Context manager: while active, the tcgen05 GEMM engine may reuse packed weight images made under the same
+    """Context manager: while active, the tensor-core GEMM engine may reuse packed weight images made under the same
     generation = hash(module token, invalidation epoch, (address, in-place version) of every weight).  Outside of it the
     cache is off, so direct C-ABI callers are never served a stale image.  Only version-bumping in-place updates are
     tracked automatically; anything else must call ``invalidate_packed_weights()`` (the trainer in parallel.py does)."""

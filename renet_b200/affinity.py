@@ -1,6 +1,6 @@
 """CPU placement of one-process-per-GPU jobs on a multi-socket host.
 
-On the 8-GPU B200 boxes GPUs 0-3 hang off NUMA node 0 and GPUs 4-7 off node 1.  The end-to-end path of this repo is
+On a typical two-socket 8-GPU server GPUs 0-3 hang off NUMA node 0 and GPUs 4-7 off node 1.  The end-to-end path of this repo is
 host-driven (batch planning in loader threads, one consumer thread issuing CUDA calls), so eight ranks whose threads
 float over both sockets -- and over each other's cores -- lose more than half of their throughput (round-1 SCALE:
 e2e efficiency 0.43 at N=8).  ``pin_rank`` restricts the calling process (and every thread it creates afterwards) to

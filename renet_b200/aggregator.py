@@ -1,4 +1,4 @@
-"""RGCNAggregator with the reference's surface (reference Aggregator.py:109-237) on the sm_100a kernels.
+"""RGCNAggregator with the reference's surface (reference Aggregator.py:109-237) on the sm_90a kernels.
 
 Kept verbatim from the reference: constructor signature and attributes, sub-modules ``rgcn1`` /
 ``rgcn2`` (so state_dict keys ``aggregator.rgcn{1,2}.{weight,loop_weight}`` carry over),
@@ -147,7 +147,7 @@ class RGCNAggregator(nn.Module):
         from .gru import fused_gru
         dev = ent_embeds.device
         hb = self._batch(hist, s, graph_dict, dev, True)
-        # weights the tcgen05 GEMM engine packs: unchanged weights (same addresses, same in-place versions) are packed
+        # weights the tensor-core GEMM engine packs: unchanged weights (same addresses, same in-place versions) are packed
         # once and reused across calls -- both directions of a step, and every step in inference
         weights = [self.rgcn1.loop_weight, self.rgcn2.loop_weight, encoder.weight_ih_l0, encoder.weight_hh_l0,
                    encoder_r.weight_ih_l0, encoder_r.weight_hh_l0]

@@ -1,8 +1,8 @@
-"""Build librenet_b200.so in-tree with nvcc for sm_100a (B200) only.
+"""Build librenet_b200.so in-tree with nvcc for sm_90a (H100) only.
 
     python -m renet_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the object files under csrc/build/ are build products (git-ignored).
 """
 import hashlib
 import os
@@ -14,7 +14,8 @@ CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'librenet_b200.so')
 BUILD_DIR = os.path.join(HERE, 'csrc', 'build')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+CUOBJDUMP = os.path.join(os.path.dirname(NVCC), 'cuobjdump')
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
@@ -56,7 +57,7 @@ def build(force=False, verbose=False):
             sys.stderr.write('nvcc failed on %s\n' % src)
     if failed:
         raise RuntimeError('librenet_b200.so: compilation failed')
-    cmd = [NVCC, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+    cmd = [NVCC, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a']
     subprocess.check_call(cmd)
     with open(stamp, 'w') as fh:
         fh.write(dig)

@@ -451,7 +451,7 @@ int renet_encode_fwd(const float* ent, const int32_t* node_ent, const int32_t* r
   RENET_CHECK_ARG(n_hot >= 0 && (n_hot == 0 || hot_rel != nullptr), "renet_encode_fwd: bad hot-relation list");
   if (n_hot == 0) hot_rel = nullptr;
   // The part of the GRU that does not depend on the RGCN output -- weight packing, bias rows, the per-sequence and
-  // per-timestamp input projections: four small launches, ~110 us of latency, a handful of CTAs -- runs on a side stream
+  // per-timestamp input projections: four small launches, latency-bound, a handful of CTAs -- runs on a side stream
   // underneath the two RGCN layers (fork / join by events; the side stream and its events are created on first use and
   // live for the process: one device, one caller stream at a time, as everywhere in this library).
   static cudaStream_t side = nullptr;

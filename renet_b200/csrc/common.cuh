@@ -1,4 +1,4 @@
-// Shared helpers for librenet_b200.so (sm_100a only).
+// Shared helpers for librenet_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -40,7 +40,7 @@ void count_launch(int n = 1);
     ::renet::count_launch();                                                          \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM: one persistent CTA per SM
 
 __device__ __forceinline__ float4 ldg_f4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
@@ -76,13 +76,13 @@ int sgemm_nt(const float* A, int64_t lda, const float* B, int64_t ldb, float* C,
 
 // 0 = automatic, 1 = tile, 3 = stream (RENET_GATHER_KERNEL=tile|stream; rgcn_fwd.cu)
 int gather_kernel_choice();
-constexpr int64_t kStreamMinEdges = 16384;   // below this a persistent 148-CTA launch costs more than the tile kernel
+constexpr int64_t kStreamMinEdges = 16384;   // below this a persistent one-CTA-per-SM launch costs more than the tile kernel
 constexpr int64_t kStreamMinNodes = 16384;
-constexpr int64_t kStreamMaxNodes = 98304;    // 79 MB of fp32 features: beyond this the source rows come from HBM, not L2
+constexpr int64_t kStreamMaxNodes = 40960;    // 33 MB of fp32 features (2/3 of the 50 MB L2): beyond this the source rows come from HBM
 bool gather_use_stream(int64_t E, int64_t N);
 void set_stream_debug_buffer(long long* p);   // debug: per-warp time stamps of the stream kernel (rgcn_fwd.cu)          // the stream kernel (rgcn_stream.cuh) serves this edge count
 
-// tcgen05 GEMM engine building blocks (umma_gemm.cu); gemm_mode() == 1 selects the engine
+// tensor-core (wgmma) GEMM engine building blocks (umma_gemm.cu); gemm_mode() == 1 selects the engine
 int gemm_mode();
 int64_t umma_packed_bytes(int N, int K);
 // packed-weight cache (umma_gemm.cu): persistent device buffer for this key, or nullptr when caching is off; *hit says
@@ -91,7 +91,7 @@ void set_weight_generation(int64_t g);
 void* packed_cache_lookup(const void* const* keys, int nkeys, int64_t bytes, bool* hit);
 bool umma_shape_ok(int N, int K);
 int umma_pack_b(const float* B, int64_t sk, int64_t sn, int N, int K, void* Bp, int tile_offset, cudaStream_t stream);
-// fused epilogues of the packed tcgen05 GEMM (umma_gemm.cu): see the comment there
+// fused epilogues of the packed wgmma GEMM (umma_gemm.cu): see the comment there
 struct EpiArgs {
   const int32_t* target;   // [M] class of every row
   const float* lse;        // [M] (EPI 2)

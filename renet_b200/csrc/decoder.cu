@@ -1,7 +1,7 @@
 // Decoder of RE-Net: logits = X @ W^T + b followed by cross-entropy (reference model.py:89-91 object prediction
 // [B, 3h] x [3h, |E|]; model.py:97-100 relation prediction [B, 2h] x [2h, R]) -- SURVEY.md section 8(f) row 3.
 //
-// Forward: the tcgen05 3xTF32 GEMM (umma_gemm.cu) with a fused epilogue: every (row, half column tile) reduces its
+// Forward: the wgmma 3xTF32 GEMM (umma_gemm.cu) with a fused epilogue: every (row, half column tile) reduces its
 // logits to a running (max, sum of exp) pair and the target's logit, so the [B, |E|] logits (94 MB at ICEWS18) never
 // reach memory; ce_reduce_kernel combines the 2*ceil(|E|/200) partials per row into logsumexp and the per-row loss.
 // Backward: the logits are recomputed by the same GEMM with the gradient epilogue

@@ -313,7 +313,7 @@ int launch_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_g
     return RENET_OK;
   };
   int rc;
-  // Tensor-core engine: weights go straight into the UMMA operand image (hi/lo planes, K-major, 128-byte swizzle),
+  // Tensor-core engine: weights go straight into the packed operand image (hi/lo planes, K-major, 128-byte swizzle),
   // ONCE per call -- the recurrent weights are re-used by every time step -- and every GEMM is one launch; the two
   // encoders' recurrent GEMMs are batched into a single launch per step.
   const bool use_umma = gemm_mode() == 1 && h % 4 == 0 && (3 * h) % 200 == 0 &&

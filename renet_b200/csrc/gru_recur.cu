@@ -6,7 +6,7 @@
 //     rows of its 32 units, split hi/lo for 3xTF32, K-major, 128-byte swizzled: 172 KB -- resident in shared memory
 //     for the whole kernel;
 //   * every step it stages its 128 x 200 tile of h_{t-1} (ld.global.cg: written by other SMs one step earlier),
-//     issues 84 tcgen05.mma (M=128, N=96, K=8) into a TMEM accumulator, and the epilogue (thread = sequence) adds the
+//     issues 84 wgmma per warpgroup (M=64 rows each, N=96, K=8) into register accumulators, and the epilogue adds the
 //     pre-computed input projections GI[row] + PQ[q] + PT[timestamp], applies the gate math and writes h_t (and the
 //     recurrent pre-activations GH, which the backward pass re-uses);
 //   * steps are separated by a grid-wide barrier (atomic counter; the launch is cooperative so all CTAs are resident).
@@ -65,21 +65,8 @@ gru_recur_kernel(const float* __restrict__ GI, const float* __restrict__ PQ, con
   const int n_chunks = (h + R_BK - 1) / R_BK;
   uint8_t* sB = smem;                                   // [chunk][hi,lo][96 rows x 128 B]
   uint8_t* sA = smem + R_MAX_CHUNKS * 2 * R_B_PLANE;    // [hi,lo][128 rows x 128 B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sA + 2 * R_A_BYTES);   // [0] A free, [1] accumulator done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t bar0 = smem_u32(bars);
-  if (tid == 0) {
-    mbar_init(bar0, 1);
-    mbar_init(bar0 + 8, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(128)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
+  const int wg = tid >> 7;                              // warpgroup: accumulator rows [64 wg, 64 wg + 64) of the tile
   // ---- W_hh slice -> shared memory (once): row n' = g*32 + ul  <-  w_hh[g*h + u0 + ul][k] ----------------------------
   const float* w_hh = enc == 0 ? w_hh4 : w_hh3;
   for (int task = tid; task < RN * 8 * n_chunks; task += R_THREADS) {
@@ -96,18 +83,13 @@ gru_recur_kernel(const float* __restrict__ GI, const float* __restrict__ PQ, con
     *reinterpret_cast<float4*>(sB + (size_t)c * 2 * R_B_PLANE + R_B_PLANE + off) = lo;
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t idesc = make_idesc_n(RN);
   const unsigned int n_ctas = gridDim.x * gridDim.y * gridDim.z;
   const int n_mtiles = (Q + 127) / 128;
   const int64_t hs_stride = (int64_t)Q * 2 * h;
-  // epilogue mapping: thread = accumulator row (sequence); warps 0-3 own units [0,16) of the slice, warps 4-7 [16,32)
-  const int erow = (warp & 3) * 32 + lane;
-  const int eu0 = (warp >> 2) * 16;
-  uint32_t mma_phase = 0, afree_phase = 0;   // mbarrier parities (uniform across the CTA: every thread waits on both)
+  float acc[RN / 2];
+#pragma unroll
+  for (int i = 0; i < RN / 2; ++i) acc[i] = 0.f;
   int a_uses = 0;
 
   for (int t = 0; t < max_len; ++t) {
@@ -139,7 +121,11 @@ gru_recur_kernel(const float* __restrict__ GI, const float* __restrict__ PQ, con
 #pragma unroll
         for (int c = 0; c < R_MAX_CHUNKS; ++c) {
           if (c < n_chunks) {
-            if (a_uses > 0) { mbar_wait(bar0, afree_phase); afree_phase ^= 1; }       // previous MMAs have read sA
+            if (a_uses > 0) {                                  // previous MMAs (both warpgroups) have read sA
+              wgmma_wait<0>();
+              acc_fence(acc);
+              __syncthreads();
+            }
             ++a_uses;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
@@ -152,60 +138,36 @@ gru_recur_kernel(const float* __restrict__ GI, const float* __restrict__ PQ, con
               *reinterpret_cast<float4*>(sA + R_A_BYTES + off) = lo;
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
             __syncthreads();
-            if (tid == 0) {
-              asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-              const uint32_t a_hi = smem_base + R_MAX_CHUNKS * 2 * R_B_PLANE, a_lo = a_hi + R_A_BYTES;
-              const uint32_t b_hi = smem_base + c * 2 * R_B_PLANE, b_lo = b_hi + R_B_PLANE;
+            const uint32_t a_hi = smem_base + R_MAX_CHUNKS * 2 * R_B_PLANE + wg * 64 * 128, a_lo = a_hi + R_A_BYTES;
+            const uint32_t b_hi = smem_base + c * 2 * R_B_PLANE, b_lo = b_hi + R_B_PLANE;
+            wgmma_fence();
+            acc_fence(acc);
 #pragma unroll
-              for (int ks = 0; ks < R_BK / 8; ++ks) {
-                const uint32_t ko = ks * 32;
-                const uint64_t dAh = make_desc_sw128(a_hi + ko), dAl = make_desc_sw128(a_lo + ko);
-                const uint64_t dBh = make_desc_sw128(b_hi + ko), dBl = make_desc_sw128(b_lo + ko);
-                umma_tf32(tmem_base, dAh, dBh, idesc, (c | ks) != 0);
-                umma_tf32(tmem_base, dAl, dBh, idesc, 1);
-                umma_tf32(tmem_base, dAh, dBl, idesc, 1);
-              }
-              umma_commit(bar0);
-              if (c == n_chunks - 1) umma_commit(bar0 + 8);
+            for (int ks = 0; ks < R_BK / 8; ++ks) {
+              const uint32_t ko = ks * 32;
+              const uint64_t dAh = make_desc_sw128(a_hi + ko), dAl = make_desc_sw128(a_lo + ko);
+              const uint64_t dBh = make_desc_sw128(b_hi + ko), dBl = make_desc_sw128(b_lo + ko);
+              wgmma_tf32_n96(acc, dAh, dBh, (c | ks) != 0);
+              wgmma_tf32_n96(acc, dAl, dBh, 1);
+              wgmma_tf32_n96(acc, dAh, dBl, 1);
             }
+            wgmma_commit();
           }
         }
+        wgmma_wait<0>();
+        acc_fence(acc);
+        __syncthreads();                                       // sA is free: it holds the epilogue tile below
       }
-      if (t > 0) {
-        mbar_wait(bar0 + 8, mma_phase);
-        mma_phase ^= 1;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      // ---- (3) epilogue.  TMEM hands every thread one ROW (sequence) of the accumulator, but all global operands are
+      // ---- (3) epilogue.  The accumulator fragments are spread over the warpgroup's threads, but all global operands are
       //      row-major: the tile goes through shared memory (the free A buffer, two halves of 64 rows) and is then
       //      processed one row per warp with lane = hidden unit, so every global access is a coalesced 128-byte segment
-      //      (an SM only sustains ~50 GB/s from L2: the strided version moved 2.4x the bytes and cost 19 us per step).
+      //      (the strided version moved 2.4x the bytes).
       constexpr int TS = RN + 4;                           // padded row stride: conflict-free 16-byte stores
       float* sT = reinterpret_cast<float*>(sA);            // [64 rows][100] floats = 25.6 KB
 #pragma unroll 1
       for (int half_rows = 0; half_rows < 2; ++half_rows) {
-        if (t > 0) {
-          if ((erow >> 6) == half_rows) {
-#pragma unroll
-            for (int g = 0; g < 3; ++g) {
-              uint32_t v[16];
-              const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(g * RU + eu0);
-              asm volatile(
-                  "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                  : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                    "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                  : "r"(taddr));
-              asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-              float* dst = sT + (erow & 63) * TS + g * RU + eu0;
-#pragma unroll
-              for (int i = 0; i < 16; i += 4)
-                *reinterpret_cast<float4*>(dst + i) = make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]),
-                                                                  __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-            }
-          }
-        }
+        if (t > 0 && wg == half_rows) acc_store(acc, sT, TS, tid & 127);   // warpgroup g holds rows [64 g, 64 g + 64)
         __syncthreads();
         const int u = u0 + lane;
         float* hn = enc == 0 ? hn4 : hn3;
@@ -266,16 +228,8 @@ gru_recur_kernel(const float* __restrict__ GI, const float* __restrict__ PQ, con
         }
         __syncthreads();
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncthreads();      // the accumulator is re-used by the next tile / step
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     }
     if (t + 1 < max_len && counts.n[t + 1] > 0) grid_barrier(barrier_counter, (unsigned int)(t + 1) * n_ctas);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(128) : "memory");
   }
 }
 

@@ -20,7 +20,7 @@ namespace renet {
 namespace {
 
 // Tile kernel (round 1; rgcn_tile.cuh): one CTA per 16 destinations.  The path for small graphs (inference on a handful of
-// sub-graphs, the read-out sub-graph of layer 2: a persistent 148-CTA launch would cost more than the work) and for DGL's
+// sub-graphs, the read-out sub-graph of layer 2: a persistent one-CTA-per-SM launch would cost more than the work) and for DGL's
 // edge-less pass-through; at batch scale the persistent kernel of rgcn_stream.cuh takes over (gather_use_stream).
 template <bool RELU, bool HAS_LOOP, bool INDEXED, int NODES = kTileNodes>
 __global__ void __launch_bounds__(kTileWarps * 32, 768 / (kTileWarps * 32))
@@ -115,11 +115,11 @@ int gather_kernel_choice() {
 }
 bool gather_use_stream(int64_t E, int64_t N) {
   // E may be an upper bound (device-assembled batches and read-out sub-graphs pass their capacity), so the destination
-  // count decides with it: the persistent kernel pays ~5 us of prologue per launch, which a few thousand destinations'
-  // worth of edges does not amortise (read-out sub-graph of an ICEWS18 batch: tile kernel 26 us, stream kernel 43 us).
-  // And it is built for feature matrices that live in L2 (ICEWS18 27 MB: 41 vs 50 us; GDELT 83 vs 119 us): with two rows
-  // in flight per warp it cannot cover HBM latency, so when the features exceed L2 (synthetic 1 M-entity shard, 800 MB:
-  // tile kernel 4.65 ms = 0.90 of the HBM roofline, stream kernel 17 ms) the tile kernel stays
+  // count decides with it: the persistent kernel pays a prologue of several microseconds per launch, which a few thousand
+  // destinations' worth of edges (the read-out sub-graph of an ICEWS18 batch) does not amortise.  And it is built for
+  // feature matrices that live in L2 (ICEWS18: 27 MB of the H100's 50 MB): with two rows in flight per warp it cannot cover
+  // HBM latency, so when the features exceed L2 (kStreamMaxNodes; the synthetic 1 M-entity shard, 800 MB) the tile kernel
+  // stays
   const int c = gather_kernel_choice();
   return c == 3 || (c == 0 && E >= kStreamMinEdges && N >= kStreamMinNodes && N <= kStreamMaxNodes);
 }
@@ -147,10 +147,9 @@ static int launch_stream_cfg(const float* H, const int32_t* h_index, const float
                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_done = true;
   }
-  // (Launching this grid with programmatic stream serialisation behind the self-loop GEMM was measured: +3.5 % on the
-  // ICEWS18 step, but with a CUDA event recorded between the two kernels the GDELT-shaped launch took 11 ms instead of
-  // 83 us -- an interaction that could not be pinned down within the round.  Plain stream order it is; the kernel's
-  // griddepcontrol.wait is a no-op then.)
+  // (Programmatic stream serialisation behind the self-loop GEMM is not used: with a CUDA event recorded between the two
+  // kernels it once made a GDELT-shaped launch orders of magnitude slower, an interaction that was never pinned down.
+  // Plain stream order it is; the kernel's griddepcontrol.wait is a no-op then.)
   long long* dbg = g_stream_dbg;
   rgcn_gather_stream_kernel<RELU, HAS_LOOP, INDEXED, false, Cfg><<<kNumSMs, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(
       H, h_index, W, row_ptr, col_src, col_type, norm, Hout, N, R2, hot_rel, n_hot, E_hint, dbg);

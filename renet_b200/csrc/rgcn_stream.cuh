@@ -1,12 +1,11 @@
 // Persistent bulk-copy ("stream") gather for the RE-Net shape (d_in = d_out = 200, 100 blocks of 2x2): the kernel behind
 // renet_rgcn_gather at batch scale (reference RGCN.py:79-94 + 42-48; DGL fn.sum, RGCN.py:91).
 //
-// Why: the tile kernel (rgcn_tile.cuh) spends ~108 warp instructions per edge at 34 % warp occupancy, re-fetches the
-// 1600-byte relation row of most edges through L2 (35 % L1 hit rate), and every 16-destination tile pays its own
-// dependent index chain and two CTA barriers: 49.5 us = 65 % of the roofline (profiles/r02_gather_ncu.txt).  Every variant
-// that brings source rows in with per-lane LDGs -- including a persistent one with 114 relation rows resident in shared
-// memory and two rows prefetched in registers -- stops at the same 49.5 us: the L1TEX request path (4 LDG.64 per edge, 7-8
-// sectors each) is the wall, not L2, HBM or the issue slots (DESIGN.md section 5).  So the loads leave the LSU path:
+// Why: the tile kernel (rgcn_tile.cuh) spends about a hundred warp instructions per edge at low warp occupancy, re-fetches
+// the 1600-byte relation row of most edges through L2, and every 16-destination tile pays its own dependent index chain and
+// two CTA barriers.  Variants that bring source rows in with per-lane LDGs -- including a persistent one with 114 relation
+// rows resident in shared memory and two rows prefetched in registers -- stop at the L1TEX request path (4 LDG.64 per
+// edge, 7-8 sectors each), not at L2, HBM or the issue slots.  So the loads leave the LSU path:
 //   * ONE persistent CTA per SM (32 warps).  CTA c owns the destinations [A_c, A_c+1) whose edge range is 1/gridDim of the
 //     graph (node-aligned to the nearer destination start: rounds of a 256-way search in row_ptr, two at ICEWS18 scale),
 //     and its warps split that EDGE range evenly at arbitrary cuts;
@@ -18,8 +17,8 @@
 //     edge i (4 x LDS.64 + 4 x LDS.128 per lane, conflict-free) while the copies of the next D edges are in flight.
 //     No register holds a load in flight; the edge indices of a block of edges are staged once in shared memory, so
 //     the per-edge code has no shuffles; the ring keeps streaming across destinations (no per-tile prologue).
-//     What bounds it now is the shared-memory pipe (ring write + ring read + relation row read: ~37 cycles per edge
-//     per SM measured, tools/stream_timeline.py), which is why more warps (32, two slots each) beat deeper rings;
+//     What bounds it then is the shared-memory pipe (ring write + ring read + relation row read per edge;
+//     tools/stream_timeline.py times it), which is why more warps (32, two slots each) beat deeper rings;
 //   * the running destination's sum stays in registers (edges are destination-sorted: a segmented reduction); a
 //     destination that starts and ends inside the warp's range goes straight from registers through the fused
 //     norm / self-loop / activation epilogue to global memory; one cut by a warp boundary is handed over through a
@@ -168,8 +167,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   const bool use_hot = R2 > 0 && R2 <= kStMaxR2 && Cfg::kHot > 0;
   const bool given_hot = use_hot && hot_rel != nullptr;
   // The prologue is a chain of dependent reads (edge count -> two search rounds -> row_ptr slice -> edge indices -> row
-  // indirection -> first rows); when the graph arrays are cold in HBM every link costs a DRAM latency (~1.4 us: 7 us in
-  // all, measured).  So first thing, the grid pulls the index arrays into L2, one 128-byte line per thread: the chain then
+  // indirection -> first rows); when the graph arrays are cold in HBM every link costs a DRAM latency.  So first thing, the grid pulls the index arrays into L2, one 128-byte line per thread: the chain then
   // pays one DRAM latency (the edge count) and L2 latencies after that.  E_hint >= E is the caller's edge count / capacity.
   {
     const int64_t gt = (int64_t)blockIdx.x * Cfg::kThreads + threadIdx.x;

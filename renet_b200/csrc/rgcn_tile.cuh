@@ -182,7 +182,7 @@ __device__ __forceinline__ void tile_accumulate(float (*agg)[200], const int* s_
       const int sb = __shfl_sync(0xffffffffu, my_s, jb), tb = __shfl_sync(0xffffffffu, my_t, jb);
       const float ca = EDGE_SCALE ? __shfl_sync(0xffffffffu, my_sc, j) : 1.f;
       const float cb = EDGE_SCALE ? __shfl_sync(0xffffffffu, my_sc, jb) : 1.f;
-      // (letting lanes 25..31 shadow lanes 0..6 to drop the predication was measured: 54.4 vs 52 us, slower)
+      // (letting lanes 25..31 shadow lanes 0..6 to drop the predication was measured slower)
       EdgeData da, db;
       if (active) {             // both edges' 16 loads are issued before any use
         load_edge<STREAM_X>(da, X, W, sa, ta, lane);

@@ -1,6 +1,6 @@
 // fp32 FFMA GEMMs used by the self-loop (RGCN.py:35) and the GRU projections (model.py:86,94).
 // fp32 parity (1e-4 vs the CPU oracle) rules out single-pass TF32; these are plain FFMA kernels
-// with register tiling.  The 3xTF32 tcgen05 path lives in umma_gemm.cu.
+// with register tiling.  The 3xTF32 wgmma path lives in umma_gemm.cu.
 //
 // Tile: 80 x 200 outputs per CTA (d_out = 200, 600 and 1200 are all multiples of 200, so no column
 // waste), 8x8 outputs per thread, K stepped by 8 with register-staged double buffering.
@@ -239,7 +239,7 @@ int umma_gemm_nn_try(const float* A, const int32_t* a_index, int64_t lda, const 
                      int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
                      cudaStream_t stream);
 
-// RENET_GEMM=ffma|umma selects the dense-GEMM engine (both are this library's own sm_100a kernels).
+// RENET_GEMM=ffma|umma selects the dense-GEMM engine (both are this library's own sm_90a kernels).
 static int g_gemm_mode = -1;
 int gemm_mode() {
   if (g_gemm_mode < 0) {
@@ -258,7 +258,7 @@ int sgemm_nn(const float* A, const int32_t* a_index, int64_t lda, const float* B
              int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
              cudaStream_t stream) {
   if (M <= 0 || N <= 0) return RENET_OK;
-  if (gemm_mode() == 1) {   // tcgen05 3xTF32 path (umma_gemm.cu); returns 0 when the shape is not supported
+  if (gemm_mode() == 1) {   // wgmma 3xTF32 path (umma_gemm.cu); returns 0 when the shape is not supported
     const int r = umma_gemm_nn_try(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
     if (r != 0) return r < 0 ? r : RENET_OK;
   }

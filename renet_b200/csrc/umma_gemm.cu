@@ -1,24 +1,23 @@
-// fp32-accurate GEMM on the 5th-generation tensor cores: C[M,N] = A[M,K] @ B[K,N] (+bias) (+C)
+// fp32-accurate GEMM on the Hopper tensor cores (wgmma): C[M,N] = A[M,K] @ B[K,N] (+bias) (+C)
 //
 // RE-Net's dense work on the hot path -- the self-loop H @ W_loop (RGCN.py:35) and the GRU input /
 // recurrent projections (model.py:86,94) -- must match a CPU fp32 oracle to 1e-4, which single-pass
-// TF32 (10-bit mantissa, ~3e-4 on K=200) does not.  This kernel issues tcgen05.mma kind::tf32 with the
+// TF32 (10-bit mantissa, ~3e-4 on K=200) does not.  This kernel issues wgmma .tf32 with the
 // 3xTF32 split:  a = a_hi + a_lo,  b = b_hi + b_lo  (hi = top 19 bits, lo = a - a_hi exactly),
-//     D += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo        (fp32 accumulation in TMEM)
+//     D += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo        (fp32 accumulation in registers)
 // which recovers ~fp32 accuracy (dropped term a_lo*b_lo ~ 2^-22 relative) at 1/3 of TF32 peak -- still
 // several times the FFMA roofline.
 //
-// Structure (one CTA per 128-row tile of A x one <=200-column tile of B, 256 threads):
+// Structure (one CTA per 128-row tile of A x one <=200-column tile of B, 256 threads = two warpgroups):
 //   * operands are staged by the threads themselves (not TMA): A rows may be gathered through an index
 //     (fused embedding lookup / read-out), B is row-major [K,N] and has to be transposed to K-major,
 //     and both need the hi/lo split, so a register pass is required anyway;
 //   * smem holds two stages of {A_hi, A_lo [128 x 40], B_hi, B_lo [208 x 40]} in the canonical
-//     no-swizzle K-major UMMA layout (8-row x 16-byte core matrices; LBO = one 4-column slab,
-//     SBO = 128 B);
-//   * one elected thread issues 15 MMAs (5 k-steps x 3 split products, M=128, N=208, K=8) per stage and
-//     commits to an mbarrier that frees the stage; loads of chunk c+1 overlap the MMAs of chunk c;
-//   * accumulator: 128 lanes x 208 fp32 columns of TMEM (256 allocated); epilogue reads it with
-//     tcgen05.ld 32x32b (thread = row) and writes C with bias / accumulate applied.
+//     no-swizzle K-major layout (8-row x 16-byte core matrices; LBO = one 4-column slab, SBO = 128 B);
+//   * warpgroup g issues 15 wgmma (5 k-steps x 3 split products, M=64 rows [64g, 64g+64), N=208, K=8) per stage;
+//     the staging of chunk c+1 overlaps the MMAs of chunk c (at most one wgmma group in flight);
+//   * accumulator: 104 fp32 registers per thread; the epilogue goes through shared memory (thread = row) and
+//     writes C with bias / accumulate applied.
 #include "common.cuh"
 #include <mutex>
 #include <vector>
@@ -40,10 +39,9 @@ constexpr int A_BYTES = USLABS * A_SLAB_BYTES;   // 20480
 constexpr int B_BYTES = USLABS * B_SLAB_BYTES;   // 33280
 constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;   // 107520
 constexpr int NUM_STAGES = 2;
-constexpr int SMEM_BYTES = NUM_STAGES * STAGE_BYTES + 64;   // + mbarriers / tmem pointer
-constexpr int TMEM_COLS = 256;
-
-__device__ __forceinline__ uint32_t make_idesc() { return make_idesc_n(UNP); }
+constexpr int SMEM_BYTES = NUM_STAGES * STAGE_BYTES;
+constexpr int CLD = UNP + 4;     // row stride (floats) of the accumulator tile in shared memory: conflict-free float4 rows
+static_assert(UM * CLD * 4 <= SMEM_BYTES, "accumulator tile reuses the operand stages");
 
 template <bool INDEXED>
 __global__ void __launch_bounds__(UTHREADS, 1)
@@ -51,29 +49,12 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
                     const float* __restrict__ B, int64_t ldb, float* __restrict__ C, int64_t ldc,
                     const float* __restrict__ bias, int64_t M, int N, int K, int accumulate) {
   extern __shared__ __align__(128) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const int64_t row0 = (int64_t)blockIdx.x * UM;
   const int n0 = blockIdx.y * UN;
   const int tile_n = min(UN, N - n0);
-
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NUM_STAGES * STAGE_BYTES);   // [0..1] stage free, [2] done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + NUM_STAGES * STAGE_BYTES + 32);
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t bar0 = smem_u32(bars);
 
-  if (tid == 0) {
-    mbar_init(bar0, 1);
-    mbar_init(bar0 + 8, 1);
-    mbar_init(bar0 + 16, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   // zero the 8 padding rows (n = 200..207) of every B slab once; they are never written again
   for (int i = tid; i < NUM_STAGES * 2 * USLABS * (UNP - UN); i += UTHREADS) {
     const int r = i % (UNP - UN), sl = (i / (UNP - UN)) % USLABS, which = (i / ((UNP - UN) * USLABS)) % 2,
@@ -82,11 +63,6 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
                                           (UN + r) * 16);
     *p = make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t idesc = make_idesc();
 
   // per-thread A source rows: task = slab * 128 + row  (5 tasks per thread per chunk)
   const float* a_rows[5];
@@ -102,14 +78,16 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
     }
   }
 
+  float acc[UNP / 2];
+#pragma unroll
+  for (int i = 0; i < UNP / 2; ++i) acc[i] = 0.f;
   const int nchunks = K / UKC;
   for (int c = 0; c < nchunks; ++c) {
-    const int st = c % NUM_STAGES;
+    const int st = c % NUM_STAGES;                       // its MMAs of chunk c-2 are complete (barrier below)
     uint8_t* sA_hi = smem + st * STAGE_BYTES;
     uint8_t* sA_lo = sA_hi + A_BYTES;
     uint8_t* sB_hi = sA_lo + A_BYTES;
     uint8_t* sB_lo = sB_hi + B_BYTES;
-    if (c >= NUM_STAGES) mbar_wait(bar0 + 8 * st, ((c / NUM_STAGES) - 1) & 1);   // MMAs of chunk c-2 done
     const int k0 = c * UKC;
     // ---- A: 128 rows x 10 slabs; thread -> (slab, row): conflict-free 16-byte smem stores ----------
 #pragma unroll
@@ -145,46 +123,46 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
         *reinterpret_cast<float4*>(sB_lo + sl * B_SLAB_BYTES + (4 * j + q) * 16) = lo;
       }
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (MMA)
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a_hi = smem_base + st * STAGE_BYTES, a_lo = a_hi + A_BYTES;
-      const uint32_t b_hi = a_lo + A_BYTES, b_lo = b_hi + B_BYTES;
+    {
+      const uint32_t a_hi = smem_base + st * STAGE_BYTES + wg * 64 * 16, a_lo = a_hi + A_BYTES;   // this warpgroup's 64 rows
+      const uint32_t b_hi = smem_base + st * STAGE_BYTES + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
+      wgmma_fence();
+      acc_fence(acc);
 #pragma unroll
       for (int ks = 0; ks < UKC / 8; ++ks) {
         const uint32_t ao = ks * 2 * A_SLAB_BYTES, bo = ks * 2 * B_SLAB_BYTES;
         const uint64_t dAh = make_desc(a_hi + ao, A_SLAB_BYTES, 128), dAl = make_desc(a_lo + ao, A_SLAB_BYTES, 128);
         const uint64_t dBh = make_desc(b_hi + bo, B_SLAB_BYTES, 128), dBl = make_desc(b_lo + bo, B_SLAB_BYTES, 128);
-        umma_tf32(tmem_base, dAh, dBh, idesc, (c | ks) != 0);
-        umma_tf32(tmem_base, dAl, dBh, idesc, 1);
-        umma_tf32(tmem_base, dAh, dBl, idesc, 1);
+        wgmma_tf32_n208(acc, dAh, dBh, (c | ks) != 0);
+        wgmma_tf32_n208(acc, dAl, dBh, 1);
+        wgmma_tf32_n208(acc, dAh, dBl, 1);
       }
-      umma_commit(bar0 + 8 * st);                         // frees this stage when the MMAs have read it
-      if (c == nchunks - 1) umma_commit(bar0 + 16);       // accumulator complete
+      wgmma_commit();
     }
+    wgmma_wait<1>();             // this warpgroup's MMAs of chunk c-1 are complete
+    acc_fence(acc);
+    __syncthreads();             // ... and the other warpgroup's: stage (c+1) % 2 may be overwritten
   }
+  wgmma_wait<0>();
+  acc_fence(acc);
+  __syncthreads();               // every MMA has read its operands: the stages hold the accumulator tile now
 
-  // ---- epilogue: TMEM -> registers -> global (thread = row; warps 0-3 cols [0,104), warps 4-7 [104,208)) ---
-  mbar_wait(bar0 + 16, 0);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  // ---- epilogue: registers -> shared tile -> global (thread = row; warps 0-3 cols [0,104), warps 4-7 [104,208)) ---
+  float* sC = reinterpret_cast<float*>(smem);
+  acc_store(acc, sC + wg * 64 * CLD, CLD, tid & 127);
+  __syncthreads();
   {
     const int q = warp & 3, half = warp >> 2;
     const int r = q * 32 + lane;
     const int64_t gr = row0 + r;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
 #pragma unroll 1
     for (int cc = half * 104; cc < half * 104 + 104; cc += 8) {
-      uint32_t v[8];
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                   : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                   : "r"(taddr + (uint32_t)cc));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
       if (gr < M && cc < tile_n) {
-        float o[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) o[i] = __uint_as_float(v[i]);
+        const float4 a0 = *reinterpret_cast<const float4*>(sC + r * CLD + cc);
+        const float4 a1 = *reinterpret_cast<const float4*>(sC + r * CLD + cc + 4);
+        float o[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
         float* cp = C + gr * ldc + n0 + cc;
         if (bias != nullptr) {
           const float4 b0 = ldg_f4(bias + n0 + cc), b1 = ldg_f4(bias + n0 + cc + 4);
@@ -201,11 +179,6 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
 }
 
 
@@ -214,19 +187,21 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
 //
 // Profiling v1 showed the tile time dominated by operand staging, not by the MMAs: every CTA re-transposed and
 // re-split the same B (W_loop / GRU weights), and the no-swizzle layout forced row-strided A loads (16 useful
-// bytes per 128-byte line with almost no L1 left beside 215 KB of shared memory).  v2:
+// bytes per 128-byte line).  v2:
 //   * B is packed ONCE per GEMM by umma_pack_b_kernel into the exact shared-memory image (hi and lo planes,
 //     K-major, SWIZZLE_128B, one 53 KB block per (column tile, 32-wide K chunk)); the GEMM CTAs fetch a block
 //     with a single cp.async.bulk (TMA) that completes on the stage's mbarrier;
 //   * A is staged by the threads with fully coalesced 128-byte row segments and conflict-free swizzled
 //     16-byte stores (chunk j of row r lands at chunk j ^ (r % 8));
-//   * K is processed in chunks of 32 (one swizzle atom): 4 MMA k-steps x 3 split products per chunk.
+//   * K is processed in chunks of 32 (one swizzle atom): 4 wgmma k-steps x 3 split products per chunk and warpgroup;
+//   * A and B are double-buffered: chunk c+1's bulk copy and A staging run while chunk c's MMAs do.
 // ======================================================================================================
 constexpr int P_BK = 32;
 constexpr int P_A_BYTES = UM * 128;                  // 16384
 constexpr int P_B_BYTES = UNP * 128;                 // 26624
 constexpr int P_B_CHUNK = 2 * P_B_BYTES;             // hi + lo planes of one (tile, chunk)
-constexpr int P_SMEM = 4 * P_A_BYTES + 2 * P_B_CHUNK + 1024 + 128;   // two tiles' A (hi,lo) + two B stages
+constexpr int P_SMEM = 4 * P_A_BYTES + 2 * P_B_CHUNK + 1024 + 128;   // two stages of A (hi,lo) and of B, barriers
+static_assert(UM * CLD * 4 <= 4 * P_A_BYTES + 2 * P_B_CHUNK, "accumulator tile reuses the operand stages");
 
 // Bp[(nt * n_chunks + kc)] = {hi plane, lo plane} of B[kc*32 .. +31][nt*200 .. +207] (zero padded)
 __global__ void __launch_bounds__(256)
@@ -259,10 +234,6 @@ umma_pack_b_kernel(const float* __restrict__ B, int64_t sk, int64_t sn, int N, i
 //          [M, N] logits never reach memory; ce_reduce_kernel turns the partials into logsumexp and the loss
 //   EPI 2  dlogits[row, col] = (exp(logit - lse[row]) - [col == target[row]]) * scale, written to memory for the two
 //          gradient GEMMs (the backward pass recomputes the logits instead of keeping them)
-
-// One CTA = a PAIR of 128-row tiles sharing every B block: the packed B chunk (53 KB) is fetched once per pair,
-// the two tiles' A buffers ping-pong (tile 1's chunk is staged while tile 0's MMAs run and vice versa), and the
-// two accumulators live side by side in TMEM (2 x 256 columns).
 template <bool INDEXED, int EPI = 0>
 __global__ void __launch_bounds__(UTHREADS, 1)
 umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_index, int64_t lda,
@@ -272,7 +243,7 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024 - (raw & 1023)) & 1023);     // swizzle atoms need 1024-byte alignment
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   // grid.z = batch x K-split.  Batched GEMMs (the two GRU encoders): per-batch operand offsets.  Split-K (long-K,
   // few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
   // partial product to C + s*split_c; the caller sums the partials.
@@ -284,36 +255,26 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
   const int cps = (n_chunks + k_splits - 1) / k_splits;
   const int c_begin = split * cps;
   const int n_local = min(cps, n_chunks - c_begin);      // >= 1: the launcher never creates an empty split
-  const int64_t row_base = (int64_t)blockIdx.x * (2 * UM);
+  const int64_t row_base = (int64_t)blockIdx.x * UM;
   const int nt = blockIdx.y;
   const int n0 = nt * UN;
   const int tile_n = min(UN, N - n0);
-  // smem: A[2 tiles][hi,lo] (4 x 16 KB), B[2 stages][hi,lo] (2 x 53 KB), barriers
+  // smem: A[2 stages][hi,lo] (4 x 16 KB), B[2 stages][hi,lo] (2 x 53 KB), barriers
   uint8_t* sA = smem;
   uint8_t* sB = smem + 4 * P_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + 2 * P_B_CHUNK);   // [0,1] B landed, [2,3] B free, [4,5] A_t free, [6] done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + 2 * P_B_CHUNK);   // [0,1] B stage landed
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar0 = smem_u32(bars);
   if (tid == 0) {
-    for (int i = 0; i < 7; ++i) mbar_init(bar0 + 8 * i, 1);
+    mbar_init(bar0, 1);
+    mbar_init(bar0 + 8, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncwarp();
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t idesc = make_idesc();
 
-  // A tasks per tile: 128 rows x 8 sixteen-byte chunks = 1024 -> 4 per thread; 8 consecutive lanes read one
+  // A tasks: 128 rows x 8 sixteen-byte chunks = 1024 -> 4 per thread; 8 consecutive lanes read one
   // 128-byte row segment (coalesced), and write it to 8 distinct swizzled chunks (conflict-free)
-  const float* a_rows[2][4];
+  const float* a_rows[4];
   uint32_t a_off[4];
   int a_k[4];
 #pragma unroll
@@ -322,187 +283,156 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     const int r = task >> 3, j = task & 7;
     a_off[t] = sw128_offset(r, j);
     a_k[t] = 4 * j;
-#pragma unroll
-    for (int tl = 0; tl < 2; ++tl) {
-      const int64_t gr = row_base + tl * UM + r;
-      a_rows[tl][t] = nullptr;
-      if (gr < M) {
-        const int64_t rr = INDEXED ? (int64_t)__ldg(a_index + gr) : gr;
-        a_rows[tl][t] = A + rr * lda;
-      }
+    const int64_t gr = row_base + r;
+    a_rows[t] = nullptr;
+    if (gr < M) {
+      const int64_t rr = INDEXED ? (int64_t)__ldg(a_index + gr) : gr;
+      a_rows[t] = A + rr * lda;
     }
   }
   const uint8_t* bp_tile = Bp + (size_t)nt * n_chunks * P_B_CHUNK;
   float4 vnext[4];
-  auto load_a = [&](int tl, int c) {
+  auto load_a = [&](int c) {
     const int k0 = (c_begin + c) * P_BK;
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
       vnext[t] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (a_rows[tl][t] != nullptr && k0 + a_k[t] < K) vnext[t] = ldg_f4(a_rows[tl][t] + k0 + a_k[t]);
+      if (a_rows[t] != nullptr && k0 + a_k[t] < K) vnext[t] = ldg_f4(a_rows[t] + k0 + a_k[t]);
     }
   };
-  load_a(0, 0);
-  for (int c = 0; c < n_local; ++c) {
-    const int bs = c & 1;
-    if (tid == 0) {   // TMA: one bulk copy per chunk brings the packed B block for BOTH tiles
-      if (c >= 2) mbar_wait(bar0 + 16 + 8 * bs, ((c >> 1) - 1) & 1);          // both tiles' MMAs of chunk c-2 done
-      const uint32_t full = bar0 + 8 * bs;
-      const uint32_t dstB = smem_base + 4 * P_A_BYTES + bs * P_B_CHUNK;
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "r"((uint32_t)P_B_CHUNK) : "memory");
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dstB),
-                   "l"(bp_tile + (size_t)(c_begin + c) * P_B_CHUNK), "r"((uint32_t)P_B_CHUNK), "r"(full)
-                   : "memory");
+  auto store_a = [&](int s) {
+    uint8_t* sA_hi = sA + s * 2 * P_A_BYTES;
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      float4 hi, lo;
+      split4(vnext[t], hi, lo);
+      *reinterpret_cast<float4*>(sA_hi + a_off[t]) = hi;
+      *reinterpret_cast<float4*>(sA_hi + P_A_BYTES + a_off[t]) = lo;
     }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
+  };
+  auto issue_b = [&](int c) {   // TMA: one bulk copy brings the packed B block of chunk c
+    const uint32_t full = bar0 + 8 * (c & 1);
+    const uint32_t dstB = smem_base + 4 * P_A_BYTES + (c & 1) * P_B_CHUNK;
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "r"((uint32_t)P_B_CHUNK) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dstB),
+                 "l"(bp_tile + (size_t)(c_begin + c) * P_B_CHUNK), "r"((uint32_t)P_B_CHUNK), "r"(full)
+                 : "memory");
+  };
+
+  if (tid == 0) issue_b(0);
+  load_a(0);
+  store_a(0);
+  __syncthreads();
+  float acc[UNP / 2];
 #pragma unroll
-    for (int tl = 0; tl < 2; ++tl) {
-      uint8_t* sA_hi = sA + tl * 2 * P_A_BYTES;
-      uint8_t* sA_lo = sA_hi + P_A_BYTES;
-      if (c >= 1) mbar_wait(bar0 + 32 + 8 * tl, (c - 1) & 1);                 // MMAs of (tile tl, chunk c-1) have read A_tl
-      float4 v[4];
+  for (int i = 0; i < UNP / 2; ++i) acc[i] = 0.f;
+  for (int c = 0; c < n_local; ++c) {
+    const int s = c & 1;
+    if (c + 1 < n_local) load_a(c + 1);                 // the next chunk's global loads fly during this chunk's MMAs
+    mbar_wait(bar0 + 8 * s, (c >> 1) & 1);              // B block landed
+    {
+      const uint32_t a_hi = smem_base + s * 2 * P_A_BYTES + wg * 64 * 128, a_lo = a_hi + P_A_BYTES;   // warpgroup's 64 rows
+      const uint32_t b_hi = smem_base + 4 * P_A_BYTES + s * P_B_CHUNK, b_lo = b_hi + P_B_BYTES;
+      wgmma_fence();
+      acc_fence(acc);
 #pragma unroll
-      for (int t = 0; t < 4; ++t) v[t] = vnext[t];
-      if (tl == 0) load_a(1, c);                                              // next step's global loads fly during this step
-      else if (c + 1 < n_local) load_a(0, c + 1);
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        float4 hi, lo;
-        split4(v[t], hi, lo);
-        *reinterpret_cast<float4*>(sA_hi + a_off[t]) = hi;
-        *reinterpret_cast<float4*>(sA_lo + a_off[t]) = lo;
+      for (int ks = 0; ks < P_BK / 8; ++ks) {
+        const uint32_t ko = ks * 32;                       // 8 fp32 = 32 bytes along the swizzled row
+        const uint64_t dAh = make_desc_sw128(a_hi + ko), dAl = make_desc_sw128(a_lo + ko);
+        const uint64_t dBh = make_desc_sw128(b_hi + ko), dBl = make_desc_sw128(b_lo + ko);
+        wgmma_tf32_n208(acc, dAh, dBh, (c | ks) != 0);
+        wgmma_tf32_n208(acc, dAl, dBh, 1);
+        wgmma_tf32_n208(acc, dAh, dBl, 1);
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+      wgmma_commit();
+    }
+    wgmma_wait<1>();                                     // this warpgroup's MMAs of chunk c-1 are complete
+    acc_fence(acc);
+    __syncthreads();                                     // ... and the other's: stage s^1 (A and B) is free
+    if (c + 1 < n_local) {
+      if (tid == 0) issue_b(c + 1);
+      store_a(s ^ 1);
       __syncthreads();
-      if (tid == 0) {
-        if (tl == 0) mbar_wait(bar0 + 8 * bs, (c >> 1) & 1);                  // B block landed
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_hi = smem_base + tl * 2 * P_A_BYTES, a_lo = a_hi + P_A_BYTES;
-        const uint32_t b_hi = smem_base + 4 * P_A_BYTES + bs * P_B_CHUNK, b_lo = b_hi + P_B_BYTES;
-        const uint32_t acc = tmem_base + tl * 256;
-#pragma unroll
-        for (int ks = 0; ks < P_BK / 8; ++ks) {
-          const uint32_t ko = ks * 32;                       // 8 fp32 = 32 bytes along the swizzled row
-          const uint64_t dAh = make_desc_sw128(a_hi + ko), dAl = make_desc_sw128(a_lo + ko);
-          const uint64_t dBh = make_desc_sw128(b_hi + ko), dBl = make_desc_sw128(b_lo + ko);
-          umma_tf32(acc, dAh, dBh, idesc, (c | ks) != 0);
-          umma_tf32(acc, dAl, dBh, idesc, 1);
-          umma_tf32(acc, dAh, dBl, idesc, 1);
-        }
-        umma_commit(bar0 + 32 + 8 * tl);                     // A_tl may be overwritten
-        if (tl == 1) {
-          umma_commit(bar0 + 16 + 8 * bs);                   // B stage may be overwritten
-          if (c == n_local - 1) umma_commit(bar0 + 48);      // both accumulators complete
-        }
-      }
     }
   }
+  wgmma_wait<0>();
+  acc_fence(acc);
+  __syncthreads();                                       // every MMA has read its operands: the stages are reused below
 
-  mbar_wait(bar0 + 48, 0);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  float* sC = reinterpret_cast<float*>(smem);
+  acc_store(acc, sC + wg * 64 * CLD, CLD, tid & 127);
+  __syncthreads();
   {
-    // thread = accumulator row; warps 0-3 take columns [0,104), warps 4-7 [104,208): 3 x (32 columns) + 1 x 8
+    // thread = accumulator row; warps 0-3 take columns [0,104), warps 4-7 [104,208), 8 at a time
     const int q = warp & 3, half = warp >> 2;
     const int r = q * 32 + lane;
     const int cbase = half * 104;
+    const int64_t gr = row_base + r;
+    const float* srow = sC + r * CLD;
+    // EPI 1 state of this thread's (row, half tile): running max / sum of exp; EPI 2: the row's logsumexp and target
+    float run_m = -3.0e38f, run_s = 0.f;
+    const int tgt = (EPI != 0 && gr < M) ? __ldg(epi.target + gr) : -1;
+    const float row_lse = (EPI == 2 && gr < M) ? __ldg(epi.lse + gr) : 0.f;
+    const float gscale = (EPI == 2) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
 #pragma unroll 1
-    for (int tl = 0; tl < 2; ++tl) {
-      const int64_t gr = row_base + tl * UM + r;
-      const uint32_t taddr = tmem_base + tl * 256 + ((uint32_t)(q * 32) << 16);
-      // EPI 1 state of this thread's (row, half tile): running max / sum of exp; EPI 2: the row's logsumexp and target
-      float run_m = -3.0e38f, run_s = 0.f;
-      const int tgt = (EPI != 0 && gr < M) ? __ldg(epi.target + gr) : -1;
-      const float row_lse = (EPI == 2 && gr < M) ? __ldg(epi.lse + gr) : 0.f;
-      const float gscale = (EPI == 2) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
-      auto emit8 = [&](const uint32_t* v8, int cc) {
-        if (gr < M && cc < tile_n) {
-          float o[8];
+    for (int cc = cbase; cc < cbase + 104; cc += 8) {
+      if (gr < M && cc < tile_n) {
+        const float4 a0 = *reinterpret_cast<const float4*>(srow + cc), a1 = *reinterpret_cast<const float4*>(srow + cc + 4);
+        float o[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+        if (EPI != 0) {
+          // fused cross-entropy epilogues: columns are guarded one by one (the class count need not be a multiple of 8)
+          const int nv = min(8, tile_n - cc);
+          float mx = -3.0e38f;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) o[i] = __uint_as_float(v8[i]);
-          if (EPI != 0) {
-            // fused cross-entropy epilogues: columns are guarded one by one (the class count need not be a multiple of 8)
-            const int nv = min(8, tile_n - cc);
-            float mx = -3.0e38f;
+          for (int i = 0; i < 8; ++i)
+            if (i < nv) {
+              if (bias != nullptr) o[i] += __ldg(bias + n0 + cc + i);
+              mx = fmaxf(mx, o[i]);
+            }
+          if (EPI == 1) {
+            const float nm = fmaxf(run_m, mx);
+            float add = 0.f;
 #pragma unroll
             for (int i = 0; i < 8; ++i)
               if (i < nv) {
-                if (bias != nullptr) o[i] += __ldg(bias + n0 + cc + i);
-                mx = fmaxf(mx, o[i]);
+                add += expf(o[i] - nm);
+                if (n0 + cc + i == tgt) epi.tlogit[gr] = o[i];
               }
-            if (EPI == 1) {
-              const float nm = fmaxf(run_m, mx);
-              float add = 0.f;
+            run_s = run_s * expf(run_m - nm) + add;
+            run_m = nm;
+          } else {
+            float* dp = C + gr * ldc + n0 + cc;
 #pragma unroll
-              for (int i = 0; i < 8; ++i)
-                if (i < nv) {
-                  add += expf(o[i] - nm);
-                  if (n0 + cc + i == tgt) epi.tlogit[gr] = o[i];
-                }
-              run_s = run_s * expf(run_m - nm) + add;
-              run_m = nm;
-            } else {
-              float* dp = C + gr * ldc + n0 + cc;
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                if (i < nv) {
-                  const float gv = (expf(o[i] - row_lse) - (n0 + cc + i == tgt ? 1.f : 0.f)) * gscale;
-                  dp[i] = gv;                                              // row-major: A of dX = dlogits @ W
-                  epi.dT[(int64_t)(n0 + cc + i) * epi.ldT + gr] = gv;      // transposed (lanes = consecutive rows: coalesced)
-                }
-            }
-            return;
+            for (int i = 0; i < 8; ++i)
+              if (i < nv) {
+                const float gv = (expf(o[i] - row_lse) - (n0 + cc + i == tgt ? 1.f : 0.f)) * gscale;
+                dp[i] = gv;                                              // row-major: A of dX = dlogits @ W
+                epi.dT[(int64_t)(n0 + cc + i) * epi.ldT + gr] = gv;      // transposed (lanes = consecutive rows: coalesced)
+              }
           }
-          float* cp = C + gr * ldc + n0 + cc;
-          if (bias != nullptr) {
-            const float4 b0 = ldg_f4(bias + n0 + cc), b1 = ldg_f4(bias + n0 + cc + 4);
-            o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w;
-            o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
-          }
-          if (accumulate) {
-            const float4 c0 = *reinterpret_cast<const float4*>(cp), c1 = *reinterpret_cast<const float4*>(cp + 4);
-            o[0] += c0.x; o[1] += c0.y; o[2] += c0.z; o[3] += c0.w;
-            o[4] += c1.x; o[5] += c1.y; o[6] += c1.z; o[7] += c1.w;
-          }
-          st_f4(cp, make_float4(o[0], o[1], o[2], o[3]));
-          st_f4(cp + 4, make_float4(o[4], o[5], o[6], o[7]));
+          continue;
         }
-      };
-#pragma unroll 1
-      for (int blk = 0; blk < 3; ++blk) {
-        uint32_t v[32];
-        const int cc = cbase + blk * 32;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr + (uint32_t)cc));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int g8 = 0; g8 < 4; ++g8) emit8(v + 8 * g8, cc + 8 * g8);
-      }
-      {
-        uint32_t v8[8];
-        const int cc = cbase + 96;
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(v8[0]), "=r"(v8[1]), "=r"(v8[2]), "=r"(v8[3]), "=r"(v8[4]), "=r"(v8[5]), "=r"(v8[6]), "=r"(v8[7])
-                     : "r"(taddr + (uint32_t)cc));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        emit8(v8, cc);
-      }
-      if (EPI == 1 && gr < M) {
-        const int64_t pi = (int64_t)(nt * 2 + half) * M + gr;
-        epi.pmax[pi] = run_m;
-        epi.psum[pi] = run_s;
+        float* cp = C + gr * ldc + n0 + cc;
+        if (bias != nullptr) {
+          const float4 b0 = ldg_f4(bias + n0 + cc), b1 = ldg_f4(bias + n0 + cc + 4);
+          o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w;
+          o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
+        }
+        if (accumulate) {
+          const float4 c0 = *reinterpret_cast<const float4*>(cp), c1 = *reinterpret_cast<const float4*>(cp + 4);
+          o[0] += c0.x; o[1] += c0.y; o[2] += c0.z; o[3] += c0.w;
+          o[4] += c1.x; o[5] += c1.y; o[6] += c1.z; o[7] += c1.w;
+        }
+        st_f4(cp, make_float4(o[0], o[1], o[2], o[3]));
+        st_f4(cp + 4, make_float4(o[4], o[5], o[6], o[7]));
       }
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
+    if (EPI == 1 && gr < M) {
+      const int64_t pi = (int64_t)(nt * 2 + half) * M + gr;
+      epi.pmax[pi] = run_m;
+      epi.psum[pi] = run_s;
+    }
   }
 }
 
@@ -515,7 +445,7 @@ static int64_t g_scratch_bytes = 0;
 void set_scratch(void* p, int64_t bytes) { g_scratch = (uint8_t*)p; g_scratch_bytes = p ? bytes : 0; }
 
 // ---- packed-weight cache (renet_set_weight_generation) ------------------------------------------------------------------
-// Packing a weight into the UMMA operand image is a kernel launch per weight per call.  Weights only change when the
+// Packing a weight into the tensor-core operand image is a kernel launch per weight per call.  Weights only change when the
 // optimiser steps, so the caller may declare a "weight generation": while it is unchanged, a packed image made for a
 // given (device, pointers, shape) key is valid and reused; a new generation invalidates every image (the buffers are
 // kept and overwritten by the next pack).  generation < 0 (the default) turns the cache off.
@@ -598,7 +528,7 @@ int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, 
   if (k_splits < 1) k_splits = 1;
   if (k_splits > n_chunks) k_splits = n_chunks;
   while (k_splits > 1 && ((n_chunks + k_splits - 1) / k_splits) * (k_splits - 1) >= n_chunks) --k_splits;   // no empty split
-  dim3 grid((unsigned)((M + 2 * UM - 1) / (2 * UM)), (unsigned)n_tiles, (unsigned)(batch * k_splits));
+  dim3 grid((unsigned)((M + UM - 1) / UM), (unsigned)n_tiles, (unsigned)(batch * k_splits));
 #define RENET_UMMA_LAUNCH(IDX, EP)                                                                                       \
   umma_gemm_packed_kernel<IDX, EP><<<grid, UTHREADS, P_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M, N, K, \
                                                                       n_chunks, accumulate, batch_a, batch_bp, batch_c, epi,  \

@@ -1,4 +1,4 @@
-"""Fused decoder: linear + cross-entropy of reference model.py:89-91 / 97-100 on the tcgen05 3xTF32 engine
+"""Fused decoder: linear + cross-entropy of reference model.py:89-91 / 97-100 on the wgmma 3xTF32 engine
 (renet_decoder_ce_fwd / _bwd): ``decoder_cross_entropy(x, weight, bias, target)`` equals
 ``F.cross_entropy(F.linear(x, weight, bias), target)`` (mean over rows) without materialising the [B, |E|] logits in
 the forward pass.  ``nn.Linear`` modules stay the parameter holders (state_dict keys ``linear.*`` / ``linear_r.*``)."""

@@ -1,5 +1,5 @@
 """The global model of RE-Net (reference global_model.py + Aggregator.RGCNAggregator_global, Aggregator.py:9-107) on the
-sm_100a kernels -- SURVEY.md section 8(f) row 4.  It produces the ``global_emb[t]`` vectors the hot path consumes
+sm_90a kernels -- SURVEY.md section 8(f) row 4.  It produces the ``global_emb[t]`` vectors the hot path consumes
 (utils.py:224-225) and is pre-trained by the reference's pretrain.py.
 
 Same class surface as the reference (constructor signatures, attribute / parameter names, so ``state_dict`` keys carry

@@ -1,4 +1,4 @@
-"""Test-time path of RE-Net on the B200 kernels (reference model.py:107-446; SURVEY.md section 8(f) row 2).
+"""Test-time path of RE-Net on the H100 kernels (reference model.py:107-446; SURVEY.md section 8(f) row 2).
 
 ``RENetInference`` is mixed into ``renet_b200.model.RENet`` and provides the reference's evaluation API --
 ``init_history``, ``pred_r_rank2``, ``predict``, ``evaluate``, ``evaluate_filter``, ``update_cache`` -- with the same

@@ -1,11 +1,11 @@
-"""RENet with the reference's class surface (reference model.py:10-104) on the sm_100a kernels.
+"""RENet with the reference's class surface (reference model.py:10-104) on the sm_90a kernels.
 
 Constructor signature, attribute and parameter names (``ent_embeds``, ``rel_embeds``, ``encoder``,
 ``encoder_r``, ``aggregator``, ``linear``, ``linear_r``, ``global_emb``, ``graph_dict`` ...) are the
 reference's, so a reference checkpoint's ``state_dict`` loads as is.  ``forward(triplets, s_hist,
 o_hist, graph_dict, subject=True) -> loss`` follows model.py:64-104: direction select, sort by
 history length, RGCN aggregate, GRU final hidden, zero rows for empty histories, the two linear
-decoders + cross-entropy (fused on the tcgen05 engine, decoder.py: SURVEY.md section 8(f) row 3).
+decoders + cross-entropy (fused on the wgmma engine, decoder.py: SURVEY.md section 8(f) row 3).
 
 The test-time autoregressive routines (model.py:107-446: ``init_history``, ``pred_r_rank2``,
 ``predict``, ``evaluate``, ``evaluate_filter``, ``update_cache``) come from ``inference.RENetInference``

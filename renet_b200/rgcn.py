@@ -1,4 +1,4 @@
-"""RGCN layers with the reference's class surface (reference RGCN.py:5-94) on the sm_100a kernels.
+"""RGCN layers with the reference's class surface (reference RGCN.py:5-94) on the sm_90a kernels.
 
 ``RGCNBlockLayer(in_feat, out_feat, num_rels, num_bases, bias=None, activation=None,
 self_loop=False, dropout=0.0)`` keeps the constructor, parameter names/shapes (``weight``

@@ -1,5 +1,5 @@
-"""-m "not gpu": librenet_b200.so builds for sm_100a, loads, and exports every symbol include/renet_b200.h
-declares (no compute calls here -- there is no GPU in the authoring container)."""
+"""-m "not gpu": librenet_b200.so builds for sm_90a, loads, and exports every symbol include/renet_b200.h
+declares (no compute calls here: these tests run without a GPU)."""
 import ctypes
 import os
 import re
@@ -49,9 +49,10 @@ def test_argument_validation_needs_no_gpu(so_path):
     assert rc == -1 and b'null pointer' in L.renet_last_error()
 
 
-def test_sass_is_sm100a(so_path):
-    out = subprocess.run(['cuobjdump', '-lelf', so_path], capture_output=True, text=True).stdout
-    assert 'sm_100a' in out, out
+def test_sass_is_sm90a(so_path):
+    from renet_b200 import build
+    out = subprocess.run([build.CUOBJDUMP, '-lelf', so_path], capture_output=True, text=True).stdout
+    assert 'sm_90a' in out, out
 
 
 def test_hot_path_never_imports_oracle():

@@ -182,7 +182,7 @@ def test_prefetched_batches_equal_direct_assembly():
 
 
 def test_packed_weight_cache_tracks_in_place_updates():
-    """The tcgen05 engine caches packed weights per (module, addresses, in-place versions): repeated encodes reuse the
+    """The tensor-core engine caches packed weights per (module, addresses, in-place versions): repeated encodes reuse the
     images, an in-place update (what an optimiser step is) re-packs, and the result equals a fresh module's."""
     import copy
     from renet_b200 import _lib

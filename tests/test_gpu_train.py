@@ -142,7 +142,7 @@ def test_nccl_two_rank_gradients_equal_accumulated_shards(tmp_path):
     depend on which samples share a batch, utils.py:149-170, so sharding changes the graphs themselves; data parallelism
     averages per-shard losses, exactly like running the reference on the shards.)"""
     if torch.cuda.device_count() < 2:
-        pytest.skip('needs 2 GPUs (gpurun --gpus 2)')
+        pytest.skip('needs 2 GPUs')
     import torch.multiprocessing as mp
     from renet_b200 import synthetic
     from renet_b200.parallel import shard_batch
@@ -250,7 +250,7 @@ def test_default_training_config_runs_on_our_kernels_only():
 
 @pytest.mark.parametrize('M,N,K', [(1024, 23033, 600), (1024, 256, 400), (37, 1001, 24), (300, 199, 8)])
 def test_fused_decoder_cross_entropy_vs_torch_fp32(M, N, K):
-    """renet_decoder_ce_fwd/_bwd (tcgen05 3xTF32 GEMM with fused logsumexp epilogue, recompute-based backward) against a
+    """renet_decoder_ce_fwd/_bwd (wgmma 3xTF32 GEMM with fused logsumexp epilogue, recompute-based backward) against a
     plain PyTorch fp64 reference of the same op (model.py:89-91,97-100): loss and all three gradients, including class
     counts that are not multiples of 8 / 200 and a last column tile of 33 classes (ICEWS18: 23033)."""
     from renet_b200.decoder import decoder_cross_entropy

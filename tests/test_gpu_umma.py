@@ -1,4 +1,4 @@
-"""-m gpu: the tcgen05 (3xTF32) GEMM engine, run in a subprocess under a timeout so that a wrong
+"""-m gpu: the wgmma (3xTF32) GEMM engine, run in a subprocess under a timeout so that a wrong
 descriptor can only fail this test (the kernel traps instead of hanging), never poison the others."""
 import os
 import subprocess

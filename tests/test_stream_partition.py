@@ -9,12 +9,12 @@ kernel whose arithmetic the -m gpu tests pin:
   * CTA ranges are node-aligned, contiguous and cover [0, N); warp ranges are contiguous and cover the CTA's edges;
   * the cost model (edges + kStNodeCost per destination) bounds the imbalance between CTAs by the heaviest destination.
 
-The constants mirror the kernel (kStNodeCost = 2, 148 CTAs, 32 warps); if the kernel's partition changes, this file changes
+The constants mirror the kernel (kStNodeCost = 2, 132 CTAs, 32 warps); if the kernel's partition changes, this file changes
 with it."""
 import numpy as np
 import pytest
 
-NODE_COST, GRID, WARPS = 2, 148, 32
+NODE_COST, GRID, WARPS = 2, 132, 32
 
 
 def cta_boundary(rp, N, E, c_idx, grid=GRID):

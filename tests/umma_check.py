@@ -1,4 +1,4 @@
-"""Run in a subprocess by tests/test_gpu_umma.py: tcgen05 3xTF32 GEMM vs fp64 and vs the FFMA kernel."""
+"""Run in a subprocess by tests/test_gpu_umma.py: wgmma 3xTF32 GEMM vs fp64 and vs the FFMA kernel."""
 import sys
 
 import numpy as np
