@@ -183,25 +183,48 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
 
 
 // ======================================================================================================
-// v2: pre-packed B + TMA bulk copies + 128-byte swizzle
+// v2: pre-packed B + TMA bulk copies + 128-byte swizzle, persistent and warp-specialised
 //
 // Profiling v1 showed the tile time dominated by operand staging, not by the MMAs: every CTA re-transposed and
 // re-split the same B (W_loop / GRU weights), and the no-swizzle layout forced row-strided A loads (16 useful
 // bytes per 128-byte line).  v2:
 //   * B is packed ONCE per GEMM by umma_pack_b_kernel into the exact shared-memory image (hi and lo planes,
-//     K-major, SWIZZLE_128B, one 53 KB block per (column tile, 32-wide K chunk)); the GEMM CTAs fetch a block
-//     with a single cp.async.bulk (TMA) that completes on the stage's mbarrier;
-//   * A is staged by the threads with fully coalesced 128-byte row segments and conflict-free swizzled
-//     16-byte stores (chunk j of row r lands at chunk j ^ (r % 8));
-//   * K is processed in chunks of 32 (one swizzle atom): 4 wgmma k-steps x 3 split products per chunk and warpgroup;
-//   * A and B are double-buffered: chunk c+1's bulk copy and A staging run while chunk c's MMAs do.
+//     K-major, SWIZZLE_128B, one 53 KB block per (column tile, 32-wide K chunk)); rows 0-103 and 104-207 of each
+//     plane are contiguous 13 KB halves (13 whole swizzle atoms), and the GEMM fetches the half it needs with two
+//     cp.async.bulk (TMA) copies that complete on the stage's mbarrier;
+//   * A is staged with fully coalesced 128-byte row segments and conflict-free swizzled 16-byte stores
+//     (chunk j of row r lands at chunk j ^ (r % 8));
+//   * K is processed in chunks of 32 (one swizzle atom); the last chunk issues only the k-steps that hold data.
+//
+// Work unit = 128 rows x one 104-column half of a 200-column tile (x one batch entry / K-split).  The grid has at most
+// one CTA per SM and CTA b walks the units [b*U/G, (b+1)*U/G), so no SM gets more than one unit above the average:
+// 34.5 k rows x 200 columns are 540 units, 4.09 per SM, at most 5 (half the work of one of the old 128 x 208 tiles
+// each; the old one-tile-per-CTA grid ran 3 waves for 2.05 waves of work).
+//
+// 384 threads.  Warpgroup 0 is the producer: per chunk it loads A (rows gathered through a_index), splits it into
+// hi/lo, stores it swizzled and issues the B copies.  Warpgroups 1 and 2 are the consumers: each owns 64 rows of the
+// unit, issues wgmma m64n104k8 (52 fp32 accumulators per thread) and runs the epilogue.  A ring of stages
+// {A hi, A lo [128 x 32], B hi, B lo [104 x 32]} with a full and an empty mbarrier per stage replaces block-wide
+// barriers; the producer runs up to a ring ahead across unit boundaries, so the next unit's operands land while the
+// consumers finish and store the current one, and the consumers keep one wgmma group in flight across chunks.
+// Each output element sees the k-steps in order and per k-step the products hi*hi, lo*hi, hi*lo, as in v1.
 // ======================================================================================================
 constexpr int P_BK = 32;
-constexpr int P_A_BYTES = UM * 128;                  // 16384
-constexpr int P_B_BYTES = UNP * 128;                 // 26624
+constexpr int P_A_BYTES = UM * 128;                  // 16384: one plane of 128 rows x 32 K
+constexpr int P_B_BYTES = UNP * 128;                 // 26624: one plane of 208 columns x 32 K
 constexpr int P_B_CHUNK = 2 * P_B_BYTES;             // hi + lo planes of one (tile, chunk)
-constexpr int P_SMEM = 4 * P_A_BYTES + 2 * P_B_CHUNK + 1024 + 128;   // two stages of A (hi,lo) and of B, barriers
-static_assert(UM * CLD * 4 <= 4 * P_A_BYTES + 2 * P_B_CHUNK, "accumulator tile reuses the operand stages");
+constexpr int P_UN = UNP / 2;                        // 104 columns per work unit
+constexpr int P_BH_BYTES = P_UN * 128;               // 13312: one half of a B plane
+constexpr int P_STAGE = 2 * P_A_BYTES + 2 * P_BH_BYTES;   // 59392: A hi, A lo, B hi half, B lo half
+constexpr int P_THREADS = 384;
+constexpr int P_CLD = P_UN + 4;                      // row stride (floats) of a consumer's staged accumulator tile
+// EPI 0 stores straight from the accumulator fragments and affords 3 stages; the cross-entropy epilogues walk each row
+// in column order through a staged 64 x 104 tile per consumer, which leaves room for 2.
+__host__ __device__ constexpr int p_stages(int epi) { return epi == 0 ? 3 : 2; }
+__host__ __device__ constexpr int p_staging_bytes(int epi) { return epi == 0 ? 0 : 2 * 64 * P_CLD * 4; }
+__host__ __device__ constexpr int p_smem(int epi) { return p_stages(epi) * P_STAGE + p_staging_bytes(epi) + 1024 + 128; }
+static_assert(p_smem(0) <= 232448 && p_smem(1) <= 232448, "one CTA's shared memory");
+static_assert(P_STAGE % 1024 == 0 && P_BH_BYTES % 1024 == 0, "swizzle atoms stay 1024-byte aligned");
 
 // Bp[(nt * n_chunks + kc)] = {hi plane, lo plane} of B[kc*32 .. +31][nt*200 .. +207] (zero padded)
 __global__ void __launch_bounds__(256)
@@ -228,208 +251,253 @@ umma_pack_b_kernel(const float* __restrict__ B, int64_t sk, int64_t sn, int N, i
   }
 }
 
+// One work unit: rows [row_base, row_base + 128), columns [n0 + 104*half, +104) of column tile nt, batch entry zb,
+// K-split `split` owning the chunks [c_begin, c_begin + n_local).  Units are numbered row tile fastest, then column
+// half, then batch x split (the order of the old grid's x, y, z).
+struct PUnit {
+  int64_t row_base;
+  int nt, half, zb, split, c_begin, n_local;
+};
+__device__ __forceinline__ PUnit p_unit(int64_t u, int64_t n_rt, int n_tiles, int n_chunks, int k_splits) {
+  PUnit w;
+  const int64_t rest = u / n_rt;
+  w.row_base = (u - rest * n_rt) * UM;
+  const int nh = (int)(rest % (2 * n_tiles)), z = (int)(rest / (2 * n_tiles));
+  w.nt = nh >> 1;
+  w.half = nh & 1;
+  w.zb = z / k_splits;
+  w.split = z - w.zb * k_splits;
+  const int cps = (n_chunks + k_splits - 1) / k_splits;
+  w.c_begin = w.split * cps;
+  w.n_local = min(cps, n_chunks - w.c_begin);      // >= 1: the launcher never creates an empty split
+  return w;
+}
+
 // Fused-epilogue modes of the packed kernel (the decoder of model.py:89-91,97-100: logits = X @ W^T + b, cross-entropy):
 //   EPI 0  C = acc (+bias) (+C)                                   -- plain GEMM
 //   EPI 1  per (row, half column tile): running max and sum of exp of the logits, and the target's logit -- the
 //          [M, N] logits never reach memory; ce_reduce_kernel turns the partials into logsumexp and the loss
 //   EPI 2  dlogits[row, col] = (exp(logit - lse[row]) - [col == target[row]]) * scale, written to memory for the two
 //          gradient GEMMs (the backward pass recomputes the logits instead of keeping them)
+// grid.x = min(units, SMs).  Batched GEMMs (the two GRU encoders) have per-batch operand offsets.  Split-K (long-K,
+// few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
+// partial product to C + s*split_c; the caller sums the partials.
 template <bool INDEXED, int EPI = 0>
-__global__ void __launch_bounds__(UTHREADS, 1)
+__global__ void __launch_bounds__(P_THREADS, 1)
 umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_index, int64_t lda,
                         const uint8_t* __restrict__ Bp, float* __restrict__ C, int64_t ldc,
                         const float* __restrict__ bias, int64_t M, int N, int K, int n_chunks, int accumulate,
-                        int64_t batch_a, int64_t batch_bp, int64_t batch_c, EpiArgs epi, int k_splits, int64_t split_c) {
+                        int64_t batch_a, int64_t batch_bp, int64_t batch_c, EpiArgs epi, int k_splits, int64_t split_c,
+                        int64_t n_units) {
+  constexpr int S = p_stages(EPI);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024 - (raw & 1023)) & 1023);     // swizzle atoms need 1024-byte alignment
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
-  // grid.z = batch x K-split.  Batched GEMMs (the two GRU encoders): per-batch operand offsets.  Split-K (long-K,
-  // few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
-  // partial product to C + s*split_c; the caller sums the partials.
-  const int zb = blockIdx.z / k_splits, split = blockIdx.z - zb * k_splits;
-  A += zb * batch_a;
-  Bp += zb * batch_bp;
-  C += zb * batch_c + (int64_t)split * split_c;
-  if (bias != nullptr) bias += zb * (int64_t)N;
-  const int cps = (n_chunks + k_splits - 1) / k_splits;
-  const int c_begin = split * cps;
-  const int n_local = min(cps, n_chunks - c_begin);      // >= 1: the launcher never creates an empty split
-  const int64_t row_base = (int64_t)blockIdx.x * UM;
-  const int nt = blockIdx.y;
-  const int n0 = nt * UN;
-  const int tile_n = min(UN, N - n0);
-  // smem: A[2 stages][hi,lo] (4 x 16 KB), B[2 stages][hi,lo] (2 x 53 KB), barriers
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + 4 * P_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + 2 * P_B_CHUNK);   // [0,1] B stage landed
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t bar0 = smem_u32(bars);
+  // smem: S stages {A hi, A lo, B hi half, B lo half}, [EPI != 0: two 64 x P_CLD staging tiles], full[S], empty[S]
+  const uint32_t full0 = smem_base + S * P_STAGE + p_staging_bytes(EPI);
+  const uint32_t empty0 = full0 + 8 * S;
+  const int tid = threadIdx.x;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warp-uniform to the compiler: the wgmma paths do not diverge
   if (tid == 0) {
-    mbar_init(bar0, 1);
-    mbar_init(bar0 + 8, 1);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full0 + 8 * s, 128);     // every producer thread arrives after its A stores; the B copies add bytes
+      mbar_init(empty0 + 8 * s, 8);      // lane 0 of each consumer warp arrives once its MMAs on the stage are done
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  const int64_t n_rt = (M + UM - 1) / UM;
+  const int n_tiles = (N + UN - 1) / UN;
+  const int64_t u_begin = (int64_t)blockIdx.x * n_units / gridDim.x, u_end = (int64_t)(blockIdx.x + 1) * n_units / gridDim.x;
 
-  // A tasks: 128 rows x 8 sixteen-byte chunks = 1024 -> 4 per thread; 8 consecutive lanes read one
-  // 128-byte row segment (coalesced), and write it to 8 distinct swizzled chunks (conflict-free)
-  const float* a_rows[4];
-  uint32_t a_off[4];
-  int a_k[4];
+  if (wg == 0) {
+    // ---- producer.  Thread t stages 16-byte piece j = t % 8 of rows t/8 + 16 i (i < 8): 8 consecutive lanes read one
+    // 128-byte row segment, and rows r and r + 16 share a swizzle phase, so row t/8 + 16 i lands at a_off + 2048 i.
+    const int j = tid & 7, r0 = tid >> 3;
+    const uint32_t a_off = sw128_offset(r0, j);
+    // load cursor: the chunk (lu, lc) whose A is loaded next; the loads of one chunk fly while the previous is stored
+    int64_t lu = u_begin;
+    int lc = 0;
+    PUnit lw{};
+    const float* a_rows[8];
+    auto set_unit = [&]() {
+      lw = p_unit(lu, n_rt, n_tiles, n_chunks, k_splits);
+      const float* Az = A + lw.zb * batch_a;
 #pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    const int task = tid + t * UTHREADS;
-    const int r = task >> 3, j = task & 7;
-    a_off[t] = sw128_offset(r, j);
-    a_k[t] = 4 * j;
-    const int64_t gr = row_base + r;
-    a_rows[t] = nullptr;
-    if (gr < M) {
-      const int64_t rr = INDEXED ? (int64_t)__ldg(a_index + gr) : gr;
-      a_rows[t] = A + rr * lda;
+      for (int i = 0; i < 8; ++i) {
+        const int64_t gr = lw.row_base + r0 + 16 * i;
+        a_rows[i] = nullptr;
+        if (gr < M) a_rows[i] = Az + (INDEXED ? (int64_t)__ldg(a_index + gr) : gr) * lda;
+      }
+    };
+    auto load = [&](float4 (&v)[8], const uint8_t*& bsrc) {
+      const int k = (lw.c_begin + lc) * P_BK + 4 * j;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (a_rows[i] != nullptr && k < K) v[i] = ldg_f4(a_rows[i] + k);
+      }
+      bsrc = Bp + lw.zb * batch_bp + ((size_t)lw.nt * n_chunks + lw.c_begin + lc) * P_B_CHUNK + lw.half * P_BH_BYTES;
+      if (++lc == lw.n_local) {
+        lc = 0;
+        if (++lu < u_end) set_unit();
+      }
+    };
+    auto commit = [&](const float4 (&v)[8], const uint8_t* bsrc, int q) {
+      const int s = q % S;
+      const uint32_t full = full0 + 8 * s, st = smem_base + s * P_STAGE;
+      mbar_wait(empty0 + 8 * s, ((q / S) & 1) ^ 1);     // the consumers are done with the stage's previous chunk
+      if (tid == 0) {
+        mbar_expect_tx(full, 2 * P_BH_BYTES);
+        bulk_copy_g2s(st + 2 * P_A_BYTES, bsrc, P_BH_BYTES, full);
+        bulk_copy_g2s(st + 2 * P_A_BYTES + P_BH_BYTES, bsrc + P_B_BYTES, P_BH_BYTES, full);
+      }
+      uint8_t* sa = smem + s * P_STAGE;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        float4 hi, lo;
+        split4(v[i], hi, lo);
+        *reinterpret_cast<float4*>(sa + a_off + 2048 * i) = hi;
+        *reinterpret_cast<float4*>(sa + P_A_BYTES + a_off + 2048 * i) = lo;
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
+      mbar_arrive(full);
+    };
+    if (lu >= u_end) return;
+    set_unit();
+    float4 va[8], vb[8];
+    const uint8_t *ba, *bb;
+    load(va, ba);
+    for (int q = 0;; q += 2) {
+      const bool more_b = lu < u_end;
+      if (more_b) load(vb, bb);
+      commit(va, ba, q);
+      if (!more_b) break;
+      const bool more_a = lu < u_end;
+      if (more_a) load(va, ba);
+      commit(vb, bb, q + 1);
+      if (!more_a) break;
     }
+    return;
   }
-  const uint8_t* bp_tile = Bp + (size_t)nt * n_chunks * P_B_CHUNK;
-  float4 vnext[4];
-  auto load_a = [&](int c) {
-    const int k0 = (c_begin + c) * P_BK;
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      vnext[t] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (a_rows[t] != nullptr && k0 + a_k[t] < K) vnext[t] = ldg_f4(a_rows[t] + k0 + a_k[t]);
-    }
-  };
-  auto store_a = [&](int s) {
-    uint8_t* sA_hi = sA + s * 2 * P_A_BYTES;
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      float4 hi, lo;
-      split4(vnext[t], hi, lo);
-      *reinterpret_cast<float4*>(sA_hi + a_off[t]) = hi;
-      *reinterpret_cast<float4*>(sA_hi + P_A_BYTES + a_off[t]) = lo;
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
-  };
-  auto issue_b = [&](int c) {   // TMA: one bulk copy brings the packed B block of chunk c
-    const uint32_t full = bar0 + 8 * (c & 1);
-    const uint32_t dstB = smem_base + 4 * P_A_BYTES + (c & 1) * P_B_CHUNK;
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "r"((uint32_t)P_B_CHUNK) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dstB),
-                 "l"(bp_tile + (size_t)(c_begin + c) * P_B_CHUNK), "r"((uint32_t)P_B_CHUNK), "r"(full)
-                 : "memory");
-  };
 
-  if (tid == 0) issue_b(0);
-  load_a(0);
-  store_a(0);
-  __syncthreads();
-  float acc[UNP / 2];
-#pragma unroll
-  for (int i = 0; i < UNP / 2; ++i) acc[i] = 0.f;
-  for (int c = 0; c < n_local; ++c) {
-    const int s = c & 1;
-    if (c + 1 < n_local) load_a(c + 1);                 // the next chunk's global loads fly during this chunk's MMAs
-    mbar_wait(bar0 + 8 * s, (c >> 1) & 1);              // B block landed
-    {
-      const uint32_t a_hi = smem_base + s * 2 * P_A_BYTES + wg * 64 * 128, a_lo = a_hi + P_A_BYTES;   // warpgroup's 64 rows
-      const uint32_t b_hi = smem_base + 4 * P_A_BYTES + s * P_B_CHUNK, b_lo = b_hi + P_B_BYTES;
-      wgmma_fence();
-      acc_fence(acc);
+  // ---- consumers: warpgroup g = 0, 1 owns rows [64 g, 64 g + 64) of every unit
+  const int g = wg - 1, wt = tid & 127, lane = tid & 31;
+  float acc[P_UN / 2];
+  int q = 0;
+  for (int64_t u = u_begin; u < u_end; ++u) {
+    const PUnit w = p_unit(u, n_rt, n_tiles, n_chunks, k_splits);
+    for (int c = 0; c < w.n_local; ++c, ++q) {
+      const int s = q % S;
+      mbar_wait(full0 + 8 * s, (q / S) & 1);           // A stored and B landed
+      const uint32_t a_hi = smem_base + s * P_STAGE + g * 64 * 128, a_lo = a_hi + P_A_BYTES;
+      const uint32_t b_hi = smem_base + s * P_STAGE + 2 * P_A_BYTES, b_lo = b_hi + P_BH_BYTES;
+      const int nks = min(P_BK / 8, (K - (w.c_begin + c) * P_BK + 7) / 8);   // k-steps that hold data
 #pragma unroll
       for (int ks = 0; ks < P_BK / 8; ++ks) {
-        const uint32_t ko = ks * 32;                       // 8 fp32 = 32 bytes along the swizzled row
-        const uint64_t dAh = make_desc_sw128(a_hi + ko), dAl = make_desc_sw128(a_lo + ko);
-        const uint64_t dBh = make_desc_sw128(b_hi + ko), dBl = make_desc_sw128(b_lo + ko);
-        wgmma_tf32_n208(acc, dAh, dBh, (c | ks) != 0);
-        wgmma_tf32_n208(acc, dAl, dBh, 1);
-        wgmma_tf32_n208(acc, dAh, dBl, 1);
+        if (ks < nks) {
+          wgmma_fence();                                 // orders the accumulator registers for this k-step's wgmma
+          const uint32_t ko = ks * 32;                   // 8 fp32 = 32 bytes along the swizzled row
+          const uint64_t dAh = make_desc_sw128(a_hi + ko), dAl = make_desc_sw128(a_lo + ko);
+          const uint64_t dBh = make_desc_sw128(b_hi + ko), dBl = make_desc_sw128(b_lo + ko);
+          wgmma_tf32_n104(acc, dAh, dBh, (c | ks) != 0);
+          wgmma_tf32_n104(acc, dAl, dBh, 1);
+          wgmma_tf32_n104(acc, dAh, dBl, 1);
+        }
       }
       wgmma_commit();
+      if (c > 0) {
+        wgmma_wait<1>();                                 // the previous chunk's MMAs are complete: release its stage
+        if (lane == 0) mbar_arrive(empty0 + 8 * ((q - 1) % S));
+      }
     }
-    wgmma_wait<1>();                                     // this warpgroup's MMAs of chunk c-1 are complete
-    acc_fence(acc);
-    __syncthreads();                                     // ... and the other's: stage s^1 (A and B) is free
-    if (c + 1 < n_local) {
-      if (tid == 0) issue_b(c + 1);
-      store_a(s ^ 1);
-      __syncthreads();
-    }
-  }
-  wgmma_wait<0>();
-  acc_fence(acc);
-  __syncthreads();                                       // every MMA has read its operands: the stages are reused below
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(empty0 + 8 * ((q - 1) % S));
 
-  float* sC = reinterpret_cast<float*>(smem);
-  acc_store(acc, sC + wg * 64 * CLD, CLD, tid & 127);
-  __syncthreads();
-  {
-    // thread = accumulator row; warps 0-3 take columns [0,104), warps 4-7 [104,208), 8 at a time
-    const int q = warp & 3, half = warp >> 2;
-    const int r = q * 32 + lane;
-    const int cbase = half * 104;
-    const int64_t gr = row_base + r;
-    const float* srow = sC + r * CLD;
-    // EPI 1 state of this thread's (row, half tile): running max / sum of exp; EPI 2: the row's logsumexp and target
-    float run_m = -3.0e38f, run_s = 0.f;
-    const int tgt = (EPI != 0 && gr < M) ? __ldg(epi.target + gr) : -1;
+    const int n0 = w.nt * UN, cb = w.half * P_UN;        // tile column of the unit's column 0
+    const int tile_n = min(UN, N - n0);
+    float* Cz = C + w.zb * batch_c + (int64_t)w.split * split_c;
+    const float* bz = bias != nullptr ? bias + w.zb * (int64_t)N : nullptr;
+    if (EPI == 0) {
+      // straight from the fragment: thread wt holds rows r0, r0 + 8 and, per 8-column group i, columns 8i + c0, +1;
+      // the 4 threads of a quad cover 32 contiguous bytes of a row
+      const int r0 = 16 * (wt >> 5) + ((wt & 31) >> 2), c0 = 2 * (wt & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t gr = w.row_base + 64 * g + r0 + 8 * h;
+        if (gr >= M) continue;
+#pragma unroll
+        for (int i = 0; i < P_UN / 8; ++i) {
+          const int cc = cb + 8 * i;
+          if (cc >= tile_n) continue;
+          float o0 = acc[4 * i + 2 * h], o1 = acc[4 * i + 2 * h + 1];
+          float* cp = Cz + gr * ldc + n0 + cc + c0;
+          if (bz != nullptr) {
+            const float2 bv = __ldg(reinterpret_cast<const float2*>(bz + n0 + cc + c0));
+            o0 += bv.x; o1 += bv.y;
+          }
+          if (accumulate) {
+            const float2 cv = *reinterpret_cast<const float2*>(cp);
+            o0 += cv.x; o1 += cv.y;
+          }
+          *reinterpret_cast<float2*>(cp) = make_float2(o0, o1);
+        }
+      }
+      continue;
+    }
+    // cross-entropy epilogues: thread = row walks the unit's 104 columns in order, 8 at a time
+    float* sC = reinterpret_cast<float*>(smem + S * P_STAGE) + g * 64 * P_CLD;
+    named_bar_sync(1 + g, 128);                          // the previous unit's rows have been read
+    acc_store(acc, sC, P_CLD, wt);
+    named_bar_sync(1 + g, 128);
+    if (wt >= 64) continue;
+    const int64_t gr = w.row_base + 64 * g + wt;
+    const float* srow = sC + wt * P_CLD;
+    float run_m = -3.0e38f, run_s = 0.f;               // EPI 1: running max / sum of exp of this (row, half tile)
+    const int tgt = gr < M ? __ldg(epi.target + gr) : -1;
     const float row_lse = (EPI == 2 && gr < M) ? __ldg(epi.lse + gr) : 0.f;
     const float gscale = (EPI == 2) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
 #pragma unroll 1
-    for (int cc = cbase; cc < cbase + 104; cc += 8) {
+    for (int lc = 0; lc < P_UN; lc += 8) {
+      const int cc = cb + lc;
       if (gr < M && cc < tile_n) {
-        const float4 a0 = *reinterpret_cast<const float4*>(srow + cc), a1 = *reinterpret_cast<const float4*>(srow + cc + 4);
+        const float4 a0 = *reinterpret_cast<const float4*>(srow + lc), a1 = *reinterpret_cast<const float4*>(srow + lc + 4);
         float o[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-        if (EPI != 0) {
-          // fused cross-entropy epilogues: columns are guarded one by one (the class count need not be a multiple of 8)
-          const int nv = min(8, tile_n - cc);
-          float mx = -3.0e38f;
+        // columns are guarded one by one (the class count need not be a multiple of 8)
+        const int nv = min(8, tile_n - cc);
+        float mx = -3.0e38f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          if (i < nv) {
+            if (bz != nullptr) o[i] += __ldg(bz + n0 + cc + i);
+            mx = fmaxf(mx, o[i]);
+          }
+        if (EPI == 1) {
+          const float nm = fmaxf(run_m, mx);
+          float add = 0.f;
 #pragma unroll
           for (int i = 0; i < 8; ++i)
             if (i < nv) {
-              if (bias != nullptr) o[i] += __ldg(bias + n0 + cc + i);
-              mx = fmaxf(mx, o[i]);
+              add += expf(o[i] - nm);
+              if (n0 + cc + i == tgt) epi.tlogit[gr] = o[i];
             }
-          if (EPI == 1) {
-            const float nm = fmaxf(run_m, mx);
-            float add = 0.f;
+          run_s = run_s * expf(run_m - nm) + add;
+          run_m = nm;
+        } else {
+          float* dp = Cz + gr * ldc + n0 + cc;
 #pragma unroll
-            for (int i = 0; i < 8; ++i)
-              if (i < nv) {
-                add += expf(o[i] - nm);
-                if (n0 + cc + i == tgt) epi.tlogit[gr] = o[i];
-              }
-            run_s = run_s * expf(run_m - nm) + add;
-            run_m = nm;
-          } else {
-            float* dp = C + gr * ldc + n0 + cc;
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              if (i < nv) {
-                const float gv = (expf(o[i] - row_lse) - (n0 + cc + i == tgt ? 1.f : 0.f)) * gscale;
-                dp[i] = gv;                                              // row-major: A of dX = dlogits @ W
-                epi.dT[(int64_t)(n0 + cc + i) * epi.ldT + gr] = gv;      // transposed (lanes = consecutive rows: coalesced)
-              }
-          }
-          continue;
+          for (int i = 0; i < 8; ++i)
+            if (i < nv) {
+              const float gv = (expf(o[i] - row_lse) - (n0 + cc + i == tgt ? 1.f : 0.f)) * gscale;
+              dp[i] = gv;                                              // row-major: A of dX = dlogits @ W
+              epi.dT[(int64_t)(n0 + cc + i) * epi.ldT + gr] = gv;      // transposed (lanes = consecutive rows: coalesced)
+            }
         }
-        float* cp = C + gr * ldc + n0 + cc;
-        if (bias != nullptr) {
-          const float4 b0 = ldg_f4(bias + n0 + cc), b1 = ldg_f4(bias + n0 + cc + 4);
-          o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w;
-          o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
-        }
-        if (accumulate) {
-          const float4 c0 = *reinterpret_cast<const float4*>(cp), c1 = *reinterpret_cast<const float4*>(cp + 4);
-          o[0] += c0.x; o[1] += c0.y; o[2] += c0.z; o[3] += c0.w;
-          o[4] += c1.x; o[5] += c1.y; o[6] += c1.z; o[7] += c1.w;
-        }
-        st_f4(cp, make_float4(o[0], o[1], o[2], o[3]));
-        st_f4(cp + 4, make_float4(o[4], o[5], o[6], o[7]));
       }
     }
     if (EPI == 1 && gr < M) {
-      const int64_t pi = (int64_t)(nt * 2 + half) * M + gr;
+      const int64_t pi = (int64_t)(w.nt * 2 + w.half) * M + gr;
       epi.pmax[pi] = run_m;
       epi.psum[pi] = run_s;
     }
@@ -518,21 +586,23 @@ int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, 
   if (M <= 0) return RENET_OK;
   static bool attr2 = false;
   if (!attr2) {
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM));
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM));
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM));
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(0)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(0)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(1)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(2)));
     attr2 = true;
   }
   const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
   if (k_splits < 1) k_splits = 1;
   if (k_splits > n_chunks) k_splits = n_chunks;
   while (k_splits > 1 && ((n_chunks + k_splits - 1) / k_splits) * (k_splits - 1) >= n_chunks) --k_splits;   // no empty split
-  dim3 grid((unsigned)((M + UM - 1) / UM), (unsigned)n_tiles, (unsigned)(batch * k_splits));
+  // persistent grid: at most one CTA per SM, each walking a balanced range of 128 x 104 work units
+  const int64_t n_units = (M + UM - 1) / UM * (2 * n_tiles) * batch * k_splits;
+  const unsigned grid = (unsigned)(n_units < kNumSMs ? n_units : kNumSMs);
 #define RENET_UMMA_LAUNCH(IDX, EP)                                                                                       \
-  umma_gemm_packed_kernel<IDX, EP><<<grid, UTHREADS, P_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M, N, K, \
-                                                                      n_chunks, accumulate, batch_a, batch_bp, batch_c, epi,  \
-                                                                      k_splits, split_c)
+  umma_gemm_packed_kernel<IDX, EP><<<grid, P_THREADS, p_smem(EP), stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, \
+                                                                           M, N, K, n_chunks, accumulate, batch_a, batch_bp,  \
+                                                                           batch_c, epi, k_splits, split_c, n_units)
   if (epi_mode == 1) RENET_UMMA_LAUNCH(false, 1);
   else if (epi_mode == 2) RENET_UMMA_LAUNCH(false, 2);
   else if (a_index) RENET_UMMA_LAUNCH(true, 0);
