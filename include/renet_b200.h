@@ -128,6 +128,11 @@ int renet_rgcn_gather_hot(const float* H, const int32_t* h_index, const float* W
  * gather launch writes per-warp time stamps into it (SM clock at entry / after the partition / first edge / last edge /
  * exit, global timer at entry and exit, edge count).  Pass NULL to switch it off; never set in production code. */
 int renet_debug_stream_timing(void* buffer);
+/* DEBUG ONLY (tools/gemm_timeline.py): while `buffer` (device, 132 x 4 x 8 int64) is non-NULL, every packed tensor-core GEMM
+ * launch writes one record per warpgroup into it (global timer at entry and exit, SM clocks entry -> exit and spent waiting
+ * on operand barriers, in wgmma waits, in the epilogue and splitting A, work items and role).  Pass NULL to switch it off;
+ * never set in production code. */
+int renet_debug_gemm_timing(void* buffer);
 
 /* ------------------------------------------------------------------------------------------------
  * RGCN block-diagonal layer, backward (autograd of the above; the reference relies on

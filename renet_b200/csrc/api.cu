@@ -219,6 +219,11 @@ int renet_debug_stream_timing(void* buffer) {
   return RENET_OK;
 }
 
+int renet_debug_gemm_timing(void* buffer) {
+  set_gemm_debug_buffer(static_cast<long long*>(buffer));
+  return RENET_OK;
+}
+
 int renet_rgcn_block_fwd(const float* H, const int32_t* h_index, const float* W, const float* Wloop,
                          const int32_t* row_ptr, const int32_t* col_src, const int32_t* col_type,
                          const float* norm, float* Hout, int64_t N, int64_t E, int32_t d_in, int32_t d_out,

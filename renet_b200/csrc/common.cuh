@@ -85,6 +85,7 @@ void set_stream_debug_buffer(long long* p);   // debug: per-warp time stamps of 
 // tensor-core (wgmma) GEMM engine building blocks (umma_gemm.cu); gemm_mode() == 1 selects the engine
 int gemm_mode();
 int64_t umma_packed_bytes(int N, int K);
+void set_gemm_debug_buffer(long long* p);     // debug: per-warpgroup time stamps of the packed GEMM kernels (umma_gemm.cu)
 // packed-weight cache (umma_gemm.cu): persistent device buffer for this key, or nullptr when caching is off; *hit says
 // whether it already holds the image for the current weight generation
 void set_weight_generation(int64_t g);

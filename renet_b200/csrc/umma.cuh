@@ -134,6 +134,39 @@ __device__ __forceinline__ void wgmma_tf32_n104(float (&d)[52], uint64_t adesc, 
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// Same product with A in registers (the RS form): warp w of the warpgroup supplies rows [16w, 16w + 16); lane l holds
+// a0 = (l/4, l%4), a1 = (l/4 + 8, l%4), a2 = (l/4, l%4 + 4), a3 = (l/4 + 8, l%4 + 4) of the k8 step.  The registers are
+// read asynchronously: they must not be redefined before the group's wgmma.wait_group.
+__device__ __forceinline__ void wgmma_tf32_n104_rs(float (&d)[52], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                   uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %57, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n104k8.f32.tf32.tf32 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51"
+      "}, {%52,%53,%54,%55}, %56, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(accumulate));
+}
+// keeps the compiler from reusing wgmma A-operand registers before the wgmma.wait_group that ends their group
+template <int NR>
+__device__ __forceinline__ void reg_fence(uint32_t (&r)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+r"(r[i])::"memory");
+}
+
 // D[64 x 96] (+)= A[64 x 8] . B[96 x 8]^T, tf32 in, fp32 accumulators in registers (m64n96k8 fragment layout)
 __device__ __forceinline__ void wgmma_tf32_n96(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(

@@ -273,6 +273,63 @@ __device__ __forceinline__ PUnit p_unit(int64_t u, int64_t n_rt, int n_tiles, in
   return w;
 }
 
+// Debug timeline (renet_debug_gemm_timing, tools/gemm_timeline.py; dbg is nullptr in production): thread 0 of every
+// warpgroup writes one record of 8 int64 at dbg[(blockIdx.x * 4 + warpgroup) * 8]:
+//   global timer at entry and exit, SM clocks entry -> exit, SM clocks spent waiting on operand barriers (streaming
+//   producer: empty; streaming consumer: full; resident: the B chunks), in wgmma.wait_group, in the epilogue, and (resident)
+//   in the hi/lo split of A, which absorbs the wait for its global loads; then items done | role << 32
+//   (role 0 = streaming producer, 1 = streaming consumer, 2 = resident consumer).
+struct GemmStamps {
+  long long* rec;
+  long long g0, c0, bar, mma, epi, aop;
+  int items;
+  __device__ __forceinline__ GemmStamps(long long* dbg, int wg) : bar(0), mma(0), epi(0), aop(0), items(0) {
+    rec = (dbg != nullptr && (threadIdx.x & 127) == 0) ? dbg + ((int64_t)blockIdx.x * 4 + wg) * 8 : nullptr;
+    g0 = c0 = 0;
+    if (rec) {
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g0));
+      c0 = clock64();
+    }
+  }
+  __device__ __forceinline__ long long now() const { return rec ? clock64() : 0; }
+  __device__ __forceinline__ void finish(int role) const {
+    if (!rec) return;
+    long long g1;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1));
+    rec[0] = g0; rec[1] = g1; rec[2] = clock64() - c0; rec[3] = bar; rec[4] = mma; rec[5] = epi; rec[6] = aop;
+    rec[7] = (long long)items | ((long long)role << 32);
+  }
+};
+
+// EPI 0 straight from a warpgroup's m64n104 fragment: thread wt holds rows r0, r0 + 8 of the 64 rows at row_base and, per
+// 8-column group i, columns 8i + c0, +1 of the 104 at tile column cb; the 4 threads of a quad cover 32 contiguous bytes
+__device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], float* __restrict__ Cz, int64_t ldc,
+                                               const float* __restrict__ bz, int64_t row_base, int64_t M, int n0, int cb,
+                                               int tile_n, int accumulate, int wt) {
+  const int r0 = 16 * (wt >> 5) + ((wt & 31) >> 2), c0 = 2 * (wt & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t gr = row_base + r0 + 8 * h;
+    if (gr >= M) continue;
+#pragma unroll
+    for (int i = 0; i < P_UN / 8; ++i) {
+      const int cc = cb + 8 * i;
+      if (cc >= tile_n) continue;
+      float o0 = acc[4 * i + 2 * h], o1 = acc[4 * i + 2 * h + 1];
+      float* cp = Cz + gr * ldc + n0 + cc + c0;
+      if (bz != nullptr) {
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(bz + n0 + cc + c0));
+        o0 += bv.x; o1 += bv.y;
+      }
+      if (accumulate) {
+        const float2 cv = *reinterpret_cast<const float2*>(cp);
+        o0 += cv.x; o1 += cv.y;
+      }
+      *reinterpret_cast<float2*>(cp) = make_float2(o0, o1);
+    }
+  }
+}
+
 // Fused-epilogue modes of the packed kernel (the decoder of model.py:89-91,97-100: logits = X @ W^T + b, cross-entropy):
 //   EPI 0  C = acc (+bias) (+C)                                   -- plain GEMM
 //   EPI 1  per (row, half column tile): running max and sum of exp of the logits, and the target's logit -- the
@@ -288,7 +345,7 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
                         const uint8_t* __restrict__ Bp, float* __restrict__ C, int64_t ldc,
                         const float* __restrict__ bias, int64_t M, int N, int K, int n_chunks, int accumulate,
                         int64_t batch_a, int64_t batch_bp, int64_t batch_c, EpiArgs epi, int k_splits, int64_t split_c,
-                        int64_t n_units) {
+                        int64_t n_units, long long* dbg) {
   constexpr int S = p_stages(EPI);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -299,6 +356,7 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
   const uint32_t empty0 = full0 + 8 * S;
   const int tid = threadIdx.x;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warp-uniform to the compiler: the wgmma paths do not diverge
+  GemmStamps ts(dbg, wg);
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(full0 + 8 * s, 128);     // every producer thread arrives after its A stores; the B copies add bytes
@@ -347,7 +405,10 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     auto commit = [&](const float4 (&v)[8], const uint8_t* bsrc, int q) {
       const int s = q % S;
       const uint32_t full = full0 + 8 * s, st = smem_base + s * P_STAGE;
+      const long long t0 = ts.now();
       mbar_wait(empty0 + 8 * s, ((q / S) & 1) ^ 1);     // the consumers are done with the stage's previous chunk
+      ts.bar += ts.now() - t0;
+      ++ts.items;
       if (tid == 0) {
         mbar_expect_tx(full, 2 * P_BH_BYTES);
         bulk_copy_g2s(st + 2 * P_A_BYTES, bsrc, P_BH_BYTES, full);
@@ -364,21 +425,23 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
       mbar_arrive(full);
     };
-    if (lu >= u_end) return;
-    set_unit();
-    float4 va[8], vb[8];
-    const uint8_t *ba, *bb;
-    load(va, ba);
-    for (int q = 0;; q += 2) {
-      const bool more_b = lu < u_end;
-      if (more_b) load(vb, bb);
-      commit(va, ba, q);
-      if (!more_b) break;
-      const bool more_a = lu < u_end;
-      if (more_a) load(va, ba);
-      commit(vb, bb, q + 1);
-      if (!more_a) break;
+    if (lu < u_end) {
+      set_unit();
+      float4 va[8], vb[8];
+      const uint8_t *ba, *bb;
+      load(va, ba);
+      for (int q = 0;; q += 2) {
+        const bool more_b = lu < u_end;
+        if (more_b) load(vb, bb);
+        commit(va, ba, q);
+        if (!more_b) break;
+        const bool more_a = lu < u_end;
+        if (more_a) load(va, ba);
+        commit(vb, bb, q + 1);
+        if (!more_a) break;
+      }
     }
+    ts.finish(0);
     return;
   }
 
@@ -388,9 +451,12 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
   int q = 0;
   for (int64_t u = u_begin; u < u_end; ++u) {
     const PUnit w = p_unit(u, n_rt, n_tiles, n_chunks, k_splits);
+    ++ts.items;
     for (int c = 0; c < w.n_local; ++c, ++q) {
       const int s = q % S;
+      long long t0 = ts.now();
       mbar_wait(full0 + 8 * s, (q / S) & 1);           // A stored and B landed
+      ts.bar += ts.now() - t0;
       const uint32_t a_hi = smem_base + s * P_STAGE + g * 64 * 128, a_lo = a_hi + P_A_BYTES;
       const uint32_t b_hi = smem_base + s * P_STAGE + 2 * P_A_BYTES, b_lo = b_hi + P_BH_BYTES;
       const int nks = min(P_BK / 8, (K - (w.c_begin + c) * P_BK + 7) / 8);   // k-steps that hold data
@@ -408,11 +474,15 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
       }
       wgmma_commit();
       if (c > 0) {
+        t0 = ts.now();
         wgmma_wait<1>();                                 // the previous chunk's MMAs are complete: release its stage
+        ts.mma += ts.now() - t0;
         if (lane == 0) mbar_arrive(empty0 + 8 * ((q - 1) % S));
       }
     }
+    long long t0 = ts.now();
     wgmma_wait<0>();
+    ts.mma += ts.now() - t0;
     if (lane == 0) mbar_arrive(empty0 + 8 * ((q - 1) % S));
 
     const int n0 = w.nt * UN, cb = w.half * P_UN;        // tile column of the unit's column 0
@@ -420,30 +490,9 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     float* Cz = C + w.zb * batch_c + (int64_t)w.split * split_c;
     const float* bz = bias != nullptr ? bias + w.zb * (int64_t)N : nullptr;
     if (EPI == 0) {
-      // straight from the fragment: thread wt holds rows r0, r0 + 8 and, per 8-column group i, columns 8i + c0, +1;
-      // the 4 threads of a quad cover 32 contiguous bytes of a row
-      const int r0 = 16 * (wt >> 5) + ((wt & 31) >> 2), c0 = 2 * (wt & 3);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t gr = w.row_base + 64 * g + r0 + 8 * h;
-        if (gr >= M) continue;
-#pragma unroll
-        for (int i = 0; i < P_UN / 8; ++i) {
-          const int cc = cb + 8 * i;
-          if (cc >= tile_n) continue;
-          float o0 = acc[4 * i + 2 * h], o1 = acc[4 * i + 2 * h + 1];
-          float* cp = Cz + gr * ldc + n0 + cc + c0;
-          if (bz != nullptr) {
-            const float2 bv = __ldg(reinterpret_cast<const float2*>(bz + n0 + cc + c0));
-            o0 += bv.x; o1 += bv.y;
-          }
-          if (accumulate) {
-            const float2 cv = *reinterpret_cast<const float2*>(cp);
-            o0 += cv.x; o1 += cv.y;
-          }
-          *reinterpret_cast<float2*>(cp) = make_float2(o0, o1);
-        }
-      }
+      t0 = ts.now();
+      store_fragment(acc, Cz, ldc, bz, w.row_base + 64 * g, M, n0, cb, tile_n, accumulate, wt);
+      ts.epi += ts.now() - t0;
       continue;
     }
     // cross-entropy epilogues: thread = row walks the unit's 104 columns in order, 8 at a time
@@ -502,6 +551,142 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
       epi.psum[pi] = run_s;
     }
   }
+  ts.finish(1);
+}
+
+// ======================================================================================================
+// Resident-panel kernel: EPI 0, no split-K, K <= 224 (the self-loop, the GRU projections)
+//
+// The timeline of the streaming kernel above (DESIGN §5) shows its consumers starved of operands: every 128 x 104 unit
+// re-reads its 186 KB B half from L2 and has its A staged through shared memory by the producer.  Here a panel is one
+// (batch entry, column tile, 104-column half) of the packed B.  The CTAs are split evenly over the panels and CTA j of a
+// panel's n owns the 64-row tiles [j*R/n, (j+1)*R/n) of its R.  At entry thread 0 issues the copies of the panel's whole
+// hi/lo image (n_chunks x 26 KB, one mbarrier per chunk, so chunk 0's MMAs start while the rest lands); B is never
+// reloaded.  Three warpgroups, no producer: warpgroup g takes the CTA's tiles g, g + 3, ... and feeds A to wgmma from
+// registers (m64n104k8, RS form).  Each thread loads its fragment's elements of rows r and r + 8 straight from global memory
+// (rows gathered through a_index), the next chunk's while the current chunk's wgmma group runs, and splits them into
+// hi/lo in registers.  Each output element sees the k-steps in order and per k-step the products hi*hi, lo*hi, hi*lo, with
+// the same operands as in the streaming kernel.
+// ======================================================================================================
+constexpr int R_MAX_CHUNKS = 7;                      // K <= 224: the whole panel fits in shared memory
+constexpr int R_CHUNK = 2 * P_BH_BYTES;              // 26624: hi and lo halves of one 32-wide K chunk of a panel
+constexpr int R_THREADS = 384;
+constexpr int R_SMEM = R_MAX_CHUNKS * R_CHUNK + 1024 + 8 * R_MAX_CHUNKS;
+static_assert(R_SMEM <= 232448, "one CTA's shared memory");
+
+template <bool INDEXED>
+__global__ void __launch_bounds__(R_THREADS, 1)
+umma_gemm_resident_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_index, int64_t lda,
+                          const uint8_t* __restrict__ Bp, float* __restrict__ C, int64_t ldc, const float* __restrict__ bias,
+                          int64_t M, int N, int K, int n_chunks, int accumulate, int64_t batch_a, int64_t batch_bp,
+                          int64_t batch_c, int n_panels, long long* dbg) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t sb = raw + ((1024 - (raw & 1023)) & 1023);       // swizzle atoms need 1024-byte alignment
+  const uint32_t bar0 = sb + R_MAX_CHUNKS * R_CHUNK;
+  const int tid = threadIdx.x;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+  // panel p owns the CTAs [p*G/P, (p+1)*G/P) (G >= P: at least one each)
+  const int G = gridDim.x, b = blockIdx.x;
+  const int p = (int)(((int64_t)(b + 1) * n_panels - 1) / G);
+  const int cta0 = (int)((int64_t)p * G / n_panels), ncta = (int)((int64_t)(p + 1) * G / n_panels) - cta0;
+  const int64_t n_rt = (M + 63) / 64;
+  const int64_t t_begin = (int64_t)(b - cta0) * n_rt / ncta, t_end = (int64_t)(b - cta0 + 1) * n_rt / ncta;
+  // the launcher's grid gives every CTA a tile; a CTA without one must not issue copies it would never wait for
+  if (t_begin == t_end) return;
+  const int n_tiles = (N + UN - 1) / UN;
+  const int half = p & 1, nt = (p >> 1) % n_tiles, zb = (p >> 1) / n_tiles;
+  GemmStamps ts(dbg, wg);
+  if (tid == 0) {
+    for (int c = 0; c < n_chunks; ++c) mbar_init(bar0 + 8 * c, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    const uint8_t* src = Bp + zb * batch_bp + (size_t)nt * n_chunks * P_B_CHUNK + half * P_BH_BYTES;
+    for (int c = 0; c < n_chunks; ++c) {
+      const uint32_t bar = bar0 + 8 * c, dst = sb + c * R_CHUNK;
+      mbar_expect_tx(bar, R_CHUNK);
+      bulk_copy_g2s(dst, src + (size_t)c * P_B_CHUNK, P_BH_BYTES, bar);
+      bulk_copy_g2s(dst + P_BH_BYTES, src + (size_t)c * P_B_CHUNK + P_B_BYTES, P_BH_BYTES, bar);
+      mbar_arrive(bar);
+    }
+  }
+  __syncthreads();                                                // the barriers are initialised
+
+  const int wt = tid & 127, lane = tid & 31, tig = lane & 3;
+  const int ra = 16 * (wt >> 5) + (lane >> 2);                    // this thread's fragment rows: ra, ra + 8
+  const float* Az = A + zb * batch_a;
+  auto row_ptr = [&](int64_t gr) -> const float* {
+    return gr < M ? Az + (INDEXED ? (int64_t)__ldg(a_index + gr) : gr) * lda : nullptr;
+  };
+  // v[j] = A[row ra][32c + 4j + tig], v[8 + j] = the same of row ra + 8: k-step ks takes j = 2ks (a0, a1) and 2ks + 1 (a2, a3)
+  auto load = [&](float (&v)[16], const float* pa, const float* pb, int c) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = c * P_BK + 4 * j + tig;
+      v[j] = (pa != nullptr && k < K) ? __ldg(pa + k) : 0.f;
+      v[8 + j] = (pb != nullptr && k < K) ? __ldg(pb + k) : 0.f;
+    }
+  };
+  int64_t t = t_begin + wg;
+  const float *pa = nullptr, *pb = nullptr;
+  float v[16];
+  if (t < t_end) {
+    pa = row_ptr(t * 64 + ra);
+    pb = row_ptr(t * 64 + ra + 8);
+    load(v, pa, pb, 0);
+  }
+  const int n0 = nt * UN, cb = half * P_UN, tile_n = min(UN, N - n0);
+  float* Cz = C + zb * batch_c;
+  const float* bz = bias != nullptr ? bias + zb * (int64_t)N : nullptr;
+  float acc[P_UN / 2];
+  for (; t < t_end; t += 3) {
+    ++ts.items;
+    for (int c = 0; c < n_chunks; ++c) {
+      long long t0 = ts.now();
+      uint32_t hi[16], lo[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        float h, l;
+        split_tf32(v[j], h, l);
+        hi[j] = __float_as_uint(h);
+        lo[j] = __float_as_uint(l);
+      }
+      ts.aop += ts.now() - t0;
+      if (c + 1 < n_chunks) {
+        load(v, pa, pb, c + 1);
+      } else if (t + 3 < t_end) {                                 // the next tile's first chunk
+        pa = row_ptr((t + 3) * 64 + ra);
+        pb = row_ptr((t + 3) * 64 + ra + 8);
+        load(v, pa, pb, 0);
+      }
+      t0 = ts.now();
+      mbar_wait(bar0 + 8 * c, 0);                                 // chunk c of the panel has landed (once per CTA)
+      ts.bar += ts.now() - t0;
+      const int nks = min(P_BK / 8, (K - c * P_BK + 7) / 8);      // k-steps that hold data
+      const uint32_t b_hi = sb + c * R_CHUNK, b_lo = b_hi + P_BH_BYTES;
+      wgmma_fence();                                              // orders the A and accumulator registers for the wgmma
+#pragma unroll
+      for (int ks = 0; ks < P_BK / 8; ++ks) {
+        if (ks < nks) {
+          const uint64_t dBh = make_desc_sw128(b_hi + ks * 32), dBl = make_desc_sw128(b_lo + ks * 32);
+          const int j = 2 * ks;
+          wgmma_tf32_n104_rs(acc, hi[j], hi[8 + j], hi[j + 1], hi[9 + j], dBh, (c | ks) != 0);
+          wgmma_tf32_n104_rs(acc, lo[j], lo[8 + j], lo[j + 1], lo[9 + j], dBh, 1);
+          wgmma_tf32_n104_rs(acc, hi[j], hi[8 + j], hi[j + 1], hi[9 + j], dBl, 1);
+        }
+      }
+      wgmma_commit();
+      t0 = ts.now();
+      wgmma_wait<0>();
+      ts.mma += ts.now() - t0;
+      acc_fence(acc);
+      reg_fence(hi);
+      reg_fence(lo);
+    }
+    const long long t0 = ts.now();
+    store_fragment(acc, Cz, ldc, bz, t * 64, M, n0, cb, tile_n, accumulate, wt);
+    ts.epi += ts.now() - t0;
+  }
+  ts.finish(2);
 }
 
 }  // namespace
@@ -511,6 +696,8 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
 static uint8_t* g_scratch = nullptr;
 static int64_t g_scratch_bytes = 0;
 void set_scratch(void* p, int64_t bytes) { g_scratch = (uint8_t*)p; g_scratch_bytes = p ? bytes : 0; }
+static long long* g_gemm_dbg = nullptr;
+void set_gemm_debug_buffer(long long* p) { g_gemm_dbg = p; }
 
 // ---- packed-weight cache (renet_set_weight_generation) ------------------------------------------------------------------
 // Packing a weight into the tensor-core operand image is a kernel launch per weight per call.  Weights only change when the
@@ -596,13 +783,36 @@ int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, 
   if (k_splits < 1) k_splits = 1;
   if (k_splits > n_chunks) k_splits = n_chunks;
   while (k_splits > 1 && ((n_chunks + k_splits - 1) / k_splits) * (k_splits - 1) >= n_chunks) --k_splits;   // no empty split
+  const int n_panels = batch * n_tiles * 2;
+  if (epi_mode == 0 && k_splits == 1 && n_chunks <= R_MAX_CHUNKS && n_panels <= kNumSMs) {
+    static bool attr_r = false;
+    if (!attr_r) {
+      RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_resident_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, R_SMEM));
+      RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_resident_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, R_SMEM));
+      attr_r = true;
+    }
+    // every panel gets at least one CTA; a CTA never holds more than one panel
+    const int64_t n_work = (int64_t)n_panels * ((M + 63) / 64);
+    const unsigned grid = (unsigned)(n_work < kNumSMs ? n_work : kNumSMs);
+    if (a_index)
+      umma_gemm_resident_kernel<true><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
+                                                                          N, K, n_chunks, accumulate, batch_a, batch_bp,
+                                                                          batch_c, n_panels, g_gemm_dbg);
+    else
+      umma_gemm_resident_kernel<false><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
+                                                                           N, K, n_chunks, accumulate, batch_a, batch_bp,
+                                                                           batch_c, n_panels, g_gemm_dbg);
+    RENET_CHECK_LAUNCH("umma_gemm_resident_kernel");
+    return 1;
+  }
   // persistent grid: at most one CTA per SM, each walking a balanced range of 128 x 104 work units
   const int64_t n_units = (M + UM - 1) / UM * (2 * n_tiles) * batch * k_splits;
   const unsigned grid = (unsigned)(n_units < kNumSMs ? n_units : kNumSMs);
 #define RENET_UMMA_LAUNCH(IDX, EP)                                                                                       \
   umma_gemm_packed_kernel<IDX, EP><<<grid, P_THREADS, p_smem(EP), stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, \
                                                                            M, N, K, n_chunks, accumulate, batch_a, batch_bp,  \
-                                                                           batch_c, epi, k_splits, split_c, n_units)
+                                                                           batch_c, epi, k_splits, split_c, n_units, \
+                                                                           g_gemm_dbg)
   if (epi_mode == 1) RENET_UMMA_LAUNCH(false, 1);
   else if (epi_mode == 2) RENET_UMMA_LAUNCH(false, 2);
   else if (a_index) RENET_UMMA_LAUNCH(true, 0);
