@@ -11,14 +11,18 @@
 //     and its warps split that EDGE range evenly at arbitrary cuts;
 //   * the most frequent relation rows -- a list the caller passes (relation frequencies are a property of the dataset:
 //     GraphStore computes it once), else the top of a histogram of the CTA's own edge types built in the prologue -- are
-//     fetched once into shared memory by cp.async.bulk on an mbarrier;
-//   * per edge one elected lane issues a cp.async.bulk of the 800-byte source row (and, for a cold relation, of the
-//     1600-byte relation row) into a per-warp ring of D slots, completing on the slot's mbarrier; the warp consumes
-//     edge i (4 x LDS.64 + 4 x LDS.128 per lane, conflict-free) while the copies of the next D edges are in flight.
-//     No register holds a load in flight; the edge indices of a block of edges are staged once in shared memory, so
-//     the per-edge code has no shuffles; the ring keeps streaming across destinations (no per-tile prologue).
-//     What bounds it then is the shared-memory pipe (ring write + ring read + relation row read per edge;
-//     tools/stream_timeline.py times it), which is why more warps (32, two slots each) beat deeper rings;
+//     fetched once into shared memory by cp.async.bulk, as many as fit (82 forward: about three quarters of an ICEWS18
+//     batch's edges), in 8 groups on 8 mbarriers: an edge waits only for its own group, so the edge loop does not wait for the
+//     table;
+//   * per edge one elected lane issues a cp.async.bulk of the 800-byte source row into a per-warp ring of D slots,
+//     completing on the slot's mbarrier; the warp consumes edge i (4 x LDS.64 + 4 x LDS.128 per lane, conflict-free)
+//     while the copies of the next D edges are in flight.  The 1600-byte row of a cold relation is loaded by the lanes
+//     straight into the registers that a resident row would be read into (4 x LDG.128, issued before the wait for the
+//     source row); the other 31 warps cover its L2 latency.  The edge indices of a block of edges are staged once in
+//     shared memory, so the per-edge code has no shuffles; the ring keeps streaming across destinations.
+//     On the H100 the edge loop is bound by what each edge moves from L2 (tools/stream_timeline.py: 74 SM cycles per
+//     edge with cold rows in the ring and 18 resident rows, 61 with 82; the shared-memory work is about 30): so the
+//     ring holds source rows only and the shared memory goes to resident relation rows;
 //   * the running destination's sum stays in registers (edges are destination-sorted: a segmented reduction); a
 //     destination that starts and ends inside the warp's range goes straight from registers through the fused
 //     norm / self-loop / activation epilogue to global memory; one cut by a warp boundary is handed over through a
@@ -36,21 +40,23 @@ namespace renet {
 constexpr int kStRpCap = 1024;           // row_ptr entries of the CTA's destinations kept in shared memory
 constexpr int kStMaxR2 = 2048;           // relation-id range of the hot-row lookup table (beyond: every row comes from L2)
 constexpr int kStNodeCost = 2;           // a destination (epilogue: self-loop row, norm, 800-byte store) costs about two edges
-constexpr int kStSlot = 2400;            // ring slot: 800 B source row + 1600 B relation row (cold relations only)
+constexpr int kStSlot = 800;             // ring slot: one source row (cold relation rows are loaded into registers)
+constexpr int kStHotGroups = 8;          // the resident rows land in 8 groups, one mbarrier each
 // WARPS warps per CTA (>= 16), D edges in flight per warp, HOT relation rows resident per CTA; shared memory map (bytes)
 template <int WARPS, int D, int HOT, bool BWD>
 struct StCfg {
   static constexpr int kWarps = WARPS, kThreads = WARPS * 32, kD = D, kHot = HOT;
+  static constexpr int kHotPerGroup = (HOT + kStHotGroups - 1) / kStHotGroups;
   static constexpr int kBlk = (32 / D) * D;                                 // edges per index block (a multiple of D)
-  static constexpr int kOffRing = 0;                                        // [warps][D][2400]; prologue scratch: cnt + hist
+  static constexpr int kOffRing = 0;                                        // [warps][D][800]; prologue scratch: cnt + hist
   static constexpr int kOffHot = kOffRing + WARPS * D * kStSlot;            // [HOT][1600]
   static constexpr int kOffHeads = kOffHot + HOT * 1600;                    // [warps][200] floats
   static constexpr int kOffRp = kOffHeads + WARPS * 800;                    // [kStRpCap] ints
   static constexpr int kOffSlotOf = kOffRp + kStRpCap * 4;                  // [kStMaxR2] uint8: 1 + hot slot, 0 = cold
-  static constexpr int kOffIdx = kOffSlotOf + kStMaxR2;                     // [warps][2][32] int2 {source row, relation | w_off16 << 16}
+  static constexpr int kOffIdx = kOffSlotOf + kStMaxR2;                     // [warps][2][32] int2 {source row, see block_stage}
   static constexpr int kOffSc = kOffIdx + WARPS * 64 * 8;                   // BWD: [warps][2][32] float edge scales
-  static constexpr int kOffBars = kOffSc + (BWD ? WARPS * 64 * 4 : 0);      // mbarriers: [warps][D] ring slots, hot rows, [warps] heads
-  static constexpr int kOffFlags = kOffBars + (WARPS * D + 1 + WARPS) * 8;  // [warps] (unused) + partition scratch (16) + range starts [warps + 1]
+  static constexpr int kOffBars = kOffSc + (BWD ? WARPS * 64 * 4 : 0);      // mbarriers: [warps][D] ring slots, [8] hot groups, [warps] heads
+  static constexpr int kOffFlags = kOffBars + (WARPS * D + kStHotGroups + WARPS) * 8;  // [warps] (unused) + partition scratch (16) + range starts [warps + 1]
   static constexpr int kSmemBytes = kOffFlags + (2 * WARPS + 17) * 4;
   static_assert(WARPS >= 16 && WARPS <= 32, "stream gather: the partition search needs 512 threads");
   static_assert(kBlk == 32, "stream gather: index blocks are 32 edges (D = 2 or 4)");
@@ -58,8 +64,9 @@ struct StCfg {
   static_assert(WARPS * D * kStSlot >= (kStMaxR2 + 256 + 8) * 4, "stream gather: prologue scratch lives in the ring");
   static_assert(HOT <= 254 && (kOffHot + HOT * 1600) / 16 < 65536, "stream gather: hot rows are addressed by 16-bit offsets");
 };
+// as many resident rows as fit: forward 82 (about three quarters of ICEWS18's edges with the dataset ranking), backward 77
 template <bool BWD>
-using StDefault = StCfg<32, 2, BWD ? 13 : 18, BWD>;
+using StDefault = StCfg<32, 2, BWD ? 77 : 82, BWD>;
 
 namespace {
 
@@ -115,11 +122,6 @@ __device__ __forceinline__ uint32_t st_lds_u32(uint32_t a) {
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(a));
   return r;
 }
-__device__ __forceinline__ uint2 st_lds_u2(uint32_t a) {
-  uint2 r;
-  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "r"(a));
-  return r;
-}
 __device__ __forceinline__ uint32_t st_opaque(uint32_t v) {    // keeps a loop-invariant address in a register (no rematerialisation)
   asm volatile("" : "+r"(v));
   return v;
@@ -143,11 +145,17 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   // dbg (tools/stream_timeline.py only; nullptr otherwise): 8 stamps per warp -- SM clock at entry / after the partition /
   // at the first edge / after the last edge / at exit, global timer at entry and exit, edge count
   extern __shared__ __align__(128) uint8_t st_smem[];
-  long long t_entry = 0, g_entry = 0;
-  if (dbg) {
-    t_entry = clock64();
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g_entry));
-  }
+  // each stamp is stored when it is taken (its address from the launch parameters and special registers): no register
+  // holds a stamp through the edge loop
+  auto stamp = [&](int k, long long v) {
+    if (dbg && (threadIdx.x & 31) == 0) dbg[((int64_t)blockIdx.x * Cfg::kWarps + (threadIdx.x >> 5)) * 8 + k] = v;
+  };
+  auto global_timer = []() {
+    long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+  };
+  if (dbg) { stamp(0, clock64()); stamp(5, global_timer()); }
   constexpr int D = Cfg::kD, kBlk = Cfg::kBlk, kStWarps = Cfg::kWarps, kStThreads = Cfg::kThreads;
   float* heads = reinterpret_cast<float*>(st_smem + Cfg::kOffHeads);
   int32_t* s_rp = reinterpret_cast<int32_t*>(st_smem + Cfg::kOffRp);
@@ -181,8 +189,8 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     if (pf) asm volatile("prefetch.global.L2 [%0];" ::"l"(pf));
   }
   const int E = __ldg(row_ptr + N);
-  const uint32_t hot_bar = smem_u32(bars + kStWarps * D);
-  const uint32_t head_bar0 = hot_bar + 8;                  // [warps]: "this warp's head slot is written"
+  const uint32_t hot_bar0 = smem_u32(bars + kStWarps * D);   // [8]: "the resident rows of group g have landed"
+  const uint32_t head_bar0 = hot_bar0 + kStHotGroups * 8;    // [warps]: "this warp's head slot is written"
 
   if (tid < 16) s_part[tid] = 0;
   if (tid < kStWarps) flags[tid] = 0;
@@ -190,24 +198,35 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
 #pragma unroll
     for (int k = 0; k < D; ++k) mbar_init(smem_u32(bars + warp * D + k), 1);
     mbar_init(head_bar0 + warp * 8, 1);
-    if (warp == 0) mbar_init(hot_bar, 1);
+    if (warp == 0)
+      for (int gr = 0; gr < kStHotGroups; ++gr) mbar_init(hot_bar0 + gr * 8, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (!given_hot)
     for (int i = tid; i < kStMaxR2 + 256; i += kStThreads) cnt[i] = 0;
   for (int i = tid; i < kStMaxR2 / 4; i += kStThreads) reinterpret_cast<uint32_t*>(slot_of)[i] = 0u;
   __syncthreads();
+  // resident rows (slot sl holds relation row_of(sl)) -> shared memory, one warp; slot sl lands on the barrier of group
+  // sl / kHotPerGroup, so an edge waits only for its own group and the edge loop starts before the table is complete.
+  // Every group barrier gets its one arrival (an empty group completes at once).
+  auto load_hot = [&](int n_hot, auto row_of) {
+    if (lane < kStHotGroups) {
+      const int rows = min(max(n_hot - lane * Cfg::kHotPerGroup, 0), Cfg::kHotPerGroup);
+      st_expect_tx(hot_bar0 + lane * 8, (uint32_t)rows * 1600u);
+    }
+    __syncwarp();
+    for (int sl = lane; sl < n_hot; sl += 32)
+      st_bulk_g2s(smem_u32(st_smem + Cfg::kOffHot + sl * 1600), W + (int64_t)row_of(sl) * 400, 1600,
+                  hot_bar0 + (sl / Cfg::kHotPerGroup) * 8);
+  };
   // ---- hot rows from the caller's list: fetched while the partition search runs --------------------------------------------
   if (given_hot && warp == 1) {
-    const int n_hot = min(n_hot_arg, Cfg::kHot);
-    if (lane == 0) st_expect_tx(hot_bar, (uint32_t)n_hot * 1600u);
-    __syncwarp();
-    for (int sl = lane; sl < n_hot; sl += 32) {
+    load_hot(min(n_hot_arg, Cfg::kHot), [&](int sl) {
       const int r = __ldg(hot_rel + sl);
       const bool ok = r >= 0 && r < R2;                    // an id outside the table is ignored (its slot holds row 0, unused)
       if (ok) slot_of[r] = (uint8_t)(sl + 1);
-      st_bulk_g2s(smem_u32(st_smem + Cfg::kOffHot + sl * 1600), W + (int64_t)(ok ? r : 0) * 400, 1600, hot_bar);
-    }
+      return ok ? r : 0;
+    });
   }
   // ---- CTA partition: destinations [A, A_next) own 1/gridDim of the edges (node-aligned).  Threads 0..255 look for
   //      lower_bound(row_ptr, T_c), threads 256..511 for lower_bound(row_ptr, T_c+1).  Invariant: the answer lies in
@@ -256,7 +275,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     const int64_t k_hi = (int64_t)ce + (int64_t)kStNodeCost * A_next, k_lo = (int64_t)(s_part[15] - 1) + (int64_t)kStNodeCost * (A_next - 1);
     if (s_part[15] && k_hi - tgt > tgt - k_lo) { --A_next; ce = s_part[15] - 1; }
   }
-  const long long t_part = dbg ? clock64() : 0;
+  if (dbg) stamp(1, clock64());
   const int n_rp = A_next - A + 1;
   const bool rp_in_smem = n_rp <= kStRpCap;
   auto rp = [&](int v) -> int { return rp_in_smem ? s_rp[v - A] : __ldg(row_ptr + v); };   // row_ptr[v], v in [A, A_next]
@@ -301,10 +320,11 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
       if (INDEXED) ld_s = __ldg(x_index + ld_s);
     }
   };
-  auto block_stage = [&](int b) {      // phase 3: to shared memory (hot rows are addressed by their byte offset / 16)
+  // phase 3: to shared memory.  Second word: a resident row's byte offset / 16 << 16 | its group, else the relation id
+  auto block_stage = [&](int b) {
     const int hs = use_hot ? (int)slot_of[ld_t] : 0;
     const int woff16 = hs ? (Cfg::kOffHot + (hs - 1) * 1600) >> 4 : 0;
-    my_idx[(b & 1) * 32 + lane] = make_int2(ld_s, ld_t | (woff16 << 16));
+    my_idx[(b & 1) * 32 + lane] = make_int2(ld_s, hs ? (woff16 << 16) | ((hs - 1) / Cfg::kHotPerGroup) : ld_t);
     if (BWD) my_sc[(b & 1) * 32 + lane] = ld_sc;
     __syncwarp();
   };
@@ -360,13 +380,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
       }
       __syncthreads();
     }
-    const int n_hot = min(s_part[9], Cfg::kHot);
-    if (warp == 1) {
-      if (lane == 0) st_expect_tx(hot_bar, (uint32_t)n_hot * 1600u);
-      __syncwarp();
-      for (int sl = lane; sl < n_hot; sl += 32)
-        st_bulk_g2s(smem_u32(st_smem + Cfg::kOffHot + sl * 1600), W + (int64_t)hist[sl] * 400, 1600, hot_bar);
-    }
+    if (warp == 1) load_hot(min(s_part[9], Cfg::kHot), [&](int sl) { return hist[sl]; });
   }
   block_gather(0);
   __syncthreads();                     // s_rp, slot_of complete; the ring (= cnt / hist) may be overwritten from here on
@@ -376,15 +390,13 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   const uint32_t ring = st_opaque(smem_u32(st_smem + Cfg::kOffRing + warp * D * kStSlot));
   const uint32_t bar0 = st_opaque(smem_u32(bars + warp * D));
   const uint32_t idx_a = st_opaque(smem_u32(my_idx));        // entry of local edge k: idx_a + (k & 63) * 8
-  // copies of local edge k into ring slot `slot` (both warp-uniform)
+  // copy of local edge k's source row into ring slot `slot` (both warp-uniform)
   auto issue = [&](int k, int slot) {
     if (st_elect_one()) {
-      const uint2 ix = st_lds_u2(idx_a + (((uint32_t)k & 63u) << 3));
-      const bool cold = (ix.y >> 16) == 0;
-      const uint32_t bar = bar0 + slot * 8, dst = ring + slot * kStSlot;
-      st_expect_tx(bar, cold ? 2400u : 800u);
-      st_bulk_g2s(dst, X + (int64_t)(int)ix.x * 200, 800, bar);
-      if (cold) st_bulk_g2s(dst + 800, W + (int64_t)(ix.y & 0xffffu) * 400, 1600, bar);
+      const uint32_t src = st_lds_u32(idx_a + (((uint32_t)k & 63u) << 3));
+      const uint32_t bar = bar0 + slot * 8;
+      st_expect_tx(bar, 800u);
+      st_bulk_g2s(ring + slot * kStSlot, X + (int64_t)(int)src * 200, 800, bar);
     }
   };
   // Everything above read graph structure, weights and the relation ranking only; from here on the kernel touches what
@@ -413,20 +425,20 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   float acc[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-  // self-loop row (already in Hout) and norm of the running destination, and of the next one (fetched one destination
-  // ahead: a run of degree-1 destinations would otherwise expose one global latency per destination)
-  float2 lp[4], lp_n[4];
-  float nrm = 1.f, nrm_n = 1.f;
+  // self-loop row (already in Hout) and norm of the running destination, fetched when it becomes the running one: its
+  // epilogue comes at least one edge later, and one edge of a warp outlasts a load (32 warps take turns on the SM)
+  float2 lp[4];
+  float nrm = 1.f;
 #pragma unroll
-  for (int k = 0; k < 4; ++k) lp[k] = lp_n[k] = make_float2(0.f, 0.f);
-  auto fetch_dest = [&](int v, float2 (&l)[4], float& nr) {
+  for (int k = 0; k < 4; ++k) lp[k] = make_float2(0.f, 0.f);
+  auto fetch_dest = [&](int v) {
     if (v < A_next) {
       if (HAS_LOOP) {
 #pragma unroll
         for (int k = 0; k < 4; ++k)
-          if (k < 3 || tail4) l[k] = *reinterpret_cast<const float2*>(Hout + (int64_t)v * 200 + 2 * (lane + 32 * k));
+          if (k < 3 || tail4) lp[k] = *reinterpret_cast<const float2*>(Hout + (int64_t)v * 200 + 2 * (lane + 32 * k));
       }
-      if (!BWD) nr = __ldg(norm + v);
+      if (!BWD) nrm = __ldg(norm + v);
     }
   };
   auto epilogue = [&](int v) {         // registers -> global, fused norm / self-loop / activation
@@ -462,23 +474,20 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     ++cur;
     cur_beg = cur_end;
     cur_end = cur < A_next ? rp(cur + 1) : ce;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) lp[k] = lp_n[k];
-    nrm = nrm_n;
-    fetch_dest(cur + 1, lp_n, nrm_n);              // (rows of destinations without edges are fetched too: harmless)
+    fetch_dest(cur);                               // (rows of destinations without edges are fetched too: harmless)
   };
-  if (!continued) fetch_dest(cur, lp, nrm);
-  fetch_dest(cur + 1, lp_n, nrm_n);
+  if (!continued) fetch_dest(cur);
 
-  if (use_hot) mbar_wait(hot_bar, 0);
-  const uint32_t ring_l8 = st_opaque(ring + 8 * lane), ring_l16 = st_opaque(ring + 800 + 16 * lane);
+  const uint32_t ring_l8 = st_opaque(ring + 8 * lane);
   const uint32_t smem_l16 = st_opaque(smem_u32(st_smem) + 16 * lane);
+  const float* w_l4 = W + 4 * lane;                         // lane's first block of a cold relation row
+  uint32_t hot_seen = 0;                                     // bit g: this warp has seen hot group g complete
   const uint32_t sc_a = BWD ? st_opaque(smem_u32(my_sc)) : 0u;
   uint32_t parity = 0;
   // index blocks: load -> dependent loads -> stage, spread over the block so that no load is waited for
   constexpr int kP1 = (kBlk / D / 3) * D, kP2 = (2 * (kBlk / D) / 3) * D;
   int phase_at = kP1, phase = 0, blk = 0;
-  const long long t_loop = dbg ? clock64() : 0;
+  if (dbg) stamp(2, clock64());
   for (int g = 0; g < n; g += D) {     // one pass over the ring: slot numbers are compile-time constants
     if (g == phase_at) {
       if (phase == 0) { block_gather(blk + 1); phase_at += kP2 - kP1; phase = 1; }
@@ -490,17 +499,28 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
       const int i = g + slot;
       if (i < n) {
         while (e0 + i >= cur_end) advance();       // warp-uniform: the running destination is complete
-        const uint32_t woff16 = st_lds_u32(idx_a + (((uint32_t)i & 63u) << 3) + 4) >> 16;
-        const uint32_t wa = woff16 ? smem_l16 + (woff16 << 4) : ring_l16 + slot * kStSlot;
+        const uint32_t wsel = st_lds_u32(idx_a + (((uint32_t)i & 63u) << 3) + 4);
+        const uint32_t woff16 = wsel >> 16;
         const float sc = BWD ? __uint_as_float(st_lds_u32(sc_a + (((uint32_t)i & 63u) << 2))) : 1.f;
-        st_wait(bar0 + slot * 8, parity);
         float2 h[4];
         float4 w[4];
+        w[3] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (woff16) {                  // resident row: wait for its group once per warp
+          const uint32_t grp = wsel & 0xffffu;
+          if (!((hot_seen >> grp) & 1u)) { mbar_wait(hot_bar0 + grp * 8, 0); hot_seen |= 1u << grp; }
+          const uint32_t wa = smem_l16 + (woff16 << 4);
+          w[0] = st_lds_f4<0>(wa); w[1] = st_lds_f4<512>(wa); w[2] = st_lds_f4<1024>(wa);
+          if (tail4) w[3] = st_lds_f4<1536>(wa);
+        } else {                       // cold row: straight from L2 into registers, in flight while the source row is awaited
+          const float* wr = w_l4 + (int64_t)(int)wsel * 400;
+          w[0] = ldg_f4(wr); w[1] = ldg_f4(wr + 128); w[2] = ldg_f4(wr + 256);
+          if (tail4) w[3] = ldg_f4(wr + 384);
+        }
+        st_wait(bar0 + slot * 8, parity);
         h[0] = st_lds_f2<slot * kStSlot>(ring_l8);       h[1] = st_lds_f2<slot * kStSlot + 256>(ring_l8);
         h[2] = st_lds_f2<slot * kStSlot + 512>(ring_l8);
-        w[0] = st_lds_f4<0>(wa); w[1] = st_lds_f4<512>(wa); w[2] = st_lds_f4<1024>(wa);
-        h[3] = make_float2(0.f, 0.f); w[3] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (tail4) { h[3] = st_lds_f2<slot * kStSlot + 768>(ring_l8); w[3] = st_lds_f4<1536>(wa); }
+        h[3] = make_float2(0.f, 0.f);
+        if (tail4) h[3] = st_lds_f2<slot * kStSlot + 768>(ring_l8);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const float x = BWD ? h[k].x * sc : h[k].x, y = BWD ? h[k].y * sc : h[k].y;
@@ -524,7 +544,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     }
     parity ^= 1u;
   }
-  const long long t_done = dbg ? clock64() : 0;
+  if (dbg) stamp(3, clock64());
   // ---- end of the range ------------------------------------------------------------------------------------------------------
   if (n > 0) {
     if (cur_end <= e1) {
@@ -571,12 +591,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
       }
     }
   }
-  if (dbg && lane == 0) {
-    long long g_exit;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g_exit));
-    long long* d = dbg + ((int64_t)blockIdx.x * kStWarps + warp) * 8;
-    d[0] = t_entry; d[1] = t_part; d[2] = t_loop; d[3] = t_done; d[4] = clock64(); d[5] = g_entry; d[6] = g_exit; d[7] = n;
-  }
+  if (dbg) { stamp(4, clock64()); stamp(6, global_timer()); stamp(7, n); }
 }
 
 }  // namespace renet

@@ -18,7 +18,7 @@ dev = torch.device('cuda:0')
 L, P = _lib.lib(), _lib.ptr
 T = {'icews18': 240, 'gdelt': 2138, 'icews14': 181}[preset]
 tkg = synthetic.SyntheticTKG(preset, seed=999, num_timestamps=T)
-WARPS = int(os.environ.get('RENET_STREAM_WARPS', '16'))      # warps per CTA of the configuration under test (RENET_STREAM_CFG)
+CTAS, MAX_WARPS = 132, 32      # the grid is one CTA per SM; no configuration runs more than 32 warps (StCfg)
 R2 = 2 * tkg.num_r
 gs = hoststore.GraphStore(tkg.graph_dict)
 hs = hoststore.HistoryStore(tkg.s_hist, tkg.s_hist_t, tkg.quads[:, 0], gs)
@@ -36,7 +36,8 @@ if use_hot:
     for gg in tkg.graph_dict.values():
         freq += np.bincount(np.asarray(gg.type_s, dtype=np.int64), minlength=R2)
     hot = torch.from_numpy(np.argsort(-freq, kind='stable')[:128].astype(np.int32)).to(dev)
-buf = torch.zeros(148 * WARPS * 8, dtype=torch.int64, device=dev)
+# room for the largest configuration: the kernel writes CTAS x (its warps) records of 8 stamps, packed from the start
+buf = torch.zeros(CTAS * MAX_WARPS * 8, dtype=torch.int64, device=dev)
 stream = _lib.stream()
 
 
@@ -57,8 +58,12 @@ L.renet_debug_stream_timing(P(buf))
 call()
 torch.cuda.synchronize()
 L.renet_debug_stream_timing(None)
-d = buf.cpu().numpy().reshape(148, WARPS, 8).astype(np.float64)
-clk = 1.965e3          # cycles per us at the maximum SM clock
+rec = buf.cpu().numpy().reshape(-1, 8)
+n_rec = int(np.count_nonzero(rec[:, 5]))         # every warp stamps its entry time: records written = CTAs x warps
+assert n_rec % CTAS == 0 and not rec[n_rec:].any(), 'unexpected stamp layout (%d records)' % n_rec
+WARPS = n_rec // CTAS
+d = rec[:n_rec].reshape(CTAS, WARPS, 8).astype(np.float64)
+clk = 1.98e3           # cycles per us at the maximum SM clock (H100 SXM: clocks.max.sm 1980 MHz)
 g0 = d[:, :, 5].min()
 print('N %d E %d; kernel span by the global timer: %.1f us (first entry -> last exit)' % (g.N, g.E, (d[:, :, 6].max() - g0) / 1e3))
 print('CTA entry skew: max %.1f us; CTA exit (last warp) - global start: min %.1f / median %.1f / max %.1f us' % (
