@@ -84,6 +84,10 @@ void set_stream_debug_buffer(long long* p);   // debug: per-warp time stamps of 
 
 // tensor-core (wgmma) GEMM engine building blocks (umma_gemm.cu); gemm_mode() == 1 selects the engine
 int gemm_mode();
+// An indexed wgmma product of at least this many rows (EPI 0, no accumulate, resident panel) computes each distinct index
+// once and copies the rows out (umma_gemm_dedup).  Layer 1's self-loop (N ~ 33 k nodes, ~20 % distinct entities) is above
+// it; layer 2's read-out rows (S ~ 8.5 k, all distinct) are below, where the extra passes would be pure cost (DESIGN §5).
+constexpr int64_t kDedupMinRows = 16384;
 int64_t umma_packed_bytes(int N, int K);
 void set_gemm_debug_buffer(long long* p);     // debug: per-warpgroup time stamps of the packed GEMM kernels (umma_gemm.cu)
 // packed-weight cache (umma_gemm.cu): persistent device buffer for this key, or nullptr when caching is off; *hit says

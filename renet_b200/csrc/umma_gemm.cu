@@ -567,6 +567,8 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
 // (rows gathered through a_index), the next chunk's while the current chunk's wgmma group runs, and splits them into
 // hi/lo in registers.  Each output element sees the k-steps in order and per k-step the products hi*hi, lo*hi, hi*lo, with
 // the same operands as in the streaming kernel.
+// The row count is M, or *m_dev when m_dev is set (the deduplicated self-loop product below, whose row count is only known
+// on the device): the tiles are split from it, so the work scales with the rows actually present, not with the grid.
 // ======================================================================================================
 constexpr int R_MAX_CHUNKS = 7;                      // K <= 224: the whole panel fits in shared memory
 constexpr int R_CHUNK = 2 * P_BH_BYTES;              // 26624: hi and lo halves of one 32-wide K chunk of a panel
@@ -578,21 +580,22 @@ template <bool INDEXED>
 __global__ void __launch_bounds__(R_THREADS, 1)
 umma_gemm_resident_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_index, int64_t lda,
                           const uint8_t* __restrict__ Bp, float* __restrict__ C, int64_t ldc, const float* __restrict__ bias,
-                          int64_t M, int N, int K, int n_chunks, int accumulate, int64_t batch_a, int64_t batch_bp,
-                          int64_t batch_c, int n_panels, long long* dbg) {
+                          int64_t M, const int32_t* __restrict__ m_dev, int N, int K, int n_chunks, int accumulate,
+                          int64_t batch_a, int64_t batch_bp, int64_t batch_c, int n_panels, long long* dbg) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t sb = raw + ((1024 - (raw & 1023)) & 1023);       // swizzle atoms need 1024-byte alignment
   const uint32_t bar0 = sb + R_MAX_CHUNKS * R_CHUNK;
   const int tid = threadIdx.x;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+  if (m_dev != nullptr) M = *m_dev;
   // panel p owns the CTAs [p*G/P, (p+1)*G/P) (G >= P: at least one each)
   const int G = gridDim.x, b = blockIdx.x;
   const int p = (int)(((int64_t)(b + 1) * n_panels - 1) / G);
   const int cta0 = (int)((int64_t)p * G / n_panels), ncta = (int)((int64_t)(p + 1) * G / n_panels) - cta0;
   const int64_t n_rt = (M + 63) / 64;
   const int64_t t_begin = (int64_t)(b - cta0) * n_rt / ncta, t_end = (int64_t)(b - cta0 + 1) * n_rt / ncta;
-  // the launcher's grid gives every CTA a tile; a CTA without one must not issue copies it would never wait for
+  // with a device row count (or rows < CTAs) a CTA may have no tile: it must not issue copies it would never wait for
   if (t_begin == t_end) return;
   const int n_tiles = (N + UN - 1) / UN;
   const int half = p & 1, nt = (p >> 1) % n_tiles, zb = (p >> 1) / n_tiles;
@@ -689,6 +692,64 @@ umma_gemm_resident_kernel(const float* __restrict__ A, const int32_t* __restrict
   ts.finish(2);
 }
 
+// ======================================================================================================
+// Deduplicated indexed product: C[n] = A[a_index[n]] @ B for n < M, each distinct row computed once
+//
+// Layer 1's self-loop row of node n is ent_embeds[node_ent[n]] @ W_loop: it depends on the node's entity only, and the batched
+// graph is a disjoint union of per-timestamp components, so an entity is a node in many of them (ICEWS18: ~20 % of the
+// nodes carry a distinct entity, DESIGN §3).  Three launches, no host synchronisation:
+//   1. dedup_insert_kernel: inserts a_index[0..M) into an open-addressing table of 2^bits >= 2M 64-bit keys
+//      (epoch << 32 | index).  The epoch changes every call, so a key of an earlier call reads as a free slot and the table
+//      is never cleared.  The thread whose CAS claims a slot takes u = atomicAdd(count) and writes uniq[u] and slot_row[slot];
+//      every thread records its slot in link[n].  The slot is read before the CAS, so the many inserts of a hub entity
+//      mostly find the key without an atomic.  The order of the u is not deterministic; no output bit depends on it.
+//   2. umma_gemm_resident_kernel over the U = count distinct rows (indexed through uniq) into a compact P[U, N], its row count
+//      read from the device.  Every distinct row sees the same operands, k-steps and product order as it would undeduplicated.
+//   3. dedup_expand_kernel: C[n] = P[slot_row[link[n]]], one warp per node, 128-bit loads and stores; it also zeroes count
+//      for the next call (the GEMM, its only reader, has completed).
+// ======================================================================================================
+__device__ __forceinline__ uint32_t dedup_hash(uint32_t v, int bits) { return (v * 0x9E3779B1u) >> (32 - bits); }
+
+__global__ void __launch_bounds__(256)
+dedup_insert_kernel(const int32_t* __restrict__ a_index, int64_t M, unsigned long long* __restrict__ table, int bits,
+                    uint32_t epoch, int32_t* __restrict__ slot_row, int32_t* __restrict__ uniq, int32_t* __restrict__ link,
+                    int32_t* __restrict__ count) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= M) return;
+  const uint32_t v = (uint32_t)__ldg(a_index + n);
+  const unsigned long long key = ((unsigned long long)epoch << 32) | v;
+  const uint32_t mask = (1u << bits) - 1;
+  uint32_t s = dedup_hash(v, bits);
+  for (;;) {
+    const unsigned long long cur = __ldcg(table + s);
+    if (cur == key) break;
+    if ((uint32_t)(cur >> 32) == epoch) {          // another index of this call: linear probing
+      s = (s + 1) & mask;
+      continue;
+    }
+    if (atomicCAS(table + s, cur, key) == cur) {   // the slot was free in this call and is ours
+      const int32_t u = atomicAdd(count, 1);
+      uniq[u] = (int32_t)v;
+      slot_row[s] = u;
+      break;
+    }
+    // another thread claimed the slot first: read it again
+  }
+  link[n] = (int32_t)s;
+}
+
+__global__ void __launch_bounds__(256)
+dedup_expand_kernel(const float* __restrict__ P, const int32_t* __restrict__ slot_row, const int32_t* __restrict__ link,
+                    float* __restrict__ C, int64_t ldc, int64_t M, int N, int32_t* __restrict__ count) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) *count = 0;
+  const int64_t n = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (n >= M) return;
+  const int64_t u = __ldg(slot_row + __ldg(link + n));
+  const float* src = P + u * N;
+  float* dst = C + n * ldc;
+  for (int j = 4 * (threadIdx.x & 31); j < N; j += 128) st_f4(dst + j, ldg_f4(src + j));
+}
+
 }  // namespace
 
 // Returns 1 if the shape was taken by the tensor-core path (launch enqueued), 0 if the caller should
@@ -764,6 +825,124 @@ int umma_pack_b(const float* B, int64_t sk, int64_t sn, int N, int K, void* Bp, 
   return RENET_OK;
 }
 
+// The resident-panel kernel serves EPI 0 products without split-K whose panels fit shared memory and the grid.
+static bool resident_ok(int N, int K, int batch) {
+  return (K + P_BK - 1) / P_BK <= R_MAX_CHUNKS && batch * ((N + UN - 1) / UN) * 2 <= kNumSMs;
+}
+
+// M rows, or *m_dev rows (m_dev != nullptr; M is then an upper bound that sizes the grid)
+static int launch_resident(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
+                           const float* bias, int64_t M, const int32_t* m_dev, int N, int K, bool accumulate, int batch,
+                           int64_t batch_a, int64_t batch_bp, int64_t batch_c, cudaStream_t stream) {
+  static bool attr_r = false;
+  if (!attr_r) {
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_resident_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, R_SMEM));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_resident_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, R_SMEM));
+    attr_r = true;
+  }
+  const int n_chunks = (K + P_BK - 1) / P_BK, n_panels = batch * ((N + UN - 1) / UN) * 2;
+  // every panel gets at least one CTA; a CTA never holds more than one panel
+  const int64_t n_work = (int64_t)n_panels * ((M + 63) / 64);
+  const unsigned grid = (unsigned)(n_work < kNumSMs ? n_work : kNumSMs);
+  if (a_index)
+    umma_gemm_resident_kernel<true><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
+                                                                        m_dev, N, K, n_chunks, accumulate, batch_a, batch_bp,
+                                                                        batch_c, n_panels, g_gemm_dbg);
+  else
+    umma_gemm_resident_kernel<false><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
+                                                                         m_dev, N, K, n_chunks, accumulate, batch_a, batch_bp,
+                                                                         batch_c, n_panels, g_gemm_dbg);
+  RENET_CHECK_LAUNCH("umma_gemm_resident_kernel");
+  return RENET_OK;
+}
+
+// ---- workspace of the deduplicated product (umma_gemm_dedup) ----------------------------------------------------------
+// One per (device, stream): renet_encode_fwd runs GEMMs on a side stream concurrently with the caller's, and each stream's
+// calls are ordered among themselves, so a workspace is only ever used by the work of its own stream.  It grows on demand
+// with stream-ordered allocations: the old block is freed behind the work already queued on that stream.  The table is
+// zeroed once when allocated (epoch 0 = empty) and never again.
+namespace {
+struct DedupWs {
+  int device;
+  cudaStream_t stream;
+  float* P;                        // [rows, N] compact distinct-row products
+  int64_t p_floats;
+  uint8_t* ix;                     // table [slots] u64 | slot_row [slots] | uniq [rows] | link [rows] | count
+  int64_t rows, slots;
+  uint32_t epoch;
+};
+std::mutex g_dedup_mu;
+std::vector<DedupWs> g_dedup;
+constexpr int kDedupMaxStreams = 8;
+}  // namespace
+
+static int dedup_workspace(int64_t M, int N, cudaStream_t stream, DedupWs* out) {
+  std::lock_guard<std::mutex> lk(g_dedup_mu);
+  int dev = 0;
+  RENET_CHECK_CUDA(cudaGetDevice(&dev));
+  DedupWs* w = nullptr;
+  for (auto& e : g_dedup)
+    if (e.device == dev && e.stream == stream) w = &e;
+  if (w == nullptr) {
+    if ((int)g_dedup.size() >= kDedupMaxStreams) {   // bounded: drop the oldest (its stream may be gone: free synchronously)
+      RENET_CHECK_CUDA(cudaDeviceSynchronize());
+      RENET_CHECK_CUDA(cudaFree(g_dedup.front().P));
+      RENET_CHECK_CUDA(cudaFree(g_dedup.front().ix));
+      g_dedup.erase(g_dedup.begin());
+    }
+    g_dedup.push_back(DedupWs{dev, stream, nullptr, 0, nullptr, 0, 0, 0});
+    w = &g_dedup.back();
+  }
+  const int64_t rows = (M + 16383) / 16384 * 16384;        // grow in steps: batches vary by a few thousand rows
+  if (M * N > w->p_floats) {
+    if (w->P) RENET_CHECK_CUDA(cudaFreeAsync(w->P, stream));
+    w->P = nullptr;
+    w->p_floats = 0;
+    RENET_CHECK_CUDA(cudaMallocAsync((void**)&w->P, (size_t)(rows * N) * sizeof(float), stream));
+    w->p_floats = rows * N;
+  }
+  if (M > w->rows) {
+    if (w->ix) RENET_CHECK_CUDA(cudaFreeAsync(w->ix, stream));
+    w->ix = nullptr;
+    w->rows = w->slots = 0;
+    int64_t s = 1;
+    while (s < 2 * rows) s <<= 1;
+    const size_t bytes = (size_t)s * 12 + (size_t)rows * 8 + 16;
+    RENET_CHECK_CUDA(cudaMallocAsync((void**)&w->ix, bytes, stream));
+    RENET_CHECK_CUDA(cudaMemsetAsync(w->ix, 0, bytes, stream));   // empty table, count = 0
+    w->rows = rows;
+    w->slots = s;
+  }
+  if (++w->epoch == 0) {                                    // wrapped: keys of epoch 0 would read as this call's
+    RENET_CHECK_CUDA(cudaMemsetAsync(w->ix, 0, (size_t)w->slots * 8, stream));
+    w->epoch = 1;
+  }
+  *out = *w;
+  return RENET_OK;
+}
+
+// C[n] = A[a_index[n]] @ Bp (+bias) for n < M through the distinct rows of a_index (see the kernels above)
+static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
+                           const float* bias, int64_t M, int N, int K, cudaStream_t stream) {
+  DedupWs w;
+  int rc = dedup_workspace(M, N, stream, &w);
+  if (rc) return rc;
+  int bits = 1;
+  while ((int64_t(1) << bits) < 2 * M) ++bits;              // the table of this call: 2^bits >= 2M of the w.slots
+  unsigned long long* table = reinterpret_cast<unsigned long long*>(w.ix);
+  int32_t* slot_row = reinterpret_cast<int32_t*>(w.ix + w.slots * 8);
+  int32_t* uniq = slot_row + w.slots;
+  int32_t* link = uniq + w.rows;
+  int32_t* count = link + w.rows;
+  dedup_insert_kernel<<<(unsigned)((M + 255) / 256), 256, 0, stream>>>(a_index, M, table, bits, w.epoch, slot_row, uniq, link,
+                                                                       count);
+  RENET_CHECK_LAUNCH("dedup_insert_kernel");
+  if ((rc = launch_resident(A, uniq, lda, Bp, w.P, N, bias, M, count, N, K, false, 1, 0, 0, 0, stream))) return rc;
+  dedup_expand_kernel<<<(unsigned)((M + 7) / 8), 256, 0, stream>>>(w.P, slot_row, link, C, ldc, M, N, count);
+  RENET_CHECK_LAUNCH("dedup_expand_kernel");
+  return RENET_OK;
+}
+
 // C[b] (+)= A[b] @ Bpacked[b] (+bias[b]) for b < batch; strides in elements (A, C) / bytes (Bp).
 // epi_mode 1 / 2: fused cross-entropy epilogues (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
@@ -783,27 +962,10 @@ int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, 
   if (k_splits < 1) k_splits = 1;
   if (k_splits > n_chunks) k_splits = n_chunks;
   while (k_splits > 1 && ((n_chunks + k_splits - 1) / k_splits) * (k_splits - 1) >= n_chunks) --k_splits;   // no empty split
-  const int n_panels = batch * n_tiles * 2;
-  if (epi_mode == 0 && k_splits == 1 && n_chunks <= R_MAX_CHUNKS && n_panels <= kNumSMs) {
-    static bool attr_r = false;
-    if (!attr_r) {
-      RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_resident_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, R_SMEM));
-      RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_resident_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, R_SMEM));
-      attr_r = true;
-    }
-    // every panel gets at least one CTA; a CTA never holds more than one panel
-    const int64_t n_work = (int64_t)n_panels * ((M + 63) / 64);
-    const unsigned grid = (unsigned)(n_work < kNumSMs ? n_work : kNumSMs);
-    if (a_index)
-      umma_gemm_resident_kernel<true><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
-                                                                          N, K, n_chunks, accumulate, batch_a, batch_bp,
-                                                                          batch_c, n_panels, g_gemm_dbg);
-    else
-      umma_gemm_resident_kernel<false><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
-                                                                           N, K, n_chunks, accumulate, batch_a, batch_bp,
-                                                                           batch_c, n_panels, g_gemm_dbg);
-    RENET_CHECK_LAUNCH("umma_gemm_resident_kernel");
-    return 1;
+  if (epi_mode == 0 && k_splits == 1 && resident_ok(N, K, batch)) {
+    const int rc = launch_resident(A, a_index, lda, Bp, C, ldc, bias, M, nullptr, N, K, accumulate, batch, batch_a, batch_bp,
+                                   batch_c, stream);
+    return rc ? rc : 1;
   }
   // persistent grid: at most one CTA per SM, each walking a balanced range of 128 x 104 work units
   const int64_t n_units = (M + UM - 1) / UM * (2 * n_tiles) * batch * k_splits;
@@ -846,7 +1008,10 @@ int umma_gemm_nn_try(const float* A, const int32_t* a_index, int64_t lda, const 
     void* Bp = cached ? cached : g_scratch;
     int rc = hit ? 0 : umma_pack_b(B, ldb, 1, N, K, Bp, 0, stream);
     if (rc) return rc;
-    rc = umma_gemm_prepacked(A, a_index, lda, Bp, C, ldc, bias, M, N, K, accumulate, 1, 0, 0, 0, stream);
+    if (a_index != nullptr && !accumulate && M >= kDedupMinRows && resident_ok(N, K, 1))
+      rc = umma_gemm_dedup(A, a_index, lda, Bp, C, ldc, bias, M, N, K, stream);
+    else
+      rc = umma_gemm_prepacked(A, a_index, lda, Bp, C, ldc, bias, M, N, K, accumulate, 1, 0, 0, 0, stream);
     return rc ? rc : 1;
   }
   const bool ok = (K % UKC == 0) && K >= UKC && (N % 8 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) &&
