@@ -133,6 +133,36 @@ int renet_debug_stream_timing(void* buffer);
  * on operand barriers, in wgmma waits, in the epilogue and splitting A, work items and role).  Pass NULL to switch it off;
  * never set in production code. */
 int renet_debug_gemm_timing(void* buffer);
+/* DEBUG / TEST ONLY (tests/gemm_contract_check.py): one product of the dense-GEMM engine in any argument form the library's
+ * callers use, on the kernel the engine's dispatch picks or on a forced one, reporting which kernel ran, so that a test can
+ * compare every path with a reference and pin the path that served each case.  A pass-through with no arithmetic of its
+ * own; never used in production code.
+ *   form RENET_GEMM_FORM_NN:        C (+)= A[a_index] @ B (+bias)   A rows through a_index (or NULL); row-major operands
+ *                                   with lda / ldb / ldc; kernel 0 dispatches exactly as the self-loop, GRU and RGCN products
+ *                                   do (engine, scratch buffer, shape and alignment decide).
+ *   form RENET_GEMM_FORM_PREPACKED: for b < batch: B + b*batch_b (row-major [K,N], ldb) is packed into `workspace`, then
+ *                                   C + b*batch_c (+)= (A + b*batch_a)[a_index] @ B_b (+ bias + b*N), all entries in one
+ *                                   tensor-core launch: the form of the GRU's projections and recurrent products.
+ *   form RENET_GEMM_FORM_TN:        C (+)= A[a_index]^T @ B   A [K, lda] (M columns used), B [K, ldb]; no bias; without
+ *                                   accumulate C is zeroed first (weight gradients).
+ * kernel: 0, or a renet_gemm_kernel to force.  A forced kernel must be able to serve the form and its preconditions must hold
+ * (for example RESIDENT needs K <= 224, LEGACY K % 40 == 0, FFMA_TILED 16-byte aligned operands); otherwise the call returns
+ * RENET_ERR_INVALID_ARG before anything is launched.  The packed kernels (PREPACKED form, or STREAMING / RESIDENT / DEDUP
+ * forced in the NN form) pack B into `workspace`: batch * ceil(N/200) * ceil(K/32) * 53248 bytes, 128-byte aligned.
+ * Returns the renet_gemm_kernel that computed C (0 when M == 0), or a negative renet_status. */
+typedef enum { RENET_GEMM_FORM_NN = 0, RENET_GEMM_FORM_PREPACKED = 1, RENET_GEMM_FORM_TN = 2 } renet_gemm_form;
+typedef enum {
+  RENET_GEMM_FFMA_TILED = 1,   /* fp32 FFMA, register-tiled (tn form: split-K)                                       */
+  RENET_GEMM_FFMA_NAIVE = 2,   /* fp32 FFMA, one thread per output (unaligned operands, N or K not multiples of 4)   */
+  RENET_GEMM_LEGACY = 3,       /* wgmma 3xTF32 staging B itself: no scratch buffer; K % 40 == 0                       */
+  RENET_GEMM_STREAMING = 4,    /* wgmma 3xTF32, packed B streamed per 128 x 104 unit, persistent, warp-specialised  */
+  RENET_GEMM_RESIDENT = 5,     /* wgmma 3xTF32, packed B panel resident in shared memory (K <= 224)                  */
+  RENET_GEMM_DEDUP = 6         /* RESIDENT over the distinct rows of a_index, copied out to every row               */
+} renet_gemm_kernel;
+int renet_debug_gemm(int32_t form, int32_t kernel, const float* A, const int32_t* a_index, int64_t lda, const float* B,
+                     int64_t ldb, float* C, int64_t ldc, const float* bias, int64_t M, int32_t N, int64_t K, int32_t accumulate,
+                     int32_t batch, int64_t batch_a, int64_t batch_b, int64_t batch_c, void* workspace, int64_t workspace_bytes,
+                     void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * RGCN block-diagonal layer, backward (autograd of the above; the reference relies on

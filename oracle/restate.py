@@ -260,7 +260,7 @@ def packed_inputs(H2, readout, seq_len, s_tem, r_tem, ent, rel, glob_rows):
     X3 = [H2[readout] | ent[s] | glob[t]], returned sequence-major [S,4h],[S,3h] plus the packed
     (time-major) permutation that pack_padded_sequence(batch_first=True) applies, and batch_sizes."""
     rows = H2[readout]
-    seq_of_row = torch.repeat_interleave(torch.arange(len(seq_len)), torch.as_tensor(seq_len))
+    seq_of_row = torch.repeat_interleave(torch.arange(len(seq_len)), torch.as_tensor(seq_len)).to(s_tem.device)
     e = ent[s_tem[seq_of_row]]
     r = rel[r_tem[seq_of_row]]
     X4 = torch.cat((rows, e, r, glob_rows), dim=1)
@@ -306,13 +306,14 @@ def gru_final_hidden(X, seq_len, w_ih, w_hh, b_ih, b_hh):
 
 
 def gru_final_hidden_batched(X, seq_len, w_ih, w_hh, b_ih, b_hh):
-    """Same as gru_final_hidden, vectorised over sequences per time step (lengths sorted desc)."""
+    """Same as gru_final_hidden, vectorised over sequences per time step (lengths sorted desc).  Runs in X's dtype on X's
+    device."""
     seq_len = np.asarray(seq_len, dtype=np.int64)
     Q = len(seq_len)
     hdim = w_hh.shape[1]
-    starts = torch.as_tensor(np.concatenate(([0], np.cumsum(seq_len)[:-1])).astype(np.int64))
+    starts = torch.as_tensor(np.concatenate(([0], np.cumsum(seq_len)[:-1])).astype(np.int64), device=X.device)
     gi_all = X @ w_ih.t() + b_ih
-    h = torch.zeros(Q, hdim, dtype=X.dtype)
+    h = torch.zeros(Q, hdim, dtype=X.dtype, device=X.device)
     for t in range(int(seq_len.max()) if Q else 0):
         n_act = int((seq_len > t).sum())
         gi = gi_all[starts[:n_act] + t]

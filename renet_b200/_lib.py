@@ -30,6 +30,8 @@ SIGNATURES = {
     'renet_rgcn_gather': (ctypes.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     'renet_debug_stream_timing': (ctypes.c_int, [_vp]),
     'renet_debug_gemm_timing': (ctypes.c_int, [_vp]),
+    'renet_debug_gemm': (ctypes.c_int, [_i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i64, _i32, _i32,
+                                        _i64, _i64, _i64, _vp, _i64, _vp]),
     'renet_rgcn_gather_hot': (ctypes.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp]),
     'renet_rgcn_block_bwd': (ctypes.c_int, [_vp] * 17 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),
     'renet_rgcn_bipartite_bwd': (ctypes.c_int, [_vp] * 14 + [_i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),

@@ -18,6 +18,9 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+static thread_local int g_last_gemm_kernel = 0;
+void note_gemm_kernel(int kernel) { g_last_gemm_kernel = kernel; }
+int last_gemm_kernel() { return g_last_gemm_kernel; }
 
 // launchers defined in the other translation units
 int launch_rgcn_gather(const float* H, const int32_t* h_index, const float* W, const int32_t* row_ptr,
@@ -222,6 +225,16 @@ int renet_debug_stream_timing(void* buffer) {
 int renet_debug_gemm_timing(void* buffer) {
   set_gemm_debug_buffer(static_cast<long long*>(buffer));
   return RENET_OK;
+}
+
+int renet_debug_gemm(int32_t form, int32_t kernel, const float* A, const int32_t* a_index, int64_t lda, const float* B,
+                     int64_t ldb, float* C, int64_t ldc, const float* bias, int64_t M, int32_t N, int64_t K, int32_t accumulate,
+                     int32_t batch, int64_t batch_a, int64_t batch_b, int64_t batch_c, void* workspace, int64_t workspace_bytes,
+                     void* stream) {
+  note_gemm_kernel(0);
+  const int rc = debug_gemm(form, kernel, A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate != 0, batch, batch_a,
+                            batch_b, batch_c, workspace, workspace_bytes, (cudaStream_t)stream);
+  return rc ? rc : last_gemm_kernel();
 }
 
 int renet_rgcn_block_fwd(const float* H, const int32_t* h_index, const float* W, const float* Wloop,

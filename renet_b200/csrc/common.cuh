@@ -11,6 +11,9 @@ namespace renet {
 
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
+// every dense-GEMM launcher records which kernel (renet_gemm_kernel) it ran; renet_debug_gemm reports it
+void note_gemm_kernel(int kernel);
+int last_gemm_kernel();
 
 #define RENET_CHECK_ARG(cond, ...)                  \
   do {                                              \
@@ -67,9 +70,19 @@ __device__ __forceinline__ void red_add_f4(float* p, float4 v) {
 int sgemm_nn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
              int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
              cudaStream_t stream);
+// The FFMA engine of sgemm_nn: the register-tiled kernel where sgemm_nn_tiled_ok holds (and naive is false), else one thread
+// per output
+bool sgemm_nn_tiled_ok(const float* A, int64_t lda, const float* B, int64_t ldb, const float* C, int64_t ldc,
+                       const float* bias, int32_t N, int32_t K);
+int sgemm_nn_ffma(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
+                  int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate, bool naive,
+                  cudaStream_t stream);
 // C[M,N] += / = A^T B with A [K,M] (rows of A optionally through a_index), B [K,N]:  C = A^T @ B
+// (split-K tiled kernel where sgemm_tn_tiled_ok holds and naive is false, else one thread per output)
+bool sgemm_tn_tiled_ok(const float* A, int64_t lda, const float* B, int64_t ldb, const float* C, int64_t ldc, int32_t M,
+                       int32_t N);
 int sgemm_tn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
-             int64_t ldc, int32_t M, int32_t N, int64_t K, bool accumulate, cudaStream_t stream);
+             int64_t ldc, int32_t M, int32_t N, int64_t K, bool accumulate, cudaStream_t stream, bool naive = false);
 // C[M,N] = A[M,K] @ B^T with B [N,K]
 int sgemm_nt(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
              int64_t M, int32_t N, int32_t K, bool accumulate, cudaStream_t stream);
@@ -115,5 +128,9 @@ int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, 
 int umma_gemm_prepacked(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                         const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                         int64_t batch_bp, int64_t batch_c, cudaStream_t stream);
+// renet_debug_gemm without its kernel id (umma_gemm.cu)
+int debug_gemm(int form, int kernel, const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
+               int64_t ldc, const float* bias, int64_t M, int N, int64_t K, bool accumulate, int batch, int64_t batch_a,
+               int64_t batch_b, int64_t batch_c, void* ws, int64_t ws_bytes, cudaStream_t stream);
 
 }  // namespace renet

@@ -628,16 +628,17 @@ int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_g
     if (ext_X3 == nullptr) { w_ih3 = w_ih4; w_hh3 = w_hh4; }
   }
   int rc;
-  RENET_CHECK_CUDA(cudaMemsetAsync(b.dbias, 0, 12 * h * sizeof(float), stream));
-  RENET_CHECK_CUDA(cudaMemsetAsync(b.dWhh, 0, (int64_t)h * 6 * h * sizeof(float), stream));
-  RENET_CHECK_CUDA(cudaMemsetAsync(b.dPT, 0, T * 6 * h * sizeof(float), stream));
-  if (dH2 != nullptr) RENET_CHECK_CUDA(cudaMemsetAsync(dH2, 0, N * h * sizeof(float), stream));
+  // checked before anything is written: a rejected call used to have zeroed dH2 already
   int last = 0;
   while (last < max_len && host_batch_sizes[last] > 0) ++last;
   if (last > kMaxLenWs) {
     set_error("renet_gru_bwd: max_len %d exceeds the supported %d", last, kMaxLenWs);
     return RENET_ERR_INVALID_ARG;
   }
+  RENET_CHECK_CUDA(cudaMemsetAsync(b.dbias, 0, 12 * h * sizeof(float), stream));
+  RENET_CHECK_CUDA(cudaMemsetAsync(b.dWhh, 0, (int64_t)h * 6 * h * sizeof(float), stream));
+  RENET_CHECK_CUDA(cudaMemsetAsync(b.dPT, 0, T * 6 * h * sizeof(float), stream));
+  if (dH2 != nullptr) RENET_CHECK_CUDA(cudaMemsetAsync(dH2, 0, N * h * sizeof(float), stream));
   const int64_t hs_stride = Q * 2 * h;
   const int64_t gh_stride = Q * 6 * h;
   // tensor-core engine: W_hh of both encoders packed ONCE as the B operand of dHprev += dGH @ W_hh (B[k][n] = w_hh[k*h + n])

@@ -254,6 +254,33 @@ int set_gemm_mode(int m) {
   return prev;
 }
 
+bool sgemm_nn_tiled_ok(const float* A, int64_t lda, const float* B, int64_t ldb, const float* C, int64_t ldc,
+                       const float* bias, int32_t N, int32_t K) {
+  return (K % 4 == 0) && (N % 4 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) && aligned16(A) &&
+         aligned16(B) && aligned16(C) && (bias == nullptr || aligned16(bias));
+}
+
+int sgemm_nn_ffma(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
+                  int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate, bool naive,
+                  cudaStream_t stream) {
+  if (!naive && sgemm_nn_tiled_ok(A, lda, B, ldb, C, ldc, bias, N, K)) {
+    dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((N + BN - 1) / BN));
+    if (a_index)
+      sgemm_nn_kernel<true><<<grid, NT, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
+    else
+      sgemm_nn_kernel<false><<<grid, NT, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
+    RENET_CHECK_LAUNCH("sgemm_nn_kernel");
+    note_gemm_kernel(RENET_GEMM_FFMA_TILED);
+  } else {
+    int64_t total = M * N;
+    sgemm_nn_naive<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M,
+                                                                       N, K, accumulate);
+    RENET_CHECK_LAUNCH("sgemm_nn_naive");
+    note_gemm_kernel(RENET_GEMM_FFMA_NAIVE);
+  }
+  return RENET_OK;
+}
+
 int sgemm_nn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
              int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
              cudaStream_t stream) {
@@ -262,41 +289,32 @@ int sgemm_nn(const float* A, const int32_t* a_index, int64_t lda, const float* B
     const int r = umma_gemm_nn_try(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
     if (r != 0) return r < 0 ? r : RENET_OK;
   }
-  const bool fast = (K % 4 == 0) && (N % 4 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) &&
-                    aligned16(A) && aligned16(B) && aligned16(C) && (bias == nullptr || aligned16(bias));
-  if (fast) {
-    dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((N + BN - 1) / BN));
-    if (a_index)
-      sgemm_nn_kernel<true><<<grid, NT, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
-    else
-      sgemm_nn_kernel<false><<<grid, NT, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
-    RENET_CHECK_LAUNCH("sgemm_nn_kernel");
-  } else {
-    int64_t total = M * N;
-    sgemm_nn_naive<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M,
-                                                                       N, K, accumulate);
-    RENET_CHECK_LAUNCH("sgemm_nn_naive");
-  }
-  return RENET_OK;
+  return sgemm_nn_ffma(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, false, stream);
+}
+
+bool sgemm_tn_tiled_ok(const float* A, int64_t lda, const float* B, int64_t ldb, const float* C, int64_t ldc, int32_t M,
+                       int32_t N) {
+  return (M % 4 == 0) && (N % 4 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) && aligned16(A) &&
+         aligned16(B) && aligned16(C);
 }
 
 int sgemm_tn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
-             int64_t ldc, int32_t M, int32_t N, int64_t K, bool accumulate, cudaStream_t stream) {
+             int64_t ldc, int32_t M, int32_t N, int64_t K, bool accumulate, cudaStream_t stream, bool naive) {
   if (M <= 0 || N <= 0) return RENET_OK;
   if (!accumulate) RENET_CHECK_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, N * sizeof(float), M, stream));
   if (K <= 0) return RENET_OK;
-  const bool fast = (M % 4 == 0) && (N % 4 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) &&
-                    aligned16(A) && aligned16(B) && aligned16(C);
-  if (fast) {
+  if (!naive && sgemm_tn_tiled_ok(A, lda, B, ldb, C, ldc, M, N)) {
     dim3 grid((M + TN_BM - 1) / TN_BM, (N + TN_BN - 1) / TN_BN, (unsigned)((K + TN_KCHUNK - 1) / TN_KCHUNK));
     if (a_index)
       sgemm_tn_splitk_kernel<true><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, M, N, K);
     else
       sgemm_tn_splitk_kernel<false><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, M, N, K);
     RENET_CHECK_LAUNCH("sgemm_tn_splitk_kernel");
+    note_gemm_kernel(RENET_GEMM_FFMA_TILED);
   } else {
     sgemm_tn_naive<<<(M * N + 255) / 256, 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, M, N, K);
     RENET_CHECK_LAUNCH("sgemm_tn_naive");
+    note_gemm_kernel(RENET_GEMM_FFMA_NAIVE);
   }
   return RENET_OK;
 }

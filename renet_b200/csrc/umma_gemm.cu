@@ -853,6 +853,73 @@ static int launch_resident(const float* A, const int32_t* a_index, int64_t lda, 
                                                                          m_dev, N, K, n_chunks, accumulate, batch_a, batch_bp,
                                                                          batch_c, n_panels, g_gemm_dbg);
   RENET_CHECK_LAUNCH("umma_gemm_resident_kernel");
+  note_gemm_kernel(RENET_GEMM_RESIDENT);
+  return RENET_OK;
+}
+
+// persistent grid: at most one CTA per SM, each walking a balanced range of 128 x 104 work units
+static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
+                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
+                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,
+                            cudaStream_t stream) {
+  static bool attr2 = false;
+  if (!attr2) {
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(0)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(0)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(1)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(2)));
+    attr2 = true;
+  }
+  const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
+  const int64_t n_units = (M + UM - 1) / UM * (2 * n_tiles) * batch * k_splits;
+  const unsigned grid = (unsigned)(n_units < kNumSMs ? n_units : kNumSMs);
+#define RENET_UMMA_LAUNCH(IDX, EP)                                                                                       \
+  umma_gemm_packed_kernel<IDX, EP><<<grid, P_THREADS, p_smem(EP), stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, \
+                                                                           M, N, K, n_chunks, accumulate, batch_a, batch_bp,  \
+                                                                           batch_c, epi, k_splits, split_c, n_units, \
+                                                                           g_gemm_dbg)
+  if (epi_mode == 1) RENET_UMMA_LAUNCH(false, 1);
+  else if (epi_mode == 2) RENET_UMMA_LAUNCH(false, 2);
+  else if (a_index) RENET_UMMA_LAUNCH(true, 0);
+  else RENET_UMMA_LAUNCH(false, 0);
+#undef RENET_UMMA_LAUNCH
+  RENET_CHECK_LAUNCH("umma_gemm_packed_kernel");
+  note_gemm_kernel(RENET_GEMM_STREAMING);
+  return RENET_OK;
+}
+
+// The first tensor-core kernel (umma_gemm_nn_kernel): stages B itself, so it needs no scratch buffer, but K % 40 == 0.
+static bool legacy_ok(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
+                      int N, int K) {
+  const bool aligned = ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C) |
+                         reinterpret_cast<uintptr_t>(bias)) & 15) == 0;
+  return (K % UKC == 0) && K >= UKC && (N % 8 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) && aligned;
+}
+
+static int launch_legacy(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
+                         int64_t ldc, const float* bias, int64_t M, int N, int K, bool accumulate, cudaStream_t stream) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e1 = cudaFuncSetAttribute(umma_gemm_nn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t e2 = cudaFuncSetAttribute(umma_gemm_nn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    if (e1 != cudaSuccess || e2 != cudaSuccess) {
+      set_error("cudaFuncSetAttribute(umma_gemm_nn_kernel) failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+      return RENET_ERR_CUDA;
+    }
+    attr_set = true;
+  }
+  dim3 grid((unsigned)((M + UM - 1) / UM), (unsigned)((N + UN - 1) / UN));
+  if (a_index)
+    umma_gemm_nn_kernel<true><<<grid, UTHREADS, SMEM_BYTES, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
+  else
+    umma_gemm_nn_kernel<false><<<grid, UTHREADS, SMEM_BYTES, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("launch of umma_gemm_nn_kernel failed: %s", cudaGetErrorString(e));
+    return RENET_ERR_CUDA;
+  }
+  count_launch();
+  note_gemm_kernel(RENET_GEMM_LEGACY);
   return RENET_OK;
 }
 
@@ -940,6 +1007,7 @@ static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, 
   if ((rc = launch_resident(A, uniq, lda, Bp, w.P, N, bias, M, count, N, K, false, 1, 0, 0, 0, stream))) return rc;
   dedup_expand_kernel<<<(unsigned)((M + 7) / 8), 256, 0, stream>>>(w.P, slot_row, link, C, ldc, M, N, count);
   RENET_CHECK_LAUNCH("dedup_expand_kernel");
+  note_gemm_kernel(RENET_GEMM_DEDUP);
   return RENET_OK;
 }
 
@@ -950,15 +1018,7 @@ int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, 
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,
                            cudaStream_t stream) {
   if (M <= 0) return RENET_OK;
-  static bool attr2 = false;
-  if (!attr2) {
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(0)));
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(0)));
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(1)));
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(2)));
-    attr2 = true;
-  }
-  const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
+  const int n_chunks = (K + P_BK - 1) / P_BK;
   if (k_splits < 1) k_splits = 1;
   if (k_splits > n_chunks) k_splits = n_chunks;
   while (k_splits > 1 && ((n_chunks + k_splits - 1) / k_splits) * (k_splits - 1) >= n_chunks) --k_splits;   // no empty split
@@ -967,21 +1027,9 @@ int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, 
                                    batch_c, stream);
     return rc ? rc : 1;
   }
-  // persistent grid: at most one CTA per SM, each walking a balanced range of 128 x 104 work units
-  const int64_t n_units = (M + UM - 1) / UM * (2 * n_tiles) * batch * k_splits;
-  const unsigned grid = (unsigned)(n_units < kNumSMs ? n_units : kNumSMs);
-#define RENET_UMMA_LAUNCH(IDX, EP)                                                                                       \
-  umma_gemm_packed_kernel<IDX, EP><<<grid, P_THREADS, p_smem(EP), stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, \
-                                                                           M, N, K, n_chunks, accumulate, batch_a, batch_bp,  \
-                                                                           batch_c, epi, k_splits, split_c, n_units, \
-                                                                           g_gemm_dbg)
-  if (epi_mode == 1) RENET_UMMA_LAUNCH(false, 1);
-  else if (epi_mode == 2) RENET_UMMA_LAUNCH(false, 2);
-  else if (a_index) RENET_UMMA_LAUNCH(true, 0);
-  else RENET_UMMA_LAUNCH(false, 0);
-#undef RENET_UMMA_LAUNCH
-  RENET_CHECK_LAUNCH("umma_gemm_packed_kernel");
-  return k_splits;      // > 0: the number of K-splits actually used (1 = C holds the result)
+  const int rc = launch_streaming(A, a_index, lda, Bp, C, ldc, bias, M, N, K, accumulate, batch, batch_a, batch_bp, batch_c,
+                                  epi_mode, epi, k_splits, split_c, stream);
+  return rc ? rc : k_splits;      // > 0: the number of K-splits actually used (1 = C holds the result)
 }
 
 int umma_gemm_prepacked(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
@@ -1014,31 +1062,71 @@ int umma_gemm_nn_try(const float* A, const int32_t* a_index, int64_t lda, const 
       rc = umma_gemm_prepacked(A, a_index, lda, Bp, C, ldc, bias, M, N, K, accumulate, 1, 0, 0, 0, stream);
     return rc ? rc : 1;
   }
-  const bool ok = (K % UKC == 0) && K >= UKC && (N % 8 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) &&
-                  M >= 64 && aligned;
-  if (!ok) return 0;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e1 = cudaFuncSetAttribute(umma_gemm_nn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    cudaError_t e2 = cudaFuncSetAttribute(umma_gemm_nn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e1 != cudaSuccess || e2 != cudaSuccess) {
-      set_error("cudaFuncSetAttribute(umma_gemm_nn_kernel) failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
-      return RENET_ERR_CUDA;
-    }
-    attr_set = true;
+  if (M < 64 || !legacy_ok(A, lda, B, ldb, C, ldc, bias, N, K)) return 0;
+  const int rc = launch_legacy(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
+  return rc ? rc : 1;
+}
+
+// renet_debug_gemm (include/renet_b200.h): every argument form of the engine, on the kernel the dispatch picks or on a forced
+// one.  Every precondition is checked before anything is launched.
+int debug_gemm(int form, int kernel, const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
+               int64_t ldc, const float* bias, int64_t M, int N, int64_t K, bool accumulate, int batch, int64_t batch_a,
+               int64_t batch_b, int64_t batch_c, void* ws, int64_t ws_bytes, cudaStream_t stream) {
+  RENET_CHECK_ARG(form >= RENET_GEMM_FORM_NN && form <= RENET_GEMM_FORM_TN, "renet_debug_gemm: unknown form %d", form);
+  RENET_CHECK_ARG(kernel >= 0 && kernel <= RENET_GEMM_DEDUP, "renet_debug_gemm: unknown kernel %d", kernel);
+  RENET_CHECK_ARG(M >= 0 && N > 0 && K > 0 && K < (int64_t(1) << 31) && lda > 0 && ldb > 0 && ldc > 0 && batch >= 1 &&
+                      (batch == 1 || form == RENET_GEMM_FORM_PREPACKED),
+                  "renet_debug_gemm: bad shape");
+  RENET_CHECK_ARG(A && B && C, "renet_debug_gemm: null pointer");
+  const bool ffma = kernel == RENET_GEMM_FFMA_TILED || kernel == RENET_GEMM_FFMA_NAIVE;
+  if (form == RENET_GEMM_FORM_TN) {
+    RENET_CHECK_ARG(kernel == 0 || ffma, "renet_debug_gemm: the tn form runs on the FFMA kernels only");
+    RENET_CHECK_ARG(M < (int64_t(1) << 31) && bias == nullptr, "renet_debug_gemm: the tn form takes M < 2^31 and no bias");
+    RENET_CHECK_ARG(kernel != RENET_GEMM_FFMA_TILED || sgemm_tn_tiled_ok(A, lda, B, ldb, C, ldc, (int)M, N),
+                    "renet_debug_gemm: the tiled tn kernel needs 16-byte aligned operands and M, N, ld* multiples of 4");
+    if (M == 0) return RENET_OK;
+    return sgemm_tn(A, a_index, lda, B, ldb, C, ldc, (int)M, N, K, accumulate, stream, kernel == RENET_GEMM_FFMA_NAIVE);
   }
-  dim3 grid((unsigned)((M + UM - 1) / UM), (unsigned)((N + UN - 1) / UN));
-  if (a_index)
-    umma_gemm_nn_kernel<true><<<grid, UTHREADS, SMEM_BYTES, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
-  else
-    umma_gemm_nn_kernel<false><<<grid, UTHREADS, SMEM_BYTES, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("launch of umma_gemm_nn_kernel failed: %s", cudaGetErrorString(e));
-    return RENET_ERR_CUDA;
+  if (form == RENET_GEMM_FORM_NN && (kernel == 0 || ffma || kernel == RENET_GEMM_LEGACY)) {
+    RENET_CHECK_ARG(kernel != RENET_GEMM_FFMA_TILED || sgemm_nn_tiled_ok(A, lda, B, ldb, C, ldc, bias, N, (int)K),
+                    "renet_debug_gemm: the tiled FFMA kernel needs 16-byte aligned operands and N, K, ld* multiples of 4");
+    RENET_CHECK_ARG(kernel != RENET_GEMM_LEGACY || legacy_ok(A, lda, B, ldb, C, ldc, bias, N, (int)K),
+                    "renet_debug_gemm: the legacy kernel needs K %% 40 == 0, N %% 8 == 0, ld* %% 4 == 0, 16-byte aligned operands");
+    if (M == 0) return RENET_OK;
+    if (kernel == 0) return sgemm_nn(A, a_index, lda, B, ldb, C, ldc, bias, M, N, (int)K, accumulate, stream);
+    if (ffma) return sgemm_nn_ffma(A, a_index, lda, B, ldb, C, ldc, bias, M, N, (int)K, accumulate,
+                                   kernel == RENET_GEMM_FFMA_NAIVE, stream);
+    return launch_legacy(A, a_index, lda, B, ldb, C, ldc, bias, M, N, (int)K, accumulate, stream);
   }
-  count_launch();
-  return 1;
+  // the packed kernels: B (batch of them) packed into the caller's workspace
+  RENET_CHECK_ARG(kernel == 0 || kernel == RENET_GEMM_STREAMING || kernel == RENET_GEMM_RESIDENT ||
+                      (kernel == RENET_GEMM_DEDUP && form == RENET_GEMM_FORM_NN),
+                  "renet_debug_gemm: kernel %d cannot serve form %d", kernel, form);
+  const bool aligned = ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(C) | reinterpret_cast<uintptr_t>(bias)) &
+                        15) == 0;
+  RENET_CHECK_ARG(aligned && umma_shape_ok(N, (int)K) && lda % 4 == 0 && ldc % 4 == 0 && batch_a % 4 == 0 && batch_c % 4 == 0,
+                  "renet_debug_gemm: the packed kernels need 16-byte aligned A / C / bias, K %% 4 == 0, N %% 8 == 0 and "
+                  "lda, ldc, batch strides multiples of 4");
+  RENET_CHECK_ARG((kernel != RENET_GEMM_RESIDENT && kernel != RENET_GEMM_DEDUP) || resident_ok(N, (int)K, batch),
+                  "renet_debug_gemm: the resident kernel needs K <= %d and at most %d panels", R_MAX_CHUNKS * P_BK, kNumSMs);
+  RENET_CHECK_ARG(kernel != RENET_GEMM_DEDUP || (a_index != nullptr && !accumulate),
+                  "renet_debug_gemm: the deduplicated product needs an index and no accumulate");
+  const int64_t pb = umma_packed_bytes(N, (int)K);
+  RENET_CHECK_ARG(ws != nullptr && ws_bytes >= batch * pb && (reinterpret_cast<uintptr_t>(ws) & 127) == 0,
+                  "renet_debug_gemm: the workspace needs %lld bytes, 128-byte aligned", (long long)(batch * pb));
+  if (M == 0) return RENET_OK;
+  for (int b = 0; b < batch; ++b) {
+    const int rc = umma_pack_b(B + b * batch_b, ldb, 1, N, (int)K, static_cast<uint8_t*>(ws) + b * pb, 0, stream);
+    if (rc) return rc;
+  }
+  if (kernel == RENET_GEMM_DEDUP) return umma_gemm_dedup(A, a_index, lda, ws, C, ldc, bias, M, N, (int)K, stream);
+  if (kernel == RENET_GEMM_RESIDENT)
+    return launch_resident(A, a_index, lda, ws, C, ldc, bias, M, nullptr, N, (int)K, accumulate, batch, batch_a, pb, batch_c,
+                           stream);
+  if (kernel == RENET_GEMM_STREAMING)
+    return launch_streaming(A, a_index, lda, ws, C, ldc, bias, M, N, (int)K, accumulate, batch, batch_a, pb, batch_c, 0,
+                            EpiArgs{}, 1, 0, stream);
+  return umma_gemm_prepacked(A, a_index, lda, ws, C, ldc, bias, M, N, (int)K, accumulate, batch, batch_a, pb, batch_c, stream);
 }
 
 }  // namespace renet

@@ -248,7 +248,8 @@ def test_default_training_config_runs_on_our_kernels_only():
     assert all(np.isfinite(losses)) and losses[-1] < losses[0], losses
 
 
-@pytest.mark.parametrize('M,N,K', [(1024, 23033, 600), (1024, 256, 400), (37, 1001, 24), (300, 199, 8)])
+@pytest.mark.parametrize('M,N,K', [(1024, 23033, 600), (1024, 256, 400), (37, 1001, 24), (300, 199, 8), (1024, 23033, 200),
+                                   (300, 460, 200)])
 def test_fused_decoder_cross_entropy_vs_torch_fp32(M, N, K):
     """renet_decoder_ce_fwd/_bwd (wgmma 3xTF32 GEMM with fused logsumexp epilogue, recompute-based backward) against a
     plain PyTorch fp64 reference of the same op (model.py:89-91,97-100): loss and all three gradients, including class
