@@ -46,6 +46,15 @@ int64_t renet_launch_count(void);
  * renet_set_gemm_engine returns the previous engine. */
 int renet_set_gemm_engine(int engine);
 int renet_get_gemm_engine(void);
+/* Deterministic mode, process-wide, default 0.  When on, every backward entry point (RGCN dH / dW / dW_loop, row
+ * scatter-add, GRU weight, bias and input gradients, with or without input dropout) sums each output element in an order
+ * fixed by its inputs and shapes, so repeated calls on identical inputs give bitwise identical results.  It costs extra
+ * passes over per-chunk partial sums and a stream-ordered scratch buffer per (device, stream), allocated with
+ * cudaMallocAsync on first use and grown on demand (the one exception to "nothing is allocated by the library").  When
+ * off, the reductions add with float atomics and the last bits of a gradient may vary from run to run.  The Python
+ * binding follows torch.use_deterministic_algorithms.  renet_set_deterministic returns the previous value. */
+int renet_set_deterministic(int on);
+int renet_get_deterministic(void);
 /* Packed-weight cache of the wgmma GEMM engine.   The engine consumes weights (self-loop matrices, GRU W_ih / W_hh)
  * in a packed shared-memory operand image; packing is a kernel launch per weight per call.  Declaring a weight
  * generation >= 0 promises that every weight passed by pointer is unchanged while the generation is unchanged: packed

@@ -20,6 +20,8 @@ SIGNATURES = {
     'renet_launch_count': (_i64, []),
     'renet_set_gemm_engine': (ctypes.c_int, [ctypes.c_int]),
     'renet_get_gemm_engine': (ctypes.c_int, []),
+    'renet_set_deterministic': (ctypes.c_int, [ctypes.c_int]),
+    'renet_get_deterministic': (ctypes.c_int, []),
     'renet_set_weight_generation': (ctypes.c_int, [_i64]),
     'renet_set_scratch': (ctypes.c_int, [_vp, _i64]),
     'renet_csr_workspace_bytes': (_i64, [_i64, _i64]),
@@ -108,15 +110,23 @@ def ptr(t):
 
 def stream():
     """The current CUDA stream of the current device as a raw handle.  (torch.cuda.current_stream() costs ~10 us of Python per
-    call -- device-index checks, a Stream object -- and the e2e path asks 18 times per step; the raw getter is ~0.3 us.)"""
+    call -- device-index checks, a Stream object -- and the e2e path asks 18 times per step; the raw getter is ~0.3 us.)
+
+    Every kernel call asks for its stream here, so this is also where the library's deterministic mode follows
+    torch.use_deterministic_algorithms(): the flag is read on every call and passed on when it has changed."""
     dev = torch._C._cuda_getDevice()
     if dev not in _scratch_ready:
         ensure_scratch(dev)
         _scratch_ready.add(dev)
+    det = torch.are_deterministic_algorithms_enabled()
+    if det != _deterministic[0]:
+        lib().renet_set_deterministic(int(det))
+        _deterministic[0] = det
     return ctypes.c_void_p(torch._C._cuda_getCurrentRawStream(dev))
 
 
 _scratch_ready = set()
+_deterministic = [False]       # the value last passed to renet_set_deterministic (the library starts at 0)
 
 
 def pinned_slots(pool, words):

@@ -131,6 +131,8 @@ const char* renet_last_error(void) { return g_err; }
 int64_t renet_launch_count(void) { return g_launches.load(); }
 int renet_set_gemm_engine(int engine) { return set_gemm_mode(engine); }
 int renet_get_gemm_engine(void) { return gemm_mode(); }
+int renet_set_deterministic(int on) { return set_deterministic(on); }
+int renet_get_deterministic(void) { return deterministic() ? 1 : 0; }
 int renet_set_weight_generation(int64_t generation) { renet::set_weight_generation(generation); return RENET_OK; }
 int renet_set_scratch(void* device_ptr, int64_t bytes) {
   RENET_CHECK_ARG(bytes >= 0 && (device_ptr != nullptr || bytes == 0), "renet_set_scratch: bad arguments");

@@ -65,6 +65,21 @@ __device__ __forceinline__ void red_add_f4(float* p, float4 v) {
                : "memory");
 }
 
+// deterministic mode (renet_set_deterministic): every gradient reduction of the training step sums in an order that depends
+// only on the inputs and shapes -- no float atomics, no order set by CTA scheduling (DESIGN §4)
+bool deterministic();
+int set_deterministic(int on);
+// Stream-ordered scratch of the deterministic reductions: one buffer per (device, stream), grown on demand with
+// cudaMallocAsync.  *out holds at least `bytes` until the next det_scratch call on the same stream.
+int det_scratch(int64_t bytes, cudaStream_t stream, void** out);
+// out[r * ldo + c] (+)= sum over s = 0, 1, ..., n_parts - 1 of parts[s * stride + r * cols + c]   (r < rows, c < cols)
+int launch_sum_partials(const float* parts, int n_parts, int64_t stride, int64_t rows, int cols, float* out, int64_t ldo,
+                        bool accumulate, cudaStream_t stream);
+// dst[key_i] += src[i * ld ...][0 .. d) for i < n_rows, key_i = outer ? outer[index[i]] : index[i]; the rows of each key are
+// added in ascending i (stable radix sort by key, then one warp per distinct key)
+int scatter_add_rows_det(const float* src, int64_t ld, const int32_t* index, const int32_t* outer, float* dst, int64_t n_rows,
+                         int d, cudaStream_t stream);
+
 // internal (non-exported) launchers shared between translation units -------------------------------
 // C[M,N] (ldc) = A[M,K] (rows optionally through a_index; lda) @ B[K,N] (ldb) [+ bias[N]] [+ C if accumulate]
 int sgemm_nn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,

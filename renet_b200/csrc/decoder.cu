@@ -31,16 +31,6 @@ __global__ void ce_reduce_kernel(const float* __restrict__ pmax, const float* __
   loss_rows[r] = l - tlogit[r];
 }
 
-// out[i] (+)= sum_s parts[s][i]
-__global__ void sum_partials_kernel(const float* __restrict__ parts, int n_parts, int64_t stride, int64_t n,
-                                    float* __restrict__ out, int accumulate) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float s = accumulate ? out[i] : 0.f;
-  for (int k = 0; k < n_parts; ++k) s += parts[(int64_t)k * stride + i];
-  out[i] = s;
-}
-
 // db[c] += sum_r dT[c, r]   (one warp per class)
 __global__ void rowsum_accum_kernel(const float* __restrict__ dT, int64_t ldT, int64_t M, int N, float* __restrict__ db) {
   const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -152,8 +142,7 @@ int renet_decoder_ce_bwd(const float* X, const float* W, const float* bias, cons
   const int used = umma_gemm_prepacked_ex(w.dlog, nullptr, w.ldE, w.Wkp, w.parts, K, nullptr, M, K, N, false, 1, 0, 0, 0, 0, none,
                                           kSplits, M * (int64_t)K, stream);
   if (used < 0) return used;
-  sum_partials_kernel<<<(unsigned)((M * K + 255) / 256), 256, 0, stream>>>(w.parts, used, M * (int64_t)K, M * (int64_t)K, dX, 0);
-  RENET_CHECK_LAUNCH("sum_partials_kernel");
+  if ((rc = launch_sum_partials(w.parts, used, M * (int64_t)K, M, K, dX, K, false, stream))) return rc;
   // 3. dW += dlogits^T @ X: A = dT [|E|, M], B[k][n] = X[k*K + n]
   if ((rc = umma_pack_b(X, K, 1, K, (int)M, w.Xp, 0, stream))) return rc;
   rc = umma_gemm_prepacked_ex(w.dT, nullptr, w.ldT, w.Xp, dW, K, nullptr, N, K, (int)M, true, 1, 0, 0, 0, 0, none, 1, 0, stream);

@@ -183,6 +183,24 @@ __global__ void unpack_inputs_dropout_kernel(const float* __restrict__ dX4, cons
   }
 }
 
+// deterministic mode: the same masked gradients, summed per element in place into dX4 = [S, 4h] ([row | ent | rel | glob]),
+// whose four column blocks are then scattered by scatter_add_rows_det
+__global__ void dropout_grad_rows_kernel(float* dX4, const float* __restrict__ dX3, int64_t S, int h, float p, uint64_t seed) {
+  const int64_t row = blockIdx.x;
+  if (row >= S) return;
+  const float inv = 1.f / (1.f - p);
+  const uint64_t base4 = (uint64_t)row * 4 * h, base3 = (uint64_t)S * 4 * h + (uint64_t)row * 3 * h;
+  for (int c = threadIdx.x; c < 4 * h; c += blockDim.x) {
+    const int part = c / h, k = c - part * h;
+    float gsum = dX4[row * 4 * h + c] * dropout_scale(base4 + c, seed, p, inv);
+    if (part != 2) {
+      const int c3 = (part == 3 ? 2 * h : part * h) + k;
+      gsum += dX3[row * 3 * h + c3] * dropout_scale(base3 + c3, seed, p, inv);
+    }
+    dX4[row * 4 * h + c] = gsum;
+  }
+}
+
 // PQ[q, :] = b_ih (both encoders) for every sequence
 __global__ void fill_rows_kernel(const float* __restrict__ v, float* __restrict__ out, int64_t rows, int cols) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -521,7 +539,9 @@ __global__ void gru_gate_bwd_kernel(const float* __restrict__ GI, const float* _
   dHprev[(int64_t)q * per_q + c] = dh * z;
 }
 
-// out[c] += sum_{r < n} X[r*ld + c]   (grid: column blocks x row chunks; one atomic per thread)
+// out[c] += sum_{r < n} X[r*ld + c]   (grid: column blocks x row chunks; one atomic per thread).  DET: each row chunk
+// stores its sum to out = partials [gridDim.y][cols] instead
+template <bool DET = false>
 __global__ void colsum_accum_kernel(const float* __restrict__ X, int64_t ld, int64_t n, int cols,
                                     float* __restrict__ out, int rows_per_block) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -530,7 +550,23 @@ __global__ void colsum_accum_kernel(const float* __restrict__ X, int64_t ld, int
   const int64_t r1 = min(n, r0 + rows_per_block);
   float s = 0.f;
   for (int64_t r = r0; r < r1; ++r) s += X[r * ld + c];
-  atomicAdd(out + c, s);
+  if (DET) out[(int64_t)blockIdx.y * cols + c] = s;
+  else atomicAdd(out + c, s);
+}
+
+int colsum_accum(const float* X, int64_t ld, int64_t n, int cols, float* out, int rows_per_block, cudaStream_t stream) {
+  const dim3 grid((cols + 127) / 128, (unsigned)((n + rows_per_block - 1) / rows_per_block));
+  if (!deterministic()) {
+    colsum_accum_kernel<<<grid, 128, 0, stream>>>(X, ld, n, cols, out, rows_per_block);
+    RENET_CHECK_LAUNCH("colsum_accum_kernel");
+    return RENET_OK;
+  }
+  void* parts = nullptr;
+  int rc = det_scratch((int64_t)grid.y * cols * (int64_t)sizeof(float), stream, &parts);
+  if (rc) return rc;
+  colsum_accum_kernel<true><<<grid, 128, 0, stream>>>(X, ld, n, cols, static_cast<float*>(parts), rows_per_block);
+  RENET_CHECK_LAUNCH("colsum_accum_kernel");
+  return launch_sum_partials(static_cast<float*>(parts), (int)grid.y, cols, 1, cols, out, cols, true, stream);
 }
 
 // dPQ[q, :] = sum over the rows of sequence q of dGI[row, :]
@@ -675,11 +711,7 @@ int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_g
   }
   if (last > 0) {
     // db_hh += colsum(dGH) over every step (rows of finished sequences are zeros)
-    const int rpb = 256;
-    const int64_t rows = (int64_t)last * Q;
-    dim3 grid((6 * h + 127) / 128, (unsigned)((rows + rpb - 1) / rpb));
-    colsum_accum_kernel<<<grid, 128, 0, stream>>>(b.dGH, 6 * h, rows, 6 * h, b.dbias + 6 * h, rpb);
-    RENET_CHECK_LAUNCH("colsum_accum_kernel");
+    if ((rc = colsum_accum(b.dGH, 6 * h, (int64_t)last * Q, 6 * h, b.dbias + 6 * h, 256, stream))) return rc;
   }
   if (last > 1) {
     // dWhh[k, o] += sum over steps t >= 1 of Hprev_t[:, k]^T dGH_t[:, o]: ONE K-long reduction per encoder over all steps
@@ -688,12 +720,7 @@ int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_g
     if ((rc = sgemm_tn(f.Hs + hs_stride + h, nullptr, 2 * h, b.dGH + gh_stride + 3 * h, 6 * h, b.dWhh + 3 * h, 6 * h, h, 3 * h, K, true, stream))) return rc;
   }
   // ---- biases of the input projection: every row carries b_ih once ------------------------------------
-  {
-    const int rpb = 128;
-    dim3 grid((6 * h + 127) / 128, (unsigned)((S + rpb - 1) / rpb));
-    colsum_accum_kernel<<<grid, 128, 0, stream>>>(b.dGI, 6 * h, S, 6 * h, b.dbias, rpb);
-    RENET_CHECK_LAUNCH("colsum_accum_kernel");
-  }
+  if ((rc = colsum_accum(b.dGI, 6 * h, S, 6 * h, b.dbias, 128, stream))) return rc;
   if (dropout) {
     // ---- input-dropout path: dW_ih = dGI^T @ Xd (the masked inputs the forward pass kept), dXd = dGI @ W_ih, then the
     //      masks are regenerated and the gradients scattered to H2 rows / ent / rel / glob -------------------------------------
@@ -707,7 +734,14 @@ int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_g
       if ((rc = sgemm_tn(b.dGI + 3 * h, nullptr, 6 * h, X3, k3, dw_ih3, k3, 3 * h, k3, S, true, stream))) return rc;
       if ((rc = sgemm_nn(b.dGI + 3 * h, nullptr, 6 * h, w_ih3, k3, dX3, k3, nullptr, S, k3, 3 * h, false, stream))) return rc;
     }
-    if (!dense) {
+    if (!dense && deterministic()) {
+      dropout_grad_rows_kernel<<<(unsigned)S, 128, 0, stream>>>(b.dX4, b.dX3, S, h, p_drop, seed);
+      RENET_CHECK_LAUNCH("dropout_grad_rows_kernel");
+      if ((rc = scatter_add_rows_det(b.dX4, 4 * h, readout, nullptr, dH2, S, h, stream))) return rc;
+      if ((rc = scatter_add_rows_det(b.dX4 + h, 4 * h, row_seq, seq_s, d_ent, S, h, stream))) return rc;
+      if ((rc = scatter_add_rows_det(b.dX4 + 2 * h, 4 * h, row_seq, seq_r, d_rel, S, h, stream))) return rc;
+      if (d_glob != nullptr && (rc = scatter_add_rows_det(b.dX4 + 3 * h, 4 * h, row_glob, nullptr, d_glob, S, h, stream))) return rc;
+    } else if (!dense) {
       unpack_inputs_dropout_kernel<<<(unsigned)S, 128, 0, stream>>>(b.dX4, b.dX3, readout, row_glob, row_seq, seq_s, seq_r, dH2,
                                                                    d_ent, d_rel, d_glob, S, h, p_drop, seed);
       RENET_CHECK_LAUNCH("unpack_inputs_dropout_kernel");
@@ -724,9 +758,7 @@ int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_g
     float* outs[4] = {db_ih4, db_ih3, db_hh4, db_hh3};
     for (int k = 0; k < 4; ++k) {
       if (outs[k] == nullptr) continue;                     // single GRU: the idle second encoder has no gradients
-      dim3 grid((3 * h + 127) / 128, 1);
-      colsum_accum_kernel<<<grid, 128, 0, stream>>>(b.dbias + (int64_t)k * 3 * h, 3 * h, 1, 3 * h, outs[k], 1);
-      RENET_CHECK_LAUNCH("colsum_accum_kernel");
+      if ((rc = colsum_accum(b.dbias + (int64_t)k * 3 * h, 3 * h, 1, 3 * h, outs[k], 1, stream))) return rc;
     }
     return RENET_OK;
   }
@@ -761,12 +793,8 @@ int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_g
   // biases: dbias = [db_ih4 | db_ih3 | db_hh4 | db_hh3]
   {
     float* outs[4] = {db_ih4, db_ih3, db_hh4, db_hh3};
-    for (int k = 0; k < 4; ++k) {
-      const int rpb = 1;
-      dim3 grid((3 * h + 127) / 128, 1);
-      colsum_accum_kernel<<<grid, 128, 0, stream>>>(b.dbias + (int64_t)k * 3 * h, 3 * h, 1, 3 * h, outs[k], rpb);
-      RENET_CHECK_LAUNCH("colsum_accum_kernel");
-    }
+    for (int k = 0; k < 4; ++k)
+      if ((rc = colsum_accum(b.dbias + (int64_t)k * 3 * h, 3 * h, 1, 3 * h, outs[k], 1, stream))) return rc;
   }
   // ---- input gradients: dX = dG @ W_ih[:, block] ------------------------------------------------------------------
   // read-out rows -> dH2

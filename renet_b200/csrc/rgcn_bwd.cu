@@ -54,25 +54,33 @@ __global__ void transpose_kernel(const float* __restrict__ src, float* __restric
 
 // dH[u] = dH[u] (loop part, already there when HAS_LOOP) + sum over out-edges of W^T (norm[dst] P[dst]).
 // Tile kernel (rgcn_tile.cuh): 16 source rows per CTA, the out-edge range split evenly
-// over the warps; transposed 2x2 blocks, per-edge scale norm[dst].
-template <bool HAS_LOOP>
+// over the warps; transposed 2x2 blocks, per-edge scale norm[dst].  DET: the warps hand partial rows over through
+// TileHeads (rgcn_tile.cuh) instead of shared-memory atomics, as in the forward tile kernel.
+template <bool HAS_LOOP, bool DET = false>
 __global__ void __launch_bounds__(kTileWarps * 32)
 rgcn_dh_tile_kernel(const float* __restrict__ P, const float* __restrict__ W, const int32_t* __restrict__ t_row_ptr,
                     const int32_t* __restrict__ t_col_dst, const int32_t* __restrict__ t_col_type,
                     const float* __restrict__ norm, float* __restrict__ dH, int N) {
   __shared__ __align__(16) float agg[kTileNodes][200];
+  __shared__ __align__(16) float head[DET ? kTileWarps : 1][200];
+  __shared__ int head_mask[kTileNodes];
   __shared__ int s_rp[kTileNodes + 1];
   const int tid = threadIdx.x;
   const int v0 = blockIdx.x * kTileNodes;
   const int nv = min(kTileNodes, N - v0);
-  for (int i = tid; i < kTileNodes * 200; i += kTileWarps * 32) (&agg[0][0])[i] = 0.f;
+  if (DET) {
+    if (tid < kTileNodes) head_mask[tid] = 0;
+  } else {
+    for (int i = tid; i < kTileNodes * 200; i += kTileWarps * 32) (&agg[0][0])[i] = 0.f;
+  }
   if (tid <= nv) s_rp[tid] = __ldg(t_row_ptr + v0 + tid);
   __syncthreads();
-  tile_accumulate<true, false, true>(agg, s_rp, nv, P, nullptr, W, t_col_dst, t_col_type, norm);
+  const TileHeads th = DET ? TileHeads{head, head_mask} : TileHeads{nullptr, nullptr};
+  tile_accumulate<true, false, true, true, DET>(agg, s_rp, nv, P, nullptr, W, t_col_dst, t_col_type, norm, th);
   __syncthreads();
   for (int i = tid; i < nv * 100; i += kTileWarps * 32) {
     const int r = i / 100, c = (i % 100) * 2;
-    float2 o = *reinterpret_cast<const float2*>(&agg[r][c]);
+    float2 o = DET ? tile_row_sum(agg, th, s_rp, r, c) : *reinterpret_cast<const float2*>(&agg[r][c]);
     float* op = dH + (int64_t)(v0 + r) * 200 + c;
     if (HAS_LOOP) {
       const float2 l = *reinterpret_cast<const float2*>(op);
@@ -104,9 +112,12 @@ __global__ void rgcn_dh_generic_kernel(const float* __restrict__ P, const float*
   dH[idx] = (has_loop ? dH[idx] : 0.f) + acc;
 }
 
-// dW: warp per run of kEdgesPerWarp consecutive edges of the relation-grouped list.
+// dW: warp per run of kEdgesPerWarp consecutive edges of the relation-grouped list.  DET: instead of adding its partial
+// row for relation r into dW, run w stores it to dW = partials[w + r] (unique: along the relation-grouped list the
+// (run, relation) pairs form a staircase on which w + r strictly increases; at most runs + R2 rows), and
+// rgcn_dw_reduce_kernel adds them up in run order.
 constexpr int kEdgesPerWarp = 64;
-template <bool INDEXED>
+template <bool INDEXED, bool DET = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32)
 rgcn_dw_d200_kernel(const float* __restrict__ H, const int32_t* __restrict__ h_index, const float* __restrict__ P,
                     const int32_t* __restrict__ rel_ptr, const int32_t* __restrict__ rel_src,
@@ -130,12 +141,15 @@ rgcn_dw_d200_kernel(const float* __restrict__ H, const int32_t* __restrict__ h_i
   float acc[16];
 #pragma unroll
   for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+  float* const wbase = dW + (DET ? (int64_t)warp * 400 : 0) + woff;
   auto flush = [&](int rr) {
     if (active) {
-      float* wp = dW + (int64_t)rr * 400 + woff;
+      float* wp = wbase + (int64_t)rr * 400;
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        red_add_f4(wp + 4 * k, make_float4(acc[4 * k], acc[4 * k + 1], acc[4 * k + 2], acc[4 * k + 3]));
+        const float4 v = make_float4(acc[4 * k], acc[4 * k + 1], acc[4 * k + 2], acc[4 * k + 3]);
+        if (DET) st_f4(wp + 4 * k, v);
+        else red_add_f4(wp + 4 * k, v);
         acc[4 * k] = acc[4 * k + 1] = acc[4 * k + 2] = acc[4 * k + 3] = 0.f;
       }
     }
@@ -183,6 +197,23 @@ rgcn_dw_d200_kernel(const float* __restrict__ H, const int32_t* __restrict__ h_i
   flush(r);
 }
 
+// DET dW: dW[r] += the partial rows of the runs holding relation r's edges, in run order (thread = 4 of the 400 columns)
+__global__ void __launch_bounds__(100)
+rgcn_dw_reduce_kernel(const float* __restrict__ parts, const int32_t* __restrict__ rel_ptr, float* __restrict__ dW) {
+  const int r = blockIdx.x, c = threadIdx.x * 4;
+  const int e0 = __ldg(rel_ptr + r), e1 = __ldg(rel_ptr + r + 1);
+  if (e0 >= e1) return;
+  float* op = dW + (int64_t)r * 400 + c;
+  float4 s = *reinterpret_cast<const float4*>(op);
+  const int w1 = (e1 - 1) / kEdgesPerWarp;
+#pragma unroll 8
+  for (int w = e0 / kEdgesPerWarp; w <= w1; ++w) {
+    const float4 p = ldg_f4(parts + (int64_t)(w + r) * 400 + c);
+    s.x += p.x; s.y += p.y; s.z += p.z; s.w += p.w;
+  }
+  st_f4(op, s);
+}
+
 __global__ void rgcn_dw_generic_kernel(const float* __restrict__ H, const int32_t* __restrict__ h_index,
                                        const float* __restrict__ P, const int32_t* __restrict__ rel_ptr,
                                        const int32_t* __restrict__ rel_src, const int32_t* __restrict__ rel_dst,
@@ -223,6 +254,7 @@ __global__ void scatter_add_rows_scalar_kernel(const float* __restrict__ src, co
 
 int launch_scatter_add_rows(const float* src, const int32_t* index, float* dst, int64_t n_rows, int d,
                             cudaStream_t stream) {
+  if (deterministic()) return scatter_add_rows_det(src, d, index, nullptr, dst, n_rows, d, stream);
   const bool vec = d % 4 == 0 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
   if (vec) {
     const int64_t threads = n_rows * 32;
@@ -294,6 +326,13 @@ int launch_rgcn_bwd(const float* H, const int32_t* h_index, const float* W, cons
         rgcn_gather_stream_kernel<false, false, false, true><<<kNumSMs, StDefault<true>::kThreads, StDefault<true>::kSmemBytes, stream>>>(
             P, nullptr, W, t_row_ptr, t_col_dst, t_col_type, norm, dH, (int)N, R2, nullptr, 0, (int)E, nullptr);
       RENET_CHECK_LAUNCH("rgcn_gather_stream_kernel(bwd)");
+    } else if (deterministic()) {
+      const unsigned grid = (unsigned)((N + kTileNodes - 1) / kTileNodes);
+      if (Wloop != nullptr)
+        rgcn_dh_tile_kernel<true, true><<<grid, kTileWarps * 32, 0, stream>>>(P, W, t_row_ptr, t_col_dst, t_col_type, norm, dH, (int)N);
+      else
+        rgcn_dh_tile_kernel<false, true><<<grid, kTileWarps * 32, 0, stream>>>(P, W, t_row_ptr, t_col_dst, t_col_type, norm, dH, (int)N);
+      RENET_CHECK_LAUNCH("rgcn_dh_tile_kernel");
     } else {
       const unsigned grid = (unsigned)((N + kTileNodes - 1) / kTileNodes);
       if (Wloop != nullptr)
@@ -304,6 +343,19 @@ int launch_rgcn_bwd(const float* H, const int32_t* h_index, const float* W, cons
     }
     const int64_t warps = (E + kEdgesPerWarp - 1) / kEdgesPerWarp;
     const unsigned g2 = (unsigned)((warps + kWarpsPerCta - 1) / kWarpsPerCta);
+    if (deterministic()) {
+      void* parts = nullptr;
+      if ((rc = det_scratch((warps + R2) * 400 * (int64_t)sizeof(float), stream, &parts))) return rc;
+      float* Wp = static_cast<float*>(parts);
+      if (h_index)
+        rgcn_dw_d200_kernel<true, true><<<g2, kWarpsPerCta * 32, 0, stream>>>(H, h_index, P, rel_ptr, rel_src, rel_dst, norm, Wp, (int)E, R2);
+      else
+        rgcn_dw_d200_kernel<false, true><<<g2, kWarpsPerCta * 32, 0, stream>>>(H, h_index, P, rel_ptr, rel_src, rel_dst, norm, Wp, (int)E, R2);
+      RENET_CHECK_LAUNCH("rgcn_dw_d200_kernel");
+      rgcn_dw_reduce_kernel<<<R2, 100, 0, stream>>>(Wp, rel_ptr, dW);
+      RENET_CHECK_LAUNCH("rgcn_dw_reduce_kernel");
+      return RENET_OK;
+    }
     if (h_index)
       rgcn_dw_d200_kernel<true><<<g2, kWarpsPerCta * 32, 0, stream>>>(H, h_index, P, rel_ptr, rel_src, rel_dst, norm, dW, (int)E, R2);
     else

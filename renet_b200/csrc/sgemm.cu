@@ -146,22 +146,24 @@ __global__ void sgemm_nn_naive(const float* __restrict__ A, const int32_t* __res
 }
 
 // ---- C[M,N] (+)= A^T B,  A [K, M] rows through a_index, B [K, N]; K is the long dimension ------
-// Used for dWloop = Hin^T @ G (K = number of nodes).  Split-K over CTAs, fp32 atomics into C
-// (C must be zero-initialised or hold the value to accumulate onto).
+// Used for dWloop = Hin^T @ G (K = number of nodes).  Split-K over CTAs of kchunk rows each, fp32 atomics into C
+// (C must be zero-initialised or hold the value to accumulate onto).  DET: each chunk writes its tile to
+// C = partials [gridDim.z][M][N] (ldc unused) instead, for an ordered sum afterwards.
 constexpr int TN_BM = 40, TN_BN = 200, TN_BK = 8, TN_KCHUNK = 256;
-template <bool INDEXED>
+constexpr int TN_MAX_DET_CHUNKS = 32;   // deterministic mode: bounds the partials to 32 M x N tiles
+template <bool INDEXED, bool DET = false>
 __global__ void __launch_bounds__(256)
 sgemm_tn_splitk_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_index, int64_t lda,
                        const float* __restrict__ B, int64_t ldb, float* __restrict__ C, int64_t ldc,
-                       int M, int N, int64_t K) {
+                       int M, int N, int64_t K, int64_t kchunk) {
   // tile: 40 (M) x 200 (N) outputs, thread = 4 x 8 outputs -> 10 x 25 threads
   __shared__ __align__(16) float As[TN_BK][TN_BM];
   __shared__ __align__(16) float Bs[TN_BK][TN_BN];
   const int tid = threadIdx.x;
   const int tx = tid % 25, ty = tid / 25;
   const int m0 = blockIdx.x * TN_BM, n0 = blockIdx.y * TN_BN;
-  const int64_t kbeg = (int64_t)blockIdx.z * TN_KCHUNK;
-  const int64_t kend = min(K, kbeg + TN_KCHUNK);
+  const int64_t kbeg = (int64_t)blockIdx.z * kchunk;
+  const int64_t kend = min(K, kbeg + kchunk);
   float acc[4][8];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -211,8 +213,9 @@ sgemm_tn_splitk_kernel(const float* __restrict__ A, const int32_t* __restrict__ 
     for (int h = 0; h < 2; ++h) {
       int c = n0 + h * 100 + tx * 4;
       if (c >= N) continue;
-      red_add_f4(C + (int64_t)m * ldc + c,
-                 make_float4(acc[i][h * 4 + 0], acc[i][h * 4 + 1], acc[i][h * 4 + 2], acc[i][h * 4 + 3]));
+      const float4 v = make_float4(acc[i][h * 4 + 0], acc[i][h * 4 + 1], acc[i][h * 4 + 2], acc[i][h * 4 + 3]);
+      if (DET) st_f4(C + ((int64_t)blockIdx.z * M + m) * N + c, v);
+      else red_add_f4(C + (int64_t)m * ldc + c, v);
     }
   }
 }
@@ -301,14 +304,34 @@ bool sgemm_tn_tiled_ok(const float* A, int64_t lda, const float* B, int64_t ldb,
 int sgemm_tn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
              int64_t ldc, int32_t M, int32_t N, int64_t K, bool accumulate, cudaStream_t stream, bool naive) {
   if (M <= 0 || N <= 0) return RENET_OK;
+  const bool tiled = !naive && sgemm_tn_tiled_ok(A, lda, B, ldb, C, ldc, M, N);
+  if (tiled && K > 0 && deterministic()) {
+    // the chunking depends on K alone; the chunks' tiles are summed in chunk order
+    int64_t chunks = (K + TN_KCHUNK - 1) / TN_KCHUNK;
+    if (chunks > TN_MAX_DET_CHUNKS) chunks = TN_MAX_DET_CHUNKS;
+    const int64_t kchunk = ((K + chunks - 1) / chunks + TN_BK - 1) / TN_BK * TN_BK;
+    chunks = (K + kchunk - 1) / kchunk;
+    void* parts = nullptr;
+    int rc = det_scratch(chunks * M * N * (int64_t)sizeof(float), stream, &parts);
+    if (rc) return rc;
+    dim3 grid((M + TN_BM - 1) / TN_BM, (N + TN_BN - 1) / TN_BN, (unsigned)chunks);
+    float* P = static_cast<float*>(parts);
+    if (a_index)
+      sgemm_tn_splitk_kernel<true, true><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, P, N, M, N, K, kchunk);
+    else
+      sgemm_tn_splitk_kernel<false, true><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, P, N, M, N, K, kchunk);
+    RENET_CHECK_LAUNCH("sgemm_tn_splitk_kernel");
+    note_gemm_kernel(RENET_GEMM_FFMA_TILED);
+    return launch_sum_partials(P, (int)chunks, (int64_t)M * N, M, N, C, ldc, accumulate, stream);
+  }
   if (!accumulate) RENET_CHECK_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, N * sizeof(float), M, stream));
   if (K <= 0) return RENET_OK;
-  if (!naive && sgemm_tn_tiled_ok(A, lda, B, ldb, C, ldc, M, N)) {
+  if (tiled) {
     dim3 grid((M + TN_BM - 1) / TN_BM, (N + TN_BN - 1) / TN_BN, (unsigned)((K + TN_KCHUNK - 1) / TN_KCHUNK));
     if (a_index)
-      sgemm_tn_splitk_kernel<true><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, M, N, K);
+      sgemm_tn_splitk_kernel<true><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, M, N, K, TN_KCHUNK);
     else
-      sgemm_tn_splitk_kernel<false><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, M, N, K);
+      sgemm_tn_splitk_kernel<false><<<grid, 256, 0, stream>>>(A, a_index, lda, B, ldb, C, ldc, M, N, K, TN_KCHUNK);
     RENET_CHECK_LAUNCH("sgemm_tn_splitk_kernel");
     note_gemm_kernel(RENET_GEMM_FFMA_TILED);
   } else {
