@@ -105,9 +105,12 @@ int sgemm_nt(const float* A, int64_t lda, const float* B, int64_t ldb, float* C,
 // 0 = automatic, 1 = tile, 3 = stream (RENET_GATHER_KERNEL=tile|stream; rgcn_fwd.cu)
 int gather_kernel_choice();
 constexpr int64_t kStreamMinEdges = 16384;   // below this a persistent one-CTA-per-SM launch costs more than the tile kernel
-constexpr int64_t kStreamMinNodes = 16384;
+constexpr int64_t kStreamMinNodes = 16384;   // graphs with indexed input rows (layer 1) and the backward dH
+constexpr int64_t kStreamMinPlainNodes = 2048;   // forward with plain input rows (layer 2's read-out sub-graph)
 constexpr int64_t kStreamMaxNodes = 40960;    // 33 MB of fp32 features (2/3 of the 50 MB L2): beyond this the source rows come from HBM
-bool gather_use_stream(int64_t E, int64_t N);
+// forward: indexed_input = the input rows come through an index (h_index); the backward passes true (its threshold is
+// kStreamMinNodes)
+bool gather_use_stream(int64_t E, int64_t N, bool indexed_input);
 void set_stream_debug_buffer(long long* p);   // debug: per-warp time stamps of the stream kernel (rgcn_fwd.cu)          // the stream kernel (rgcn_stream.cuh) serves this edge count
 
 // tensor-core (wgmma) GEMM engine building blocks (umma_gemm.cu); gemm_mode() == 1 selects the engine

@@ -309,7 +309,7 @@ int launch_rgcn_bwd(const float* H, const int32_t* h_index, const float* W, cons
                     ((reinterpret_cast<uintptr_t>(H) | reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(dH) |
                       reinterpret_cast<uintptr_t>(dW) | reinterpret_cast<uintptr_t>(P)) & 15) == 0;
   if (fast) {
-    if (E > 0 && gather_use_stream(E, N)) {
+    if (E > 0 && gather_use_stream(E, N, true)) {       // kStreamMinNodes, as before the forward read-out threshold
       // batch scale: the persistent bulk-copy kernel on the reversed graph -- no atomics, bitwise reproducible dH
       static bool attr_done = false;
       if (!attr_done) {

@@ -20,8 +20,9 @@ namespace renet {
 namespace {
 
 // Tile kernel (round 1; rgcn_tile.cuh): one CTA per 16 destinations.  The path for small graphs (inference on a handful of
-// sub-graphs, the read-out sub-graph of layer 2: a persistent one-CTA-per-SM launch would cost more than the work) and for DGL's
-// edge-less pass-through; at batch scale the persistent kernel of rgcn_stream.cuh takes over (gather_use_stream).
+// sub-graphs: a persistent one-CTA-per-SM launch would cost more than the work) and for DGL's edge-less pass-through; at
+// batch scale, and on layer 2's read-out sub-graph of a batch, the persistent kernel of rgcn_stream.cuh takes over
+// (gather_use_stream).
 template <bool RELU, bool HAS_LOOP, bool INDEXED, int NODES = kTileNodes>
 __global__ void __launch_bounds__(kTileWarps * 32, 768 / (kTileWarps * 32))
 rgcn_gather_d200_kernel(const float* __restrict__ H, const int32_t* __restrict__ h_index,
@@ -113,15 +114,19 @@ int gather_kernel_choice() {
   }
   return v;
 }
-bool gather_use_stream(int64_t E, int64_t N) {
+bool gather_use_stream(int64_t E, int64_t N, bool indexed_input) {
   // E may be an upper bound (device-assembled batches and read-out sub-graphs pass their capacity), so the destination
-  // count decides with it: the persistent kernel pays a prologue of several microseconds per launch, which a few thousand
-  // destinations' worth of edges (the read-out sub-graph of an ICEWS18 batch) does not amortise.  And it is built for
-  // feature matrices that live in L2 (ICEWS18: 27 MB of the H100's 50 MB): with two rows in flight per warp it cannot cover
-  // HBM latency, so when the features exceed L2 (kStreamMaxNodes; the synthetic 1 M-entity shard, 800 MB) the tile kernel
-  // stays
+  // count decides with it: the persistent kernel pays a prologue of about 7 us per launch.  Graphs whose input rows come
+  // through an index (layer 1: the embedding table through node_ent) amortise it from kStreamMinNodes on (the tile kernel
+  // is faster on 12 k- and 21 k-node layer-1 graphs, DESIGN §5: that threshold was not moved here).  Plain input rows
+  // (layer 2's read-out sub-graph: about 12 edges per destination, rows of H1) amortise it from kStreamMinPlainNodes on
+  // (measured on read-out sub-graphs of 2 k to 10 k destinations, DESIGN §5).  And the kernel is built for feature
+  // matrices that live in L2 (ICEWS18: 27 MB of the H100's 50 MB): with two rows in flight per warp it cannot cover HBM
+  // latency, so when the destinations' own feature rows exceed L2 (kStreamMaxNodes; the synthetic 1 M-entity shard, 800 MB)
+  // the tile kernel stays
   const int c = gather_kernel_choice();
-  return c == 3 || (c == 0 && E >= kStreamMinEdges && N >= kStreamMinNodes && N <= kStreamMaxNodes);
+  const int64_t min_nodes = indexed_input ? kStreamMinNodes : kStreamMinPlainNodes;
+  return c == 3 || (c == 0 && E >= kStreamMinEdges && N >= min_nodes && N <= kStreamMaxNodes);
 }
 
 // debug hook (tools/stream_timeline.py): per-warp time stamps of the next stream-kernel launches; never set in production
@@ -184,7 +189,7 @@ int launch_rgcn_gather(const float* H, const int32_t* h_index, const float* W, c
                       reinterpret_cast<uintptr_t>(Hout)) & 15) == 0;
   if (fast) {
     const int key = (relu ? 4 : 0) | (has_loop ? 2 : 0) | (h_index ? 1 : 0);
-    if (!passthrough && gather_use_stream(E, N)) {
+    if (!passthrough && gather_use_stream(E, N, h_index != nullptr)) {
 #define RENET_LAUNCH_STREAM(R, L, I) return launch_stream<R, L, I>(H, h_index, W, row_ptr, col_src, col_type, norm, Hout, (int)N, R2, hot_rel, n_hot, (int)E, stream)
       switch (key) {
         case 0: RENET_LAUNCH_STREAM(false, false, false);

@@ -75,6 +75,9 @@ __device__ __forceinline__ void st_bulk_g2s(uint32_t dst, const void* src, uint3
                "r"(bytes), "r"(bar)
                : "memory");
 }
+__device__ __forceinline__ void st_cp_async4(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
 __device__ __forceinline__ void st_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -189,6 +192,21 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     if (pf) asm volatile("prefetch.global.L2 [%0];" ::"l"(pf));
   }
   const int E = __ldg(row_ptr + N);
+  // CTA partition search, first round: its probe positions depend on N only, so its loads fly with the edge count's
+  // (the search itself is below)
+  const int half = tid >> 8, ht = tid & 255;
+  const int c_idx = blockIdx.x + half;
+  const bool searching = tid < 512 && c_idx > 0 && c_idx < (int)gridDim.x;
+  const int probe0 = min((ht + 1) * (N / 256 + 1) - 1, N);
+  const int val0 = searching ? __ldg(row_ptr + probe0) : 0;
+  // the caller's hot-relation list: copied by warp 1 into the (then unused) histogram scratch now, used after the search
+  // (slot table, resident-row copies).  An asynchronous copy: neither the warp nor a register waits for it meanwhile
+  constexpr int kHotIters = (Cfg::kHot + 31) / 32;
+  const int n_hot_given = given_hot ? min(n_hot_arg, Cfg::kHot) : 0;
+  if (warp == 1) {
+    for (int sl = lane; sl < n_hot_given; sl += 32) st_cp_async4(smem_u32(hist + sl), hot_rel + sl);
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  }
   const uint32_t hot_bar0 = smem_u32(bars + kStWarps * D);   // [8]: "the resident rows of group g have landed"
   const uint32_t head_bar0 = hot_bar0 + kStHotGroups * 8;    // [warps]: "this warp's head slot is written"
 
@@ -206,46 +224,39 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     for (int i = tid; i < kStMaxR2 + 256; i += kStThreads) cnt[i] = 0;
   for (int i = tid; i < kStMaxR2 / 4; i += kStThreads) reinterpret_cast<uint32_t*>(slot_of)[i] = 0u;
   __syncthreads();
-  // resident rows (slot sl holds relation row_of(sl)) -> shared memory, one warp; slot sl lands on the barrier of group
-  // sl / kHotPerGroup, so an edge waits only for its own group and the edge loop starts before the table is complete.
-  // Every group barrier gets its one arrival (an empty group completes at once).
+  // resident rows (slot sl = lane + 32 k holds relation row_of(k)) -> shared memory, one warp; slot sl lands on the barrier
+  // of group sl / kHotPerGroup, so an edge waits only for its own group and the edge loop starts before the table is
+  // complete.  Every group barrier gets its one arrival (an empty group completes at once).  Issued after the partition
+  // search: the grid's 17 MB of copies (82 rows x 132 SMs) would otherwise share L2 with the search's dependent reads.
   auto load_hot = [&](int n_hot, auto row_of) {
     if (lane < kStHotGroups) {
       const int rows = min(max(n_hot - lane * Cfg::kHotPerGroup, 0), Cfg::kHotPerGroup);
       st_expect_tx(hot_bar0 + lane * 8, (uint32_t)rows * 1600u);
     }
     __syncwarp();
-    for (int sl = lane; sl < n_hot; sl += 32)
-      st_bulk_g2s(smem_u32(st_smem + Cfg::kOffHot + sl * 1600), W + (int64_t)row_of(sl) * 400, 1600,
-                  hot_bar0 + (sl / Cfg::kHotPerGroup) * 8);
+#pragma unroll
+    for (int k = 0; k < kHotIters; ++k) {
+      const int sl = lane + 32 * k;
+      if (sl < n_hot)
+        st_bulk_g2s(smem_u32(st_smem + Cfg::kOffHot + sl * 1600), W + (int64_t)row_of(k) * 400, 1600,
+                    hot_bar0 + (sl / Cfg::kHotPerGroup) * 8);
+    }
   };
-  // ---- hot rows from the caller's list: fetched while the partition search runs --------------------------------------------
-  if (given_hot && warp == 1) {
-    load_hot(min(n_hot_arg, Cfg::kHot), [&](int sl) {
-      const int r = __ldg(hot_rel + sl);
-      const bool ok = r >= 0 && r < R2;                    // an id outside the table is ignored (its slot holds row 0, unused)
-      if (ok) slot_of[r] = (uint8_t)(sl + 1);
-      return ok ? r : 0;
-    });
-  }
   // ---- CTA partition: destinations [A, A_next) own 1/gridDim of the edges (node-aligned).  Threads 0..255 look for
   //      lower_bound(row_ptr, T_c), threads 256..511 for lower_bound(row_ptr, T_c+1).  Invariant: the answer lies in
   //      [lo, hi]; every round probes 256 evenly spaced entries of the bracket and keeps the 1/256 of it between the last
   //      probe below the target and the first one at or above it.  The number of rounds depends on N only (uniform over
   //      the CTA); the last round probes consecutive entries, so the thread that hits the answer also holds
   //      row_ptr[answer] and its left neighbour the entry before ---------------------------------------------------------------
-  const int half = tid >> 8, ht = tid & 255;
-  const int c_idx = blockIdx.x + half;
   // work is counted in edges + kStNodeCost per destination: key(v) = row_ptr[v] + kStNodeCost * v ascends with v
   const int64_t total_cost = (int64_t)E + (int64_t)kStNodeCost * N;
   const int64_t target = ((int64_t)c_idx * total_cost) / gridDim.x;
-  const bool searching = tid < 512 && c_idx > 0 && c_idx < (int)gridDim.x;
   int lo = 0, hi = N;
   const int rounds = N < 256 ? 1 : (N < 65536 ? 2 : (N < (1 << 24) ? 3 : 4));
   for (int r = 0; r < rounds; ++r) {
     const int step = (hi - lo) / 256 + 1;
     const int p = min(lo + (ht + 1) * step - 1, hi);       // the last probes are clipped to hi, where key >= target
-    const int val = searching ? __ldg(row_ptr + p) : 0;
+    const int val = r == 0 ? val0 : (searching ? __ldg(row_ptr + p) : 0);   // (round 0: loaded at entry, p == probe0)
     const bool below = searching && (int64_t)val + (int64_t)kStNodeCost * p < target;
     const unsigned m = __ballot_sync(0xffffffffu, below);
     if (lane == 0 && m) atomicAdd(&s_part[2 * r + (half & 1)], __popc(m));      // row_ptr ascends: # probes below the target
@@ -260,6 +271,16 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     lo = new_lo; hi = new_hi;
   }
   __syncthreads();
+  // ---- hot rows from the caller's list (slot table complete at the __syncthreads after the row_ptr slice) ---------------------
+  if (given_hot && warp == 1) {
+    asm volatile("cp.async.wait_all;" ::: "memory");      // this lane's entries of the list
+    load_hot(n_hot_given, [&](int k) {
+      const int sl = lane + 32 * k, r = hist[sl];
+      const bool ok = r >= 0 && r < R2;                    // an id outside the table is ignored (its slot holds row 0, unused)
+      if (ok) slot_of[r] = (uint8_t)(sl + 1);
+      return ok ? r : 0;
+    });
+  }
   // the boundary goes to whichever of the two destination starts around the target is nearer (halves the imbalance a
   // heavy destination causes); both CTAs that share a boundary derive it from the same target by the same rule
   int A = 0, A_next = N, cb = 0, ce = E;
@@ -380,7 +401,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
       }
       __syncthreads();
     }
-    if (warp == 1) load_hot(min(s_part[9], Cfg::kHot), [&](int sl) { return hist[sl]; });
+    if (warp == 1) load_hot(min(s_part[9], Cfg::kHot), [&](int k) { return hist[lane + 32 * k]; });
   }
   block_gather(0);
   __syncthreads();                     // s_rp, slot_of complete; the ring (= cnt / hist) may be overwritten from here on
