@@ -513,6 +513,28 @@ int renet_decoder_ce_bwd(const float* X, const float* W, const float* bias, cons
                          int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Soft-target decoder: logits z = X @ W^T + bias followed by the soft cross-entropy of the global model (reference
+ * global_model.py:53-55 with utils.py:287-290: linear_s / linear_o, X = s_q [B,h], W [|E|,h]).  P is fp32 [M, ldp]; its
+ * rows are target distributions and need not sum to 1 (all-zero rows give loss 0 and gradient 0).
+ *   renet_decoder_soft_ce_fwd : loss_rows[i] = lse[i] * psum[i] - sum_c P[i,c] z[i,c]; lse[i] = logsumexp_c z[i,c] and
+ *       psum[i] = sum_c P[i,c] (both kept for backward).  wgmma 3xTF32 GEMM with a fused epilogue (the [B,|E|] logits
+ *       never reach memory); a row's partials are combined in fp64 in a fixed order.
+ *   renet_decoder_soft_ce_bwd : for loss = scale * d_scale[0] * sum_i loss_rows[i] (the reference's mean: scale = 1/B;
+ *       d_scale = optional DEVICE scalar): dz[i,c] = scale * d_scale * (psum[i] * softmax(z)[i,c] - P[i,c]); dX [M,K]
+ *       written; dW [N,K] and dbias [N] (may be NULL) ACCUMULATED.  The logits are recomputed; dz lives in the workspace.
+ * No float atomics: both passes are bitwise reproducible.  K % 4 == 0; ldp >= N; X [M,K], W [N,K] row-major, 16-byte
+ * aligned.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t renet_decoder_soft_ce_workspace_bytes(int64_t M, int32_t N, int32_t K);
+int renet_decoder_soft_ce_fwd(const float* X, const float* W, const float* bias, const float* P, int64_t ldp, float* loss_rows,
+                              float* lse, float* psum, int64_t M, int32_t N, int32_t K, void* workspace, int64_t workspace_bytes,
+                              void* stream);
+int64_t renet_decoder_soft_ce_bwd_workspace_bytes(int64_t M, int32_t N, int32_t K);
+int renet_decoder_soft_ce_bwd(const float* X, const float* W, const float* bias, const float* P, int64_t ldp, const float* lse,
+                              const float* psum, float scale, const float* d_scale, float* dX, float* dW, float* dbias, int64_t M,
+                              int32_t N, int32_t K, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Optimiser step of the reference training loop on FLAT fp32 buffers (reference train.py:140-142:
  * torch.nn.utils.clip_grad_norm_(model.parameters(), grad_norm); Adam(lr, weight_decay).step()).  The data-parallel
  * engine keeps all parameters / gradients as views into one flat buffer each (the gradient buffer is what NCCL

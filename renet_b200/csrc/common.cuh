@@ -136,8 +136,14 @@ struct EpiArgs {
   float* tlogit;           // [M] (EPI 1): written by the one thread that sees the target column
   float* dT;               // [N, ldT] (EPI 2): the same gradient transposed (A operand of dW = dlogits^T @ X)
   int64_t ldT;
-  float scale;             // (EPI 2)
-  const float* dscale;     // (EPI 2) optional device scalar multiplied into scale (the upstream gradient, no host read)
+  float scale;             // (EPI 2, 4)
+  const float* dscale;     // (EPI 2, 4) optional device scalar multiplied into scale (the upstream gradient, no host read)
+  // soft targets (EPI 3, 4): P[row * ldp + col], rows need not sum to 1
+  const float* soft;
+  int64_t ldp;
+  float* pdot;             // [2 * n_tiles, M] (EPI 3): sum of P * logit over the (row, half column tile)
+  float* pmass;            // [2 * n_tiles, M] (EPI 3): sum of P over the same
+  const float* rowmass;    // [M] (EPI 4): sum of P over the whole row
 };
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,

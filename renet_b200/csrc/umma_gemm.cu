@@ -336,6 +336,9 @@ __device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], flo
 //          [M, N] logits never reach memory; ce_reduce_kernel turns the partials into logsumexp and the loss
 //   EPI 2  dlogits[row, col] = (exp(logit - lse[row]) - [col == target[row]]) * scale, written to memory for the two
 //          gradient GEMMs (the backward pass recomputes the logits instead of keeping them)
+//   EPI 3  soft targets P (global_model.py's soft cross-entropy): EPI 1's running max and sum of exp, and the sums of
+//          P * logit and of P, with P read at the logit's own position; soft_ce_reduce_kernel (decoder.cu) combines them
+//   EPI 4  dlogits[row, col] = (rowmass[row] * exp(logit - lse[row]) - P[row, col]) * scale, written as in EPI 2
 // grid.x = min(units, SMs).  Batched GEMMs (the two GRU encoders) have per-batch operand offsets.  Split-K (long-K,
 // few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
 // partial product to C + s*split_c; the caller sums the partials.
@@ -501,12 +504,16 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     acc_store(acc, sC, P_CLD, wt);
     named_bar_sync(1 + g, 128);
     if (wt >= 64) continue;
+    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI >= 3;
     const int64_t gr = w.row_base + 64 * g + wt;
     const float* srow = sC + wt * P_CLD;
-    float run_m = -3.0e38f, run_s = 0.f;               // EPI 1: running max / sum of exp of this (row, half tile)
-    const int tgt = gr < M ? __ldg(epi.target + gr) : -1;
-    const float row_lse = (EPI == 2 && gr < M) ? __ldg(epi.lse + gr) : 0.f;
-    const float gscale = (EPI == 2) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
+    float run_m = -3.0e38f, run_s = 0.f;               // EPI 1, 3: running max / sum of exp of this (row, half tile)
+    float run_pz = 0.f, run_p = 0.f;                   // EPI 3: sums of P * logit and of P
+    const int tgt = (!SOFT && gr < M) ? __ldg(epi.target + gr) : -1;
+    const float row_lse = (!FWD && gr < M) ? __ldg(epi.lse + gr) : 0.f;
+    const float row_mass = (EPI == 4 && gr < M) ? __ldg(epi.rowmass + gr) : 0.f;
+    const float gscale = (!FWD) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
+    const float* prow = SOFT ? epi.soft + gr * epi.ldp + n0 : nullptr;   // read only for gr < M
 #pragma unroll 1
     for (int lc = 0; lc < P_UN; lc += 8) {
       const int cc = cb + lc;
@@ -522,14 +529,20 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
             if (bz != nullptr) o[i] += __ldg(bz + n0 + cc + i);
             mx = fmaxf(mx, o[i]);
           }
-        if (EPI == 1) {
+        if (FWD) {
           const float nm = fmaxf(run_m, mx);
           float add = 0.f;
 #pragma unroll
           for (int i = 0; i < 8; ++i)
             if (i < nv) {
               add += expf(o[i] - nm);
-              if (n0 + cc + i == tgt) epi.tlogit[gr] = o[i];
+              if (SOFT) {
+                const float p = __ldg(prow + cc + i);
+                run_pz += p * o[i];
+                run_p += p;
+              } else if (n0 + cc + i == tgt) {
+                epi.tlogit[gr] = o[i];
+              }
             }
           run_s = run_s * expf(run_m - nm) + add;
           run_m = nm;
@@ -538,17 +551,22 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
 #pragma unroll
           for (int i = 0; i < 8; ++i)
             if (i < nv) {
-              const float gv = (expf(o[i] - row_lse) - (n0 + cc + i == tgt ? 1.f : 0.f)) * gscale;
+              const float gv = SOFT ? (row_mass * expf(o[i] - row_lse) - __ldg(prow + cc + i)) * gscale
+                                    : (expf(o[i] - row_lse) - (n0 + cc + i == tgt ? 1.f : 0.f)) * gscale;
               dp[i] = gv;                                              // row-major: A of dX = dlogits @ W
               epi.dT[(int64_t)(n0 + cc + i) * epi.ldT + gr] = gv;      // transposed (lanes = consecutive rows: coalesced)
             }
         }
       }
     }
-    if (EPI == 1 && gr < M) {
+    if (FWD && gr < M) {
       const int64_t pi = (int64_t)(w.nt * 2 + w.half) * M + gr;
       epi.pmax[pi] = run_m;
       epi.psum[pi] = run_s;
+      if (SOFT) {
+        epi.pdot[pi] = run_pz;
+        epi.pmass[pi] = run_p;
+      }
     }
   }
   ts.finish(1);
@@ -868,6 +886,8 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(0)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(1)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(2)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(3)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(4)));
     attr2 = true;
   }
   const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
@@ -880,6 +900,8 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
                                                                            g_gemm_dbg)
   if (epi_mode == 1) RENET_UMMA_LAUNCH(false, 1);
   else if (epi_mode == 2) RENET_UMMA_LAUNCH(false, 2);
+  else if (epi_mode == 3) RENET_UMMA_LAUNCH(false, 3);
+  else if (epi_mode == 4) RENET_UMMA_LAUNCH(false, 4);
   else if (a_index) RENET_UMMA_LAUNCH(true, 0);
   else RENET_UMMA_LAUNCH(false, 0);
 #undef RENET_UMMA_LAUNCH
@@ -1012,7 +1034,7 @@ static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, 
 }
 
 // C[b] (+)= A[b] @ Bpacked[b] (+bias[b]) for b < batch; strides in elements (A, C) / bytes (Bp).
-// epi_mode 1 / 2: fused cross-entropy epilogues (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
+// epi_mode 1-4: fused cross-entropy epilogues (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,

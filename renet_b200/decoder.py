@@ -1,7 +1,11 @@
 """Fused decoder: linear + cross-entropy of reference model.py:89-91 / 97-100 on the wgmma 3xTF32 engine
 (renet_decoder_ce_fwd / _bwd): ``decoder_cross_entropy(x, weight, bias, target)`` equals
 ``F.cross_entropy(F.linear(x, weight, bias), target)`` (mean over rows) without materialising the [B, |E|] logits in
-the forward pass.  ``nn.Linear`` modules stay the parameter holders (state_dict keys ``linear.*`` / ``linear_r.*``)."""
+the forward pass.  ``nn.Linear`` modules stay the parameter holders (state_dict keys ``linear.*`` / ``linear_r.*``).
+
+``decoder_soft_cross_entropy(x, weight, bias, soft_targets)`` is the global model's loss head on the same engine
+(renet_decoder_soft_ce_fwd / _bwd): the reference's ``soft_cross_entropy(F.linear(x, weight, bias), soft_targets)``
+(utils.py:287-290, fp64 log-softmax, mean over rows), returned as a float64 scalar like the reference's."""
 import torch
 
 from . import _lib
@@ -46,3 +50,45 @@ class _DecoderCEFn(torch.autograd.Function):
 
 def decoder_cross_entropy(x, weight, bias, target):
     return _DecoderCEFn.apply(x, weight, bias, target)
+
+
+class _DecoderSoftCEFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, soft_targets):
+        L, P = _lib.lib(), _lib.ptr
+        _lib.require_cuda(x, weight, bias, soft_targets)
+        x, weight, bias = x.contiguous(), weight.contiguous(), bias.contiguous()
+        tp = soft_targets.to(torch.float32).contiguous()          # the reference's fp64 targets, converted once
+        M, K = x.shape
+        N = weight.shape[0]
+        dev = x.device
+        loss_rows = torch.empty(M, device=dev)
+        lse = torch.empty(M, device=dev)
+        psum = torch.empty(M, device=dev)
+        nbytes = int(L.renet_decoder_soft_ce_workspace_bytes(M, N, K))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _lib.check(L.renet_decoder_soft_ce_fwd(P(x), P(weight), P(bias), P(tp), N, P(loss_rows), P(lse), P(psum), M, N, K, P(ws),
+                                               nbytes, _lib.stream()), 'renet_decoder_soft_ce_fwd')
+        ctx.save_for_backward(x, weight, bias, tp, lse, psum)
+        return loss_rows.double().mean()
+
+    @staticmethod
+    def backward(ctx, g):
+        L, P = _lib.lib(), _lib.ptr
+        x, weight, bias, tp, lse, psum = ctx.saved_tensors
+        M, K = x.shape
+        N = weight.shape[0]
+        dev = x.device
+        dx = torch.empty_like(x)
+        dw = torch.zeros_like(weight)
+        db = torch.zeros_like(bias)
+        nbytes = int(L.renet_decoder_soft_ce_bwd_workspace_bytes(M, N, K))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        g = g.contiguous().to(torch.float32)      # the upstream gradient stays on the device (no host read in backward)
+        _lib.check(L.renet_decoder_soft_ce_bwd(P(x), P(weight), P(bias), P(tp), N, P(lse), P(psum), 1.0 / M, P(g), P(dx), P(dw),
+                                               P(db), M, N, K, P(ws), nbytes, _lib.stream()), 'renet_decoder_soft_ce_bwd')
+        return dx, dw, db, None
+
+
+def decoder_soft_cross_entropy(x, weight, bias, soft_targets):
+    return _DecoderSoftCEFn.apply(x, weight, bias, soft_targets)

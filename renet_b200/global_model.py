@@ -16,7 +16,10 @@ What runs where: the whole per-timestamp graphs of the needed timestamps are bat
 destination-sorted per-timestamp edge lists: the batched graph is born in CSR form), both RGCN layers are the fused
 kernels of rgcn.py, ``dgl.max_nodes`` / ``mean_nodes`` is renet_segment_pool_fwd/_bwd, and ``encoder_global``
 (nn.GRU(h, h): parameter holder) runs through renet_gru_dense_fwd/_bwd (tensor-core input projection + the recurrence
-kernel of the hot path).  The two small linear heads and the fp64 soft cross-entropy (utils.py:287-290) stay PyTorch.
+kernel of the hot path).  The training loss -- ``linear_s`` / ``linear_o`` and the soft cross-entropy of utils.py:287-290 --
+is ``decoder.decoder_soft_cross_entropy`` (renet_decoder_soft_ce_fwd/_bwd: the logits never reach memory, no cuBLAS).
+``get_global_emb`` builds the whole table in one batched pass; only ``predict``'s head (test-time roll-over) is
+``nn.Linear``.
 """
 import numpy as np
 import torch
@@ -25,14 +28,14 @@ import torch.nn.functional as F
 from torch.nn.utils.rnn import PackedSequence
 
 from . import _lib
+from .decoder import decoder_soft_cross_entropy
 from .graph import BatchedHistoryGraph, as_history_graph
 from .rgcn import RGCNBlockLayer as RGCNLayer
 
-
-def soft_cross_entropy(pred, soft_targets):
-    """Reference utils.py:287-290 (fp64 log-softmax, mean over rows of the soft-target cross-entropy)."""
-    logp = F.log_softmax(pred.double(), dim=1)
-    return torch.mean(torch.sum(-soft_targets.double() * logp, 1))
+# get_global_emb batches its graph instances in chunks of at most this many nodes (a window larger than that is a chunk of
+# its own).  Each RGCN layer holds a [nodes, h] fp32 activation: 2^20 nodes x h = 200 is 0.8 GB.  The tables of the
+# synthetic ICEWS18- and GDELT-shaped streams have 1.9 M and 8.6 M instance nodes (DESIGN §5).
+GLOBAL_EMB_NODE_BUDGET = 1 << 20
 
 
 def whole_graph_arrays(graphs):
@@ -252,8 +255,8 @@ class RENet_global(nn.Module):
         s_q = gru_final_hidden(self.encoder_global, X, lens)
         pad = torch.zeros(len(t_host) - s_q.shape[0], self.h_dim, device=s_q.device)
         s_q = torch.cat((s_q, pad), dim=0)
-        pred = linear(s_q)
-        return soft_cross_entropy(pred, true_prob[torch.from_numpy(idx).to(true_prob.device)])
+        return decoder_soft_cross_entropy(s_q, linear.weight, linear.bias,
+                                          true_prob[torch.from_numpy(idx).to(true_prob.device)])
 
     def predict(self, t, graph_dict, subject=True):
         """Reference global_model.py:77-89: (s_q [1,1,h], logits [1,1,in_dim], probabilities [in_dim])."""
@@ -264,20 +267,55 @@ class RENet_global(nn.Module):
         return s_q, sub, torch.softmax(sub.view(-1), dim=0)
 
     def get_global_emb(self, t_list, graph_dict):
-        """Reference global_model.py:57-73: global_emb[t] for every training timestamp."""
-        global_emb = dict()
+        """Reference global_model.py:57-73: global_emb[t] for every training timestamp, with the reference's keys in its
+        order -- t == 0 skipped, each entry keyed by the previous t, the last one at t_list[-1] + one time unit -- and
+        values detached [1,1,h], each equal to ``predict(t, graph_dict)[0]``.
+
+        One batched pass instead of a predict call per timestamp: every (window, graph) occurrence is one whole-graph
+        instance of a batched graph (so in train mode each occurrence draws its own dropout mask, as the reference's
+        per-call recomputation does), both RGCN layers and the pooling run once per chunk of instances, and one GRU call
+        per chunk takes its windows sorted by length.  Raises ValueError for a t with no graph before it."""
         times = list(graph_dict.keys())
-        time_unit = times[1] - times[0]
-        prev_t = 0
-        for t in t_list:
-            t = int(t)
+        time_unit = int(times[1] - times[0])
+        t_host = [int(t) for t in t_list]
+        keys, queries, prev_t = [], [], 0
+        for t in t_host:
             if t == 0:
                 continue
-            emb, _, _ = self.predict(t, graph_dict)
-            global_emb[prev_t] = emb.detach()
+            keys.append(prev_t)
+            queries.append(t)
             prev_t = t
-        last, _, _ = self.predict(int(t_list[-1]) + int(time_unit), graph_dict)
-        global_emb[int(t_list[-1])] = last.detach()
+        keys.append(t_host[-1])
+        queries.append(t_host[-1] + time_unit)
+        # predict's window (Aggregator.py:75-95): the <= seq_len keys before the first key >= t, in insertion order.  The
+        # first key >= t is the first position where the running maximum of the keys reaches t.
+        run_max = np.maximum.accumulate(np.asarray(times, dtype=np.int64))
+        end = np.searchsorted(run_max, np.asarray(queries, dtype=np.int64), side='left')
+        if (end == 0).any():
+            raise ValueError('RENet_global.get_global_emb: no graph before t = %d (empty window)'
+                             % queries[int(np.argmax(end == 0))])
+        begin = np.maximum(end - self.seq_len, 0)
+        lens = end - begin
+        sizes = np.asarray([as_history_graph(graph_dict[t]).number_of_nodes() for t in times], dtype=np.int64)
+        prefix = np.concatenate(([0], np.cumsum(sizes)))
+        win_nodes = prefix[end] - prefix[begin]
+        order = np.argsort(-lens, kind='stable')                 # the dense GRU takes sequences sorted by length, descending
+        emb = torch.empty(len(queries), self.h_dim, device=self.ent_embeds.device)
+        with torch.no_grad():
+            lo = 0
+            while lo < len(order):
+                hi, nodes = lo + 1, int(win_nodes[order[lo]])
+                while hi < len(order) and nodes + win_nodes[order[hi]] <= GLOBAL_EMB_NODE_BUDGET:
+                    nodes += int(win_nodes[order[hi]])
+                    hi += 1
+                wins = order[lo:hi]
+                occurrences = [times[j] for w in wins for j in range(begin[w], end[w])]
+                X = self.aggregator._global_info(occurrences, self.ent_embeds, graph_dict, reverse=False)
+                emb[torch.from_numpy(wins).to(emb.device)] = gru_final_hidden(self.encoder_global, X, lens[wins])
+                lo = hi
+        global_emb = dict()
+        for i, k in enumerate(keys):
+            global_emb[k] = emb[i].view(1, 1, self.h_dim)
         return global_emb
 
     def update_global_emb(self, t, graph_dict):
