@@ -535,6 +535,32 @@ int renet_decoder_soft_ce_bwd(const float* X, const float* W, const float* bias,
                               int32_t N, int32_t K, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Grouped top-k of a softmax-weighted decoder: the candidate scoring of the test-time roll-over (reference model.py:222-279,
+ * which calls pred_r_rank2, model.py:168-213, once per sampled entity and keeps torch.topk(joint.view(-1), k)).  The rows
+ * of X [M = G*R, K] come in G groups of R consecutive rows; row m has the weight row_weight[m] >= 0.
+ *     z = X @ W^T + bias,   p[m, n] = row_weight[m] * exp(z[m, n] - logsumexp_n z[m, n])
+ * For group g: values[g, :k] = the k largest p of its R*N entries, indices[g, :k] = their flat index r*N + n (r = the row's
+ * position in the group).  Ties at the k-th value go to the lower index.  order selects how a group's k entries are laid
+ * out:
+ *   RENET_TOPK_ORDER_INDEX : ascending index among the values above the k-th value, then ascending index among the values
+ *                            equal to it -- the order torch.topk(sorted=False) returns from its radix-select path;
+ *   RENET_TOPK_ORDER_VALUE : descending value, equal values by ascending index -- the order of a stable descending sort.
+ * 3xTF32 wgmma GEMM in two passes (logsumexp, then the candidates at or above a per-group lower bound of the k-th value);
+ * the logits never reach memory.  The candidates of a group go to a buffer of `capacity` entries (>= k).  If a group finds
+ * more, *needed (device int32) is set to the largest candidate count of any group and values / indices are not valid: call
+ * again with capacity >= *needed.  *needed = 0 means the output is complete.  No float atomics; the output is bitwise
+ * reproducible.  K % 4 == 0, R*N < 2^31, 1 <= k <= min(R*N, RENET_TOPK_MAX_K); X [M,K], W [N,K] row-major, 16-byte aligned;
+ * bias [N] may be NULL; values fp32 [G,k], indices int32 [G,k].
+ * ---------------------------------------------------------------------------------------------- */
+#define RENET_TOPK_ORDER_INDEX 0
+#define RENET_TOPK_ORDER_VALUE 1
+#define RENET_TOPK_MAX_K 16384
+int64_t renet_decoder_group_topk_workspace_bytes(int64_t G, int32_t R, int32_t N, int32_t K, int32_t capacity);
+int renet_decoder_group_topk(const float* X, const float* W, const float* bias, const float* row_weight, int64_t G, int32_t R,
+                             int32_t N, int32_t K, int32_t k, int32_t order, int32_t capacity, float* values, int32_t* indices,
+                             int32_t* needed, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Optimiser step of the reference training loop on FLAT fp32 buffers (reference train.py:140-142:
  * torch.nn.utils.clip_grad_norm_(model.parameters(), grad_norm); Adam(lr, weight_decay).step()).  The data-parallel
  * engine keeps all parameters / gradients as views into one flat buffer each (the gradient buffer is what NCCL

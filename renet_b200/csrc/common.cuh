@@ -144,7 +144,17 @@ struct EpiArgs {
   float* pdot;             // [2 * n_tiles, M] (EPI 3): sum of P * logit over the (row, half column tile)
   float* pmass;            // [2 * n_tiles, M] (EPI 3): sum of P over the same
   const float* rowmass;    // [M] (EPI 4): sum of P over the whole row
+  // grouped top-k selection (EPI 5): rows come in groups of sel_R; p = row_w[row] * exp(logit - lse[row]) with
+  // p >= tau[group] is appended as (p, (row % sel_R) * N + col) to that group's candidate buffer of sel_cap entries
+  const float* row_w;
+  const float* tau;
+  int32_t* sel_count;      // [G] candidates found per group (counts past sel_cap: the capacity the call needs)
+  float* sel_val;          // [G, sel_cap]
+  int32_t* sel_idx;        // [G, sel_cap]
+  int sel_R, sel_cap;
 };
+// p = w * exp(z - lse), rounded the same way wherever the grouped top-k forms it (decoder.cu, umma_gemm.cu)
+__device__ __forceinline__ float topk_prob(float z, float lse, float w) { return __fmul_rn(w, expf(__fsub_rn(z, lse))); }
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,

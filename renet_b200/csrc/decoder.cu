@@ -15,6 +15,21 @@
 // column tile); soft_ce_reduce_kernel combines a row's partials in fp64 in a fixed order:
 //     loss_i = lse_i * sum_c P_ic - sum_c P_ic z_ic,     dlogits_ic = (sum_c' P_ic' * softmax_ic - P_ic) * scale
 // and the backward pass runs the same three products on that dlogits.  No float atomics: every sum has a fixed order.
+//
+// Grouped top-k (renet_decoder_group_topk; the test-time roll-over's candidate scoring, reference model.py:222-279 with
+// pred_r_rank2, model.py:168-213): rows come in G groups of R, row m carries a weight w_m, and
+//     p[m, n] = w_m * exp(z[m, n] - lse_m)
+// is the joint probability of the reference's joint = p_e * p_o * p_r.  Per group, the k largest p and their flat indices
+// r * N + n, without ever writing the [G*R, N] logits:
+//   1. the EPI 1 pass without a target gives every (row, half column tile) partial max / sum of exp, then lse;
+//   2. every partial max is an actual logit, so the k-th largest of w_m * exp(pmax - lse_m) over a group's R * n_part
+//      partials is a lower bound tau_g of the group's k-th p (topk_tau_kernel, a block-wide radix select; 0 when the group
+//      has fewer than k partials);
+//   3. the EPI 5 pass recomputes the logits and appends every p >= tau_g to the group's candidate buffer; a group that
+//      finds more candidates than the buffer holds is reported through *needed and nothing of the call is valid;
+//   4. topk_final_kernel radix-selects the k-th (p descending, index ascending) candidate, so ties at the k-th value go to
+//      the lower index, and bitonic-sorts the k winners into the output order in shared memory.
+// Every step is either a fixed-order computation or an integer count, so the output is bitwise reproducible.
 #include "common.cuh"
 
 namespace renet {
@@ -34,7 +49,7 @@ __global__ void ce_reduce_kernel(const float* __restrict__ pmax, const float* __
   for (int i = 0; i < n_part; ++i) s += psum[(int64_t)i * M + r] * expf(pmax[(int64_t)i * M + r] - m);
   const float l = m + logf(s);
   lse[r] = l;
-  loss_rows[r] = l - tlogit[r];
+  if (loss_rows != nullptr) loss_rows[r] = l - tlogit[r];
 }
 
 __global__ void soft_ce_reduce_kernel(const float* __restrict__ pmax, const float* __restrict__ psum,
@@ -141,6 +156,156 @@ int zero_grad_pads(const DecBwdWs& w, int64_t M, int N, cudaStream_t stream) {
   if (w.ldE > N) RENET_CHECK_CUDA(cudaMemsetAsync(w.dlog, 0, (size_t)M * w.ldE * 4, stream));
   if (w.ldT > M) RENET_CHECK_CUDA(cudaMemsetAsync(w.dT, 0, (size_t)N * w.ldT * 4, stream));
   return RENET_OK;
+}
+
+// ---- grouped top-k ---------------------------------------------------------------------------------------------------
+// Bits of a probability as an order-preserving unsigned key (p >= 0; -0 counts as +0)
+__device__ __forceinline__ uint32_t prob_bits(float p) { return p > 0.f ? __float_as_uint(p) : 0u; }
+
+// The k-th largest (1-based, k <= n) of the n keys key(0 .. n-1), block-wide: a radix select over 8-bit digits, most
+// significant first.  Every thread gets the result.  hist: 256 ints of shared memory.
+template <typename KeyT, typename F>
+__device__ KeyT block_kth_largest(int64_t n, int64_t k, F key, int* hist) {
+  __shared__ KeyT s_prefix;
+  __shared__ int64_t s_rank;
+  KeyT prefix = 0, mask = 0;
+  int64_t rank = k;                                   // the rank still wanted among the keys that match prefix
+  for (int shift = (int)sizeof(KeyT) * 8 - 8; shift >= 0; shift -= 8) {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const KeyT v = key(i);
+      if ((v & mask) == prefix) atomicAdd(hist + (int)((v >> shift) & 255), 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int64_t above = 0;
+      int d = 255;
+      for (; d > 0 && above + hist[d] < rank; --d) above += hist[d];
+      s_prefix = prefix | ((KeyT)d << shift);
+      s_rank = rank - above;
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    rank = s_rank;
+    mask |= (KeyT)255 << shift;
+  }
+  return prefix;
+}
+
+// tau[g] = the k-th largest of w_m * exp(pmax[i, m] - lse_m) over the rows m of group g and the partials i (0 when the
+// group has fewer than k partials).  One block per group.
+__global__ void __launch_bounds__(256) topk_tau_kernel(const float* __restrict__ pmax, const float* __restrict__ lse,
+                                                       const float* __restrict__ row_w, int n_part, int R, int64_t M, int k,
+                                                       float* __restrict__ tau) {
+  __shared__ int hist[256];
+  const int64_t g = blockIdx.x;
+  const int64_t n = (int64_t)R * n_part;
+  if (n < k) {
+    if (threadIdx.x == 0) tau[g] = 0.f;
+    return;
+  }
+  const int64_t m0 = g * R;
+  auto key = [&](int64_t i) -> uint32_t {
+    const int64_t part = i / R, m = m0 + (i - part * R);
+    return prob_bits(topk_prob(__ldg(pmax + part * M + m), __ldg(lse + m), __ldg(row_w + m)));
+  };
+  const uint32_t t = block_kth_largest<uint32_t>(n, k, key, hist);
+  if (threadIdx.x == 0) tau[g] = __uint_as_float(t);
+}
+
+constexpr int kTopkFinalThreads = 512;
+
+// One block per group: the k best candidates by (p descending, index ascending), written in the caller's order.
+// sort_n = the power of two >= k the shared-memory sort runs over.
+__global__ void __launch_bounds__(kTopkFinalThreads) topk_final_kernel(const float* __restrict__ cand_val,
+                                                                       const int32_t* __restrict__ cand_idx,
+                                                                       const int32_t* __restrict__ count, int cap, int k,
+                                                                       int order, int sort_n, float* __restrict__ values,
+                                                                       int32_t* __restrict__ indices, int32_t* __restrict__ needed) {
+  extern __shared__ unsigned long long s_keys[];      // [sort_n]
+  __shared__ int hist[256];
+  __shared__ int s_fill;
+  const int64_t g = blockIdx.x;
+  const int n = count[g];
+  if (n > cap) {                                       // the candidates did not fit: the caller retries with *needed
+    if (threadIdx.x == 0) atomicMax(needed, n);
+    return;
+  }
+  const float* cv = cand_val + g * cap;
+  const int32_t* ci = cand_idx + g * cap;
+  // larger key = better: p descending, then index ascending; keys are distinct because indices are
+  auto key = [&](int64_t i) -> unsigned long long {
+    return ((unsigned long long)prob_bits(cv[i]) << 32) | (uint32_t)~(uint32_t)ci[i];
+  };
+  const unsigned long long kth = block_kth_largest<unsigned long long>(n, k, key, hist);
+  const uint32_t kth_p = (uint32_t)(kth >> 32);
+  if (threadIdx.x == 0) s_fill = 0;
+  __syncthreads();
+  // the k winners, each as an ascending sort key of the output order:
+  //   order 1: p descending, ties by index ascending
+  //   order 0: index ascending among the p above the k-th p, then index ascending among those equal to it
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const unsigned long long v = key(i);
+    if (v < kth) continue;
+    const uint32_t p = (uint32_t)(v >> 32), idx = ~(uint32_t)v;
+    const unsigned long long sk = order == 1 ? ((unsigned long long)~p << 32) | idx
+                                             : ((unsigned long long)(p == kth_p) << 63) | ((unsigned long long)idx << 32) | p;
+    s_keys[atomicAdd(&s_fill, 1)] = sk;
+  }
+  for (int i = k + threadIdx.x; i < sort_n; i += blockDim.x) s_keys[i] = ~0ull;
+  __syncthreads();
+  for (int size = 2; size <= sort_n; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int i = threadIdx.x; i < sort_n / 2; i += blockDim.x) {
+        const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
+        const unsigned long long a = s_keys[lo], b = s_keys[hi];
+        if ((a > b) == ((lo & size) == 0)) {
+          s_keys[lo] = b;
+          s_keys[hi] = a;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (int j = threadIdx.x; j < k; j += blockDim.x) {
+    const unsigned long long sk = s_keys[j];
+    uint32_t p, idx;
+    if (order == 1) {
+      p = ~(uint32_t)(sk >> 32);
+      idx = (uint32_t)sk;
+    } else {
+      p = (uint32_t)sk;
+      idx = (uint32_t)(sk >> 32) & 0x7fffffffu;
+    }
+    values[g * k + j] = __uint_as_float(p);
+    indices[g * k + j] = (int32_t)idx;
+  }
+}
+
+struct TopkWs {
+  uint8_t* Wp;
+  float *pmax, *psum, *lse, *tau, *cand_val;
+  int32_t *count, *cand_idx;
+  int64_t total;
+};
+TopkWs carve_topk(void* base, int64_t G, int R, int N, int K, int cap) {
+  TopkWs w;
+  char* p = (char*)base;
+  int64_t off = 0;
+  auto take = [&](int64_t bytes) { char* q = base ? p + off : nullptr; off += align256(bytes); return q; };
+  const int64_t M = G * R;
+  const int n_part = 2 * ((N + 199) / 200);
+  w.Wp = (uint8_t*)take(umma_packed_bytes(N, K));
+  w.pmax = (float*)take((int64_t)n_part * M * 4);
+  w.psum = (float*)take((int64_t)n_part * M * 4);
+  w.lse = (float*)take(M * 4);
+  w.tau = (float*)take(G * 4);
+  w.count = (int32_t*)take(G * 4);
+  w.cand_val = (float*)take(G * cap * 4);
+  w.cand_idx = (int32_t*)take(G * cap * 4);
+  w.total = off;
+  return w;
 }
 
 }  // namespace
@@ -253,6 +418,67 @@ int renet_decoder_soft_ce_bwd(const float* X, const float* W, const float* bias,
   rc = umma_gemm_prepacked_ex(X, nullptr, K, w.Wp, w.dlog, w.ldE, bias, M, N, K, false, 1, 0, 0, 0, 4, epi, 1, 0, stream);
   if (rc < 0) return rc;
   return grad_products(X, W, dX, dW, dbias, M, N, K, w, stream);
+}
+
+int64_t renet_decoder_group_topk_workspace_bytes(int64_t G, int32_t R, int32_t N, int32_t K, int32_t capacity) {
+  return carve_topk(nullptr, G, R, N, K, capacity).total + 256;
+}
+
+int renet_decoder_group_topk(const float* X, const float* W, const float* bias, const float* row_weight, int64_t G, int32_t R,
+                             int32_t N, int32_t K, int32_t k, int32_t order, int32_t capacity, float* values, int32_t* indices,
+                             int32_t* needed, void* workspace, int64_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  RENET_CHECK_ARG(G >= 0 && R > 0 && N > 0 && K > 0 && K % 4 == 0 && (int64_t)R * N < (int64_t(1) << 31),
+                  "renet_decoder_group_topk: bad shape (K must be a multiple of 4, R * N < 2^31)");
+  RENET_CHECK_ARG(k >= 1 && (int64_t)k <= (int64_t)R * N, "renet_decoder_group_topk: k = %d outside [1, R * N = %lld]", k,
+                  (long long)R * N);
+  RENET_CHECK_ARG(k <= RENET_TOPK_MAX_K, "renet_decoder_group_topk: k = %d above RENET_TOPK_MAX_K = %d", k, RENET_TOPK_MAX_K);
+  RENET_CHECK_ARG(order == RENET_TOPK_ORDER_INDEX || order == RENET_TOPK_ORDER_VALUE, "renet_decoder_group_topk: unknown order %d",
+                  order);
+  RENET_CHECK_ARG(capacity >= k, "renet_decoder_group_topk: capacity %d < k = %d", capacity, k);
+  RENET_CHECK_ARG(needed != nullptr, "renet_decoder_group_topk: null pointer");
+  if (G == 0) return RENET_OK;
+  RENET_CHECK_ARG(X && W && row_weight && values && indices && workspace, "renet_decoder_group_topk: null pointer");
+  RENET_CHECK_ARG(workspace_bytes >= renet_decoder_group_topk_workspace_bytes(G, R, N, K, capacity),
+                  "renet_decoder_group_topk: workspace too small");
+  RENET_CHECK_ARG(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
+                  "renet_decoder_group_topk: X and W must be 16-byte aligned");
+  static bool attr = false;
+  if (!attr) {
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(topk_final_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RENET_TOPK_MAX_K * 8));
+    attr = true;
+  }
+  void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
+  TopkWs w = carve_topk(base, G, R, N, K, capacity);
+  const int64_t M = G * R;
+  const int n_part = 2 * ((N + 199) / 200);
+  RENET_CHECK_CUDA(cudaMemsetAsync(needed, 0, 4, stream));
+  RENET_CHECK_CUDA(cudaMemsetAsync(w.count, 0, (size_t)G * 4, stream));
+  // 1. lse of every row: the cross-entropy forward epilogue without a target
+  int rc = umma_pack_b(W, 1, K, N, K, w.Wp, 0, stream);          // logical B[k][n] = W[n*K + k]
+  if (rc) return rc;
+  EpiArgs epi{};
+  epi.pmax = w.pmax; epi.psum = w.psum;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 1, epi, 1, 0, stream);
+  if (rc < 0) return rc;
+  ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.pmax, w.psum, nullptr, n_part, M, w.lse, nullptr);
+  RENET_CHECK_LAUNCH("ce_reduce_kernel");
+  // 2. per-group threshold from the partial maxima
+  topk_tau_kernel<<<(unsigned)G, 256, 0, stream>>>(w.pmax, w.lse, row_weight, n_part, R, M, k, w.tau);
+  RENET_CHECK_LAUNCH("topk_tau_kernel");
+  // 3. the candidates at or above it
+  EpiArgs sel{};
+  sel.lse = w.lse; sel.row_w = row_weight; sel.tau = w.tau; sel.sel_count = w.count; sel.sel_val = w.cand_val;
+  sel.sel_idx = w.cand_idx; sel.sel_R = R; sel.sel_cap = capacity;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 5, sel, 1, 0, stream);
+  if (rc < 0) return rc;
+  // 4. the k best of each group's candidates, in the requested order
+  int sort_n = 2;
+  while (sort_n < k) sort_n <<= 1;
+  topk_final_kernel<<<(unsigned)G, kTopkFinalThreads, (size_t)sort_n * 8, stream>>>(w.cand_val, w.cand_idx, w.count, capacity, k,
+                                                                                     order, sort_n, values, indices, needed);
+  RENET_CHECK_LAUNCH("topk_final_kernel");
+  return RENET_OK;
 }
 
 }  // extern "C"

@@ -332,13 +332,17 @@ __device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], flo
 
 // Fused-epilogue modes of the packed kernel (the decoder of model.py:89-91,97-100: logits = X @ W^T + b, cross-entropy):
 //   EPI 0  C = acc (+bias) (+C)                                   -- plain GEMM
-//   EPI 1  per (row, half column tile): running max and sum of exp of the logits, and the target's logit -- the
-//          [M, N] logits never reach memory; ce_reduce_kernel turns the partials into logsumexp and the loss
+//   EPI 1  per (row, half column tile): running max and sum of exp of the logits, and the target's logit (skipped when
+//          target is null) -- the [M, N] logits never reach memory; ce_reduce_kernel turns the partials into logsumexp
+//          and the loss
 //   EPI 2  dlogits[row, col] = (exp(logit - lse[row]) - [col == target[row]]) * scale, written to memory for the two
 //          gradient GEMMs (the backward pass recomputes the logits instead of keeping them)
 //   EPI 3  soft targets P (global_model.py's soft cross-entropy): EPI 1's running max and sum of exp, and the sums of
 //          P * logit and of P, with P read at the logit's own position; soft_ce_reduce_kernel (decoder.cu) combines them
 //   EPI 4  dlogits[row, col] = (rowmass[row] * exp(logit - lse[row]) - P[row, col]) * scale, written as in EPI 2
+//   EPI 5  grouped top-k candidates (renet_decoder_group_topk): p = row_w[row] * exp(logit - lse[row]); every p at or above
+//          its group's threshold is appended to the group's candidate buffer (an integer atomic picks the slot; the final
+//          select sorts, so no output depends on the slot order)
 // grid.x = min(units, SMs).  Batched GEMMs (the two GRU encoders) have per-batch operand offsets.  Split-K (long-K,
 // few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
 // partial product to C + s*split_c; the caller sums the partials.
@@ -504,12 +508,17 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     acc_store(acc, sC, P_CLD, wt);
     named_bar_sync(1 + g, 128);
     if (wt >= 64) continue;
-    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI >= 3;
+    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI == 3 || EPI == 4, SEL = EPI == 5;
     const int64_t gr = w.row_base + 64 * g + wt;
     const float* srow = sC + wt * P_CLD;
     float run_m = -3.0e38f, run_s = 0.f;               // EPI 1, 3: running max / sum of exp of this (row, half tile)
     float run_pz = 0.f, run_p = 0.f;                   // EPI 3: sums of P * logit and of P
-    const int tgt = (!SOFT && gr < M) ? __ldg(epi.target + gr) : -1;
+    // EPI 1 without a target (the grouped top-k's first pass) only reduces the running max / sum of exp
+    const int tgt = (!SOFT && !SEL && gr < M && epi.target != nullptr) ? __ldg(epi.target + gr) : -1;
+    const int64_t sel_g = SEL ? gr / epi.sel_R : 0;
+    const int sel_base = SEL ? (int)(gr - sel_g * epi.sel_R) * N : 0;     // flat index of the row's column 0 in its group
+    const float row_w = (SEL && gr < M) ? __ldg(epi.row_w + gr) : 0.f;
+    const float sel_tau = (SEL && gr < M) ? __ldg(epi.tau + sel_g) : 0.f;
     const float row_lse = (!FWD && gr < M) ? __ldg(epi.lse + gr) : 0.f;
     const float row_mass = (EPI == 4 && gr < M) ? __ldg(epi.rowmass + gr) : 0.f;
     const float gscale = (!FWD) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
@@ -546,6 +555,19 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
             }
           run_s = run_s * expf(run_m - nm) + add;
           run_m = nm;
+        } else if (SEL) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            if (i < nv) {
+              const float p = topk_prob(o[i], row_lse, row_w);
+              if (p >= sel_tau) {                                      // rare: about k per group pass the threshold
+                const int slot = atomicAdd(epi.sel_count + sel_g, 1);
+                if (slot < epi.sel_cap) {
+                  epi.sel_val[sel_g * epi.sel_cap + slot] = p;
+                  epi.sel_idx[sel_g * epi.sel_cap + slot] = sel_base + n0 + cc + i;
+                }
+              }
+            }
         } else {
           float* dp = Cz + gr * ldc + n0 + cc;
 #pragma unroll
@@ -888,6 +910,7 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(2)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(3)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(4)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(5)));
     attr2 = true;
   }
   const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
@@ -902,6 +925,7 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
   else if (epi_mode == 2) RENET_UMMA_LAUNCH(false, 2);
   else if (epi_mode == 3) RENET_UMMA_LAUNCH(false, 3);
   else if (epi_mode == 4) RENET_UMMA_LAUNCH(false, 4);
+  else if (epi_mode == 5) RENET_UMMA_LAUNCH(false, 5);
   else if (a_index) RENET_UMMA_LAUNCH(true, 0);
   else RENET_UMMA_LAUNCH(false, 0);
 #undef RENET_UMMA_LAUNCH
@@ -1034,7 +1058,7 @@ static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, 
 }
 
 // C[b] (+)= A[b] @ Bpacked[b] (+bias[b]) for b < batch; strides in elements (A, C) / bytes (Bp).
-// epi_mode 1-4: fused cross-entropy epilogues (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
+// epi_mode 1-4: fused cross-entropy epilogues, 5: grouped top-k candidates (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,

@@ -5,7 +5,10 @@ the forward pass.  ``nn.Linear`` modules stay the parameter holders (state_dict 
 
 ``decoder_soft_cross_entropy(x, weight, bias, soft_targets)`` is the global model's loss head on the same engine
 (renet_decoder_soft_ce_fwd / _bwd): the reference's ``soft_cross_entropy(F.linear(x, weight, bias), soft_targets)``
-(utils.py:287-290, fp64 log-softmax, mean over rows), returned as a float64 scalar like the reference's."""
+(utils.py:287-290, fp64 log-softmax, mean over rows), returned as a float64 scalar like the reference's.
+
+``decoder_group_topk(x, weight, bias, row_weight, R, k)`` is the test-time roll-over's candidate scoring on the same engine
+(renet_decoder_group_topk): per group of R rows, the k largest row_weight * softmax(F.linear(x, weight, bias)) entries."""
 import torch
 
 from . import _lib
@@ -92,3 +95,45 @@ class _DecoderSoftCEFn(torch.autograd.Function):
 
 def decoder_soft_cross_entropy(x, weight, bias, soft_targets):
     return _DecoderSoftCEFn.apply(x, weight, bias, soft_targets)
+
+
+ORDER_INDEX, ORDER_VALUE = 0, 1          # RENET_TOPK_ORDER_INDEX / RENET_TOPK_ORDER_VALUE
+TOPK_MAX_K = 16384                       # RENET_TOPK_MAX_K
+
+
+def group_topk_capacity(k, size):
+    """First candidate-buffer size per group: a few times k covers the entries at or above the threshold in practice; a
+    call that needs more says so and is repeated with the exact size."""
+    return int(min(size, 4 * k + 256))
+
+
+def decoder_group_topk(x, weight, bias, row_weight, R, k, order=ORDER_INDEX, capacity=None):
+    """renet_decoder_group_topk: the rows of x [G*R, K] in groups of R, p[m, n] = row_weight[m] * softmax(x @ weight^T +
+    bias)[m, n]; per group the k largest p and their flat indices r * N + n (ties to the lower index), laid out in
+    ``order``.  Returns (values float32 [G, k], indices int64 [G, k]).  ``capacity``: the first candidate-buffer size (a
+    group that finds more candidates makes the call run once more with the size it reported)."""
+    L, P = _lib.lib(), _lib.ptr
+    _lib.require_cuda(x, weight, bias, row_weight)
+    x, weight = x.contiguous(), weight.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    row_weight = row_weight.to(torch.float32).contiguous()
+    M, K = x.shape
+    N = weight.shape[0]
+    if M % R != 0 or row_weight.numel() != M:
+        raise ValueError('decoder_group_topk: %d rows do not form groups of R = %d with one weight each' % (M, R))
+    G = M // R
+    dev = x.device
+    values = torch.empty(G, k, device=dev)
+    indices = torch.empty(G, k, dtype=torch.int32, device=dev)
+    needed = torch.zeros(1, dtype=torch.int32, device=dev)
+    cap = int(capacity) if capacity is not None else group_topk_capacity(k, R * N)
+    cap = max(cap, k)
+    while True:
+        nbytes = int(L.renet_decoder_group_topk_workspace_bytes(G, R, N, K, cap))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _lib.check(L.renet_decoder_group_topk(P(x), P(weight), P(bias), P(row_weight), G, R, N, K, k, order, cap, P(values),
+                                              P(indices), P(needed), P(ws), nbytes, _lib.stream()), 'renet_decoder_group_topk')
+        need = int(needed.item())
+        if need == 0:
+            return values, indices.long()
+        cap = need

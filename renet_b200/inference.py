@@ -18,6 +18,10 @@ import torch
 
 from .graph import get_big_graph
 
+#: (entity, relation) sequences pred_r_topk encodes and scores per chunk: 16 384 sequences of up to seq_len steps keep the
+#: batched history graph, the GRU inputs and the decoder's partial sums within a few hundred MB
+ROLLOVER_SEQ_BUDGET = 16384
+
 
 def rank_with_ties(scores, label):
     """model.py:373-379: rank = #(strictly greater) + (#equal - 1)/2 + 1."""
@@ -136,6 +140,98 @@ class RENetInference:
         p_r = torch.softmax(ob_pred_r.view(-1), dim=0)
         return p_o * p_r.view(R, 1)
 
+    def pred_r_topk(self, entities, weights, k, subject=True, capacity=None):
+        """pred_r_rank2 followed by torch.topk for many entities at once (model.py:168-213, 236-240).  For entity
+        entities[i]: the k largest entries of weights[i] * pred_r_rank2([entities[i]] * R, arange(R), subject).view(-1)
+        and their codes r * in_dim + o, as (values float32 [n, k], codes int64 [n, k]) on the model's device.
+
+        The test-time histories of a chunk of entities are encoded in one batched call (one store entry per entity, each
+        repeated once per relation, through the C++ / device batcher, over a graph store built for the chunk in which
+        every entity has its own copies of its history's graphs); entities without history get zero s_h / s_q as in
+        pred_r_rank2.  The joint distribution is never materialised: renet_decoder_group_topk scores
+        [ent_e | s_h(e, r) | rel_r] against ``linear`` with the row weights weights[i] * softmax_r(linear_r([ent_e | s_q_e]))
+        and selects each entity's k best in one pass.  A group's k entries come in the order torch.topk(sorted=False) gives
+        on a CUDA tensor of R * in_dim values (ORDER_INDEX: the values above the k-th one in index order, then those equal
+        to it; measured on an H100 with PyTorch 2.11 from R * in_dim = 9 600 to 5.9 M), since the roll-over's final
+        selection and the order of its cache updates depend on that layout."""
+        from .decoder import ORDER_INDEX, decoder_group_topk
+        from .hoststore import GraphStore, HistoryStore
+        R, h, N = self.num_rels, self.h_dim, self.in_dim
+        dev = self.ent_embeds.device
+        ents = torch.as_tensor(entities).reshape(-1).long().cpu().numpy()
+        wts = torch.as_tensor(weights).reshape(-1).to(device=dev, dtype=torch.float32)
+        n = len(ents)
+        if wts.numel() != n:
+            raise ValueError('pred_r_topk: %d entities but %d weights' % (n, wts.numel()))
+        values = torch.empty(n, k, device=dev)
+        codes = torch.empty(n, k, dtype=torch.long, device=dev)
+        rel_embeds, reverse = self._direction(subject)
+        hist = self.s_hist_test if subject else self.o_hist_test
+        hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
+        per = max(1, ROLLOVER_SEQ_BUDGET // R)
+        rel_rows = torch.arange(R, device=dev)
+        for c0 in range(0, n, per):
+            ce = ents[c0:c0 + per]
+            nc = len(ce)
+            s_h = torch.zeros(nc, R, h, device=dev)
+            s_q = torch.zeros(nc, h, device=dev)
+            has = np.flatnonzero([len(hist[e]) != 0 for e in ce])
+            if len(has):
+                he = ce[has]
+                # The batched history graph has one component per timestamp, induced by the nodes of every sample in
+                # the batch (utils.py:158-181), so an entity's encoding depends on what it is batched with.  Each entity
+                # gets its own copies of its history's graphs, under keys of its own, to encode exactly what
+                # pred_r_rank2 encodes alone.
+                span = max(len(hist_t[e]) for e in he)
+                keys = [[j * span + i for i in range(len(hist_t[e]))] for j, e in enumerate(he)]
+                graphs, glob = {}, {}
+                for e, ks in zip(he, keys):
+                    for v, t in zip(ks, hist_t[e]):
+                        graphs[v], glob[v] = self.graph_dict[int(t)], self.global_emb[int(t)]
+                gs = GraphStore(graphs)
+                store = HistoryStore([hist[e] for e in he], keys, he, gs, dedupe=False)
+                view = store.select(np.repeat(np.arange(len(he)), R))
+                s_dev = torch.from_numpy(np.repeat(he, R)).to(dev)
+                r_dev = rel_rows.repeat(len(he))
+                sh, sq, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, glob, reverse,
+                                                    self.encoder, self.encoder_r)
+                # the encoder returns the sequences length-sorted: row j is sample sample_order[j] of the view
+                idx = hb.sample_order(dev)
+                sh_v, sq_v = torch.empty_like(sh), torch.empty_like(sq)
+                sh_v[idx], sq_v[idx] = sh, sq
+                has_dev = torch.from_numpy(has).to(dev)
+                s_h[has_dev] = sh_v.view(len(he), R, h)
+                s_q[has_dev] = sq_v.view(len(he), R, h)[:, 0]                 # s_q does not depend on r (model.py:96)
+            ent = self.ent_embeds[torch.from_numpy(ce).to(dev)]
+            p_r = torch.softmax(self.linear_r(torch.cat((ent, s_q), dim=1)), dim=1)                    # [nc, R]
+            row_w = (wts[c0:c0 + nc].view(-1, 1) * p_r).reshape(-1)
+            x = torch.cat((ent.repeat_interleave(R, dim=0), s_h.view(nc * R, h), rel_embeds.repeat(nc, 1)), dim=1)
+            v, i = decoder_group_topk(x, self.linear.weight, self.linear.bias, row_w, R, k, ORDER_INDEX, capacity)
+            values[c0:c0 + nc] = v
+            codes[c0:c0 + nc] = i
+        return values, codes
+
+    def _pick_candidates(self, picks, prob, subject):
+        """The num_k most probable (relation, entity) continuations of every pick (model.py:236-240): host tensors
+        (joint probabilities [n_picks, num_k], codes r * in_dim + o [n_picks, num_k]) in picks order.  On the GPU every
+        distinct entity is scored once, all of them in one batched pass (pred_r_topk: its scores depend on the entity
+        only), and its list is repeated for each pick of it.  A model on the host has no kernels to run (the host-logic
+        checks substitute a host encoder): its picks are scored one by one through pred_r_rank2, as the reference does."""
+        K, R = self.num_k, self.num_rels
+        if self.ent_embeds.is_cuda:
+            uniq, inverse = torch.unique(picks, return_inverse=True)
+            top_p, top_i = self.pred_r_topk(uniq, prob[uniq], K, subject=subject)
+            inverse = inverse.cpu()
+            return top_p.cpu()[inverse], top_i.cpu()[inverse]
+        lists, inds = [], []
+        for e, p_e in zip(picks, prob[picks]):
+            ee = torch.full((R,), int(e), dtype=torch.long)
+            joint = float(p_e) * self.pred_r_rank2(ee, torch.arange(R), subject=subject)
+            top_p, top_i = torch.topk(joint.view(-1), K, sorted=False)
+            lists.append(top_p.view(-1).cpu())
+            inds.append(top_i.view(-1).cpu())
+        return torch.stack(lists), torch.stack(inds)
+
     def _roll_over(self, t, global_model):
         """model.py:222-330: the stream moved to a new timestamp.  Sample num_k subjects (objects) from the global
         model's distribution, score every (relation, entity) continuation for them, keep the num_k most probable
@@ -153,15 +249,9 @@ class RENetInference:
             picks = torch.distributions.categorical.Categorical(prob).sample(torch.Size([K]))
             # NOTE: the reference de-duplicates with a set of 0-dim tensors (model.py:228-234), which never matches
             # (tensors hash by identity), so repeated samples are scored again and kept as separate entries.
-            lists, inds, ents = [], [], []
-            for e, p_e in zip(picks, prob[picks]):
-                ee = torch.full((R,), int(e), dtype=torch.long)
-                joint = float(p_e) * self.pred_r_rank2(ee, torch.arange(R), subject=subject)
-                top_p, top_i = torch.topk(joint.view(-1), K, sorted=False)
-                lists.append(top_p.view(-1).cpu())
-                inds.append(top_i.view(-1).cpu())
-                ents.append(int(e))
-            _, cand = torch.topk(torch.cat(lists), K, sorted=False)
+            lists, inds = self._pick_candidates(picks, prob, subject)                     # [K picks, K] in picks order
+            ents = picks.tolist()
+            _, cand = torch.topk(lists.view(-1), K, sorted=False)
             for c in cand.tolist():
                 e = ents[c // K]
                 last[subject] = e
