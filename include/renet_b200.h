@@ -403,6 +403,17 @@ int renet_host_plan_batch(
     const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort,
     int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
     int64_t* sizes);
+/* renet_host_plan_batch with isolation groups: sample_group[i] (one entry per selected sample, i.e. per sample_idx[i]) is
+ * the group of that sample, and the components are the distinct (group, timestamp) pairs in first-appearance order
+ * instead of the distinct timestamps, so every group's nodes, edges and read-out rows are what that group batched alone
+ * gives (up to the node-id offset).  sample_group == NULL is renet_host_plan_batch, bit for bit.  Same outputs and layout;
+ * comp_graph may then repeat a graph. */
+int renet_host_plan_batch_grouped(
+    int64_t T, const int64_t* g_node_off, const int32_t* g_node_ent, const int64_t* g_edge_off,
+    const int64_t* h_samp_off, const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow,
+    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, const int64_t* sample_group, int64_t B,
+    int32_t sort, int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
+    int64_t* sizes);
 int64_t renet_induce_workspace_bytes(int64_t e_cand);
 int renet_induce_edges(const int64_t* g_edge_off, const int32_t* g_src, const int32_t* g_dst,
                        const int32_t* g_type_s, const int32_t* g_type_o, const int32_t* comp_graph,
@@ -559,6 +570,24 @@ int64_t renet_decoder_group_topk_workspace_bytes(int64_t G, int32_t R, int32_t N
 int renet_decoder_group_topk(const float* X, const float* W, const float* bias, const float* row_weight, int64_t G, int32_t R,
                              int32_t N, int32_t K, int32_t k, int32_t order, int32_t capacity, float* values, int32_t* indices,
                              int32_t* needed, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Rank of a label among a decoder's logits: the test-time scoring of reference model.py:365-419 (evaluate /
+ * evaluate_filter) for M rows at once.  z = X @ W^T + bias; row m has the label l = label[m] in [0, N).
+ *   loss_rows[m] = logsumexp_n z[m, n] - z[m, l]                 (F.cross_entropy of the row)
+ *   counts[4m + 0] = #{n : z[m, n] > z[m, l]},  counts[4m + 1] = #{n : z[m, n] == z[m, l]}   (the label included)
+ *   counts[4m + 2], counts[4m + 3]: the same with p_n = sigmoid(z[m, n]) (torch.sigmoid's fp32 rounding, bit for bit),
+ *       p_n = 0 for every n != l in the row's exclusion list excl_col[excl_begin[m] .. excl_end[m]) (int32, ascending;
+ *       rows may share a range; l in it is ignored), compared with sigmoid(z[m, l]).  excl_col == NULL: both are 0.
+ * The reference's rank is counts[gt] + (counts[eq] - 1) / 2 + 1.  3xTF32 wgmma GEMM in two passes (logsumexp and the
+ * label's logit, then the counts); the logits never reach memory, the label's logit is the same bits in both passes.  No
+ * float atomics; the output is bitwise reproducible.  K % 4 == 0; X [M,K], W [N,K] row-major, 16-byte aligned; bias [N]
+ * may be NULL; counts int32 [M,4].
+ * ---------------------------------------------------------------------------------------------- */
+int64_t renet_decoder_rank_workspace_bytes(int64_t M, int32_t N, int32_t K);
+int renet_decoder_rank(const float* X, const float* W, const float* bias, const int32_t* label, const int32_t* excl_col,
+                       const int32_t* excl_begin, const int32_t* excl_end, float* loss_rows, int32_t* counts, int64_t M, int32_t N,
+                       int32_t K, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Optimiser step of the reference training loop on FLAT fp32 buffers (reference train.py:140-142:

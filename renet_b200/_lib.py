@@ -56,6 +56,7 @@ SIGNATURES = {
     'renet_set_host_threads': (ctypes.c_int, [ctypes.c_int]),
     'renet_host_assemble_batch': (ctypes.c_int, [_i64] + [_vp] * 13 + [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _vp, _vp, _i32, _vp]),
     'renet_host_plan_batch': (ctypes.c_int, [_i64] + [_vp] * 10 + [_i64, _i32, _vp, _vp, _i64, _vp, _i32, _vp]),
+    'renet_host_plan_batch_grouped': (ctypes.c_int, [_i64] + [_vp] * 11 + [_i64, _i32, _vp, _vp, _i64, _vp, _i32, _vp]),
     'renet_induce_workspace_bytes': (_i64, [_i64]),
     'renet_induce_edges': (ctypes.c_int, [_vp] * 9 + [_i64, _i64, _i64] + [_vp] * 7 + [_i64, _vp]),
     'renet_encode_fwd': (ctypes.c_int, [_vp] * 12 + [_i64, _i64, _i32] + [_vp] * 9 + [_i32] + [_vp] * 10 +
@@ -79,6 +80,8 @@ SIGNATURES = {
     'renet_decoder_group_topk_workspace_bytes': (_i64, [_i64, _i32, _i32, _i32, _i32]),
     'renet_decoder_group_topk': (ctypes.c_int, [_vp] * 4 + [_i64, _i32, _i32, _i32, _i32, _i32, _i32] + [_vp] * 4 +
                                  [_i64, _vp]),
+    'renet_decoder_rank_workspace_bytes': (_i64, [_i64, _i32, _i32]),
+    'renet_decoder_rank': (ctypes.c_int, [_vp] * 9 + [_i64, _i32, _i32, _vp, _i64, _vp]),
     'renet_grad_sumsq_workspace_bytes': (_i64, []),
     'renet_grad_sumsq': (ctypes.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _vp]),
     'renet_adam_step': (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64] + [ctypes.c_float] * 5 + [_i64, _vp, ctypes.c_float, ctypes.c_float, _vp]),

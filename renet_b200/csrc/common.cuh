@@ -152,9 +152,20 @@ struct EpiArgs {
   float* sel_val;          // [G, sel_cap]
   int32_t* sel_idx;        // [G, sel_cap]
   int sel_R, sel_cap;
+  // rank counting (EPI 6): every logit of row `row` is compared with tlogit[row] (the label's logit from the EPI 1 pass)
+  // and rank_counts[4 * row + {0, 1, 2, 3}] += {#greater, #equal, #filtered greater, #filtered equal} (integer atomics).
+  // Filtered: sigmoid, with the columns of excl_col[excl_begin[row] .. excl_end[row]) (sorted) other than target[row]
+  // set to 0; excl_col == nullptr skips the filtered counts.
+  const int32_t* excl_col;
+  const int32_t* excl_begin;
+  const int32_t* excl_end;
+  int32_t* rank_counts;
 };
 // p = w * exp(z - lse), rounded the same way wherever the grouped top-k forms it (decoder.cu, umma_gemm.cu)
 __device__ __forceinline__ float topk_prob(float z, float lse, float w) { return __fmul_rn(w, expf(__fsub_rn(z, lse))); }
+// torch.sigmoid of a CUDA float tensor, bit for bit: 1 / (1 + exp(-z)) with the accurate expf and an IEEE division.  In fp32
+// it rounds to exactly 1 above z ~ 17 and to exactly 0 once exp(-z) overflows, and filtered ranks count those ties.
+__device__ __forceinline__ float torch_sigmoid(float z) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-z))); }
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,

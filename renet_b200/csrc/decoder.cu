@@ -30,6 +30,14 @@
 //   4. topk_final_kernel radix-selects the k-th (p descending, index ascending) candidate, so ties at the k-th value go to
 //      the lower index, and bitonic-sorts the k winners into the output order in shared memory.
 // Every step is either a fixed-order computation or an integer count, so the output is bitwise reproducible.
+//
+// Rank counts (renet_decoder_rank; test-time scoring, reference model.py:365-419): per row, the label's rank among the row's
+// logits, raw and filtered, by the tie rule #greater + (#equal - 1) / 2 + 1, without writing the [M, N] logits:
+//   1. the EPI 1 pass with the label as target gives the partials and the label's logit tlogit; ce_reduce_kernel turns
+//      them into lse and loss_rows;
+//   2. the EPI 6 pass recomputes the logits with the same packed W, bias and tile mapping, so the label's own logit equals
+//      tlogit bit for bit, and counts the logits above / equal to it, and the sigmoids above / equal to the label's with the
+//      row's exclusion list zeroed.  The counts are integers added with integer atomics: the output is reproducible.
 #include "common.cuh"
 
 namespace renet {
@@ -308,6 +316,19 @@ TopkWs carve_topk(void* base, int64_t G, int R, int N, int K, int cap) {
   return w;
 }
 
+struct RankWs {
+  DecWs fwd;
+  float* lse;
+  int64_t total;
+};
+RankWs carve_rank(void* base, int64_t M, int N, int K) {
+  RankWs w;
+  w.fwd = carve_fwd(base, M, N, K);
+  w.lse = base ? (float*)((char*)base + w.fwd.total) : nullptr;
+  w.total = w.fwd.total + align256(M * 4);
+  return w;
+}
+
 }  // namespace
 }  // namespace renet
 
@@ -478,6 +499,43 @@ int renet_decoder_group_topk(const float* X, const float* W, const float* bias, 
   topk_final_kernel<<<(unsigned)G, kTopkFinalThreads, (size_t)sort_n * 8, stream>>>(w.cand_val, w.cand_idx, w.count, capacity, k,
                                                                                      order, sort_n, values, indices, needed);
   RENET_CHECK_LAUNCH("topk_final_kernel");
+  return RENET_OK;
+}
+
+int64_t renet_decoder_rank_workspace_bytes(int64_t M, int32_t N, int32_t K) { return carve_rank(nullptr, M, N, K).total + 256; }
+
+int renet_decoder_rank(const float* X, const float* W, const float* bias, const int32_t* label, const int32_t* excl_col,
+                       const int32_t* excl_begin, const int32_t* excl_end, float* loss_rows, int32_t* counts, int64_t M, int32_t N,
+                       int32_t K, void* workspace, int64_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  RENET_CHECK_ARG(M >= 0 && N > 0 && K > 0 && K % 4 == 0, "renet_decoder_rank: bad shape (K must be a multiple of 4)");
+  if (M == 0) return RENET_OK;
+  RENET_CHECK_ARG(X && W && label && loss_rows && counts && workspace, "renet_decoder_rank: null pointer");
+  RENET_CHECK_ARG(excl_col == nullptr || (excl_begin != nullptr && excl_end != nullptr),
+                  "renet_decoder_rank: exclusion lists need excl_begin and excl_end");
+  RENET_CHECK_ARG(workspace_bytes >= renet_decoder_rank_workspace_bytes(M, N, K), "renet_decoder_rank: workspace too small");
+  RENET_CHECK_ARG(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
+                  "renet_decoder_rank: X and W must be 16-byte aligned");
+  void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
+  RankWs w = carve_rank(base, M, N, K);
+  RENET_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)M * 16, stream));
+  // 1. lse, loss and the label's logit: the cross-entropy forward epilogue
+  int rc = umma_pack_b(W, 1, K, N, K, w.fwd.Wp, 0, stream);          // logical B[k][n] = W[n*K + k]
+  if (rc) return rc;
+  EpiArgs epi{};
+  epi.target = label; epi.pmax = w.fwd.pmax; epi.psum = w.fwd.psum; epi.tlogit = w.fwd.tlogit;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 1, epi, 1, 0, stream);
+  if (rc < 0) return rc;
+  const int n_part = 2 * ((N + 199) / 200);
+  ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.fwd.pmax, w.fwd.psum, w.fwd.tlogit, n_part, M, w.lse,
+                                                                      loss_rows);
+  RENET_CHECK_LAUNCH("ce_reduce_kernel");
+  // 2. the counts against the label's logit
+  EpiArgs cnt{};
+  cnt.target = label; cnt.tlogit = w.fwd.tlogit; cnt.excl_col = excl_col; cnt.excl_begin = excl_begin; cnt.excl_end = excl_end;
+  cnt.rank_counts = counts;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 6, cnt, 1, 0, stream);
+  if (rc < 0) return rc;
   return RENET_OK;
 }
 

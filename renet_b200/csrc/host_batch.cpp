@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/renet_b200.h"
@@ -61,7 +62,8 @@ struct Plan {
 int build_plan(Plan& P, const char* fn, int64_t T, const int64_t* g_node_off, const int32_t* g_node_ent, const int64_t* h_samp_off,
                const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow, const int64_t* h_ent_off,
                const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort, int64_t* s_idx_out,
-               int32_t max_len_capacity, int32_t* newid_out = nullptr, int64_t newid_capacity = 0) {
+               int32_t max_len_capacity, int32_t* newid_out = nullptr, int64_t newid_capacity = 0,
+               const int64_t* sample_group = nullptr) {
   // ---- 1. order samples by history length, descending, stable (model.py:80-81, utils.py:212-215) ----
   P.len.resize(B);
   int max_len = 0;
@@ -87,10 +89,12 @@ int build_plan(Plan& P, const char* fn, int64_t T, const int64_t* g_node_off, co
   }
   P.Q = Q; P.S = S;
   if (S == 0) return RENET_OK;
-  // ---- 2. components = distinct timestamps in first-appearance order (utils.py:149-170) ----------------
+  // ---- 2. components = distinct timestamps in first-appearance order (utils.py:149-170); with isolation groups, the
+  // distinct (group, timestamp) pairs in first-appearance order ------------------------------------------------------
   std::vector<int32_t> comp_of_graph(T, -1);
   P.row_comp.resize(S); P.row_srow.resize(S); P.row_seq.resize(S);
   std::vector<int64_t> row_entry(S);
+  std::vector<int64_t> row_group(sample_group ? S : 0);
   int64_t r = 0;
   for (int64_t q = 0; q < Q; ++q) {           // pass A: the samples' entry lists (contiguous per sample)
     const int64_t smp = sample_idx[s_idx_out[q]];
@@ -98,8 +102,10 @@ int build_plan(Plan& P, const char* fn, int64_t T, const int64_t* g_node_off, co
     for (int64_t ei = h_samp_off[smp]; ei < h_samp_off[smp + 1]; ++ei, ++r) {
       row_entry[r] = h_samp_entry[ei];
       P.row_seq[r] = (int32_t)q;
+      if (sample_group) row_group[r] = sample_group[s_idx_out[q]];
     }
   }
+  std::unordered_map<int64_t, std::unordered_map<int32_t, int32_t>> comp_of_pair;   // group -> graph -> component
   constexpr int64_t kAheadB = 16;
   for (int64_t i = 0; i < S; ++i) {           // pass B: per-entry fields (random reads: prefetched ahead)
     if (i + kAheadB < S) {
@@ -108,8 +114,14 @@ int build_plan(Plan& P, const char* fn, int64_t T, const int64_t* g_node_off, co
     }
     const int64_t e = row_entry[i];
     const int32_t g = h_ent_graph[e];
-    if (comp_of_graph[g] < 0) { comp_of_graph[g] = (int32_t)P.comp_graph.size(); P.comp_graph.push_back(g); }
-    P.row_comp[i] = comp_of_graph[g];
+    if (sample_group) {
+      auto ins = comp_of_pair[row_group[i]].emplace(g, (int32_t)P.comp_graph.size());
+      if (ins.second) P.comp_graph.push_back(g);
+      P.row_comp[i] = ins.first->second;
+    } else {
+      if (comp_of_graph[g] < 0) { comp_of_graph[g] = (int32_t)P.comp_graph.size(); P.comp_graph.push_back(g); }
+      P.row_comp[i] = comp_of_graph[g];
+    }
     P.row_srow[i] = h_ent_srow[e];
   }
   const int64_t G = P.G = (int64_t)P.comp_graph.size();
@@ -317,16 +329,19 @@ extern "C" int renet_host_assemble_batch(
 //   mark_off[G+1] cand_off[G+1]
 // newid: per component c, one word per local row of its timestamp's graph (offset mark_off[c]): batched node id or -1;
 // cand_off: prefix sum of the components' (un-induced) edge counts, i.e. the candidate edges the device filters.
-extern "C" int renet_host_plan_batch(
+// sample_group (optional, one entry per selected sample): isolation groups -- the components are the distinct (group,
+// timestamp) pairs, so the node sets of different groups never mix.  comp_graph, mark_off, cand_off and renet_induce_edges
+// already work per component and let any component point at any graph, so the device half is the same.
+extern "C" int renet_host_plan_batch_grouped(
     int64_t T, const int64_t* g_node_off, const int32_t* g_node_ent, const int64_t* g_edge_off,
     const int64_t* h_samp_off, const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow,
-    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort,
-    int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
+    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, const int64_t* sample_group, int64_t B,
+    int32_t sort, int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
     int64_t* sizes /* [10]: N, E_cand, S, Q, G, max_len, words_used, M, 0, 0 */) {
   if (B < 0 || !sizes) { renet::set_error("renet_host_plan_batch: bad arguments"); return RENET_ERR_INVALID_ARG; }
   Plan P;
   int prc = build_plan(P, "renet_host_plan_batch", T, g_node_off, g_node_ent, h_samp_off, h_samp_entry, h_ent_graph, h_ent_srow, h_ent_off,
-                       h_nbr_row, sample_idx, B, sort, s_idx_out, max_len_capacity, out, out_capacity);
+                       h_nbr_row, sample_idx, B, sort, s_idx_out, max_len_capacity, out, out_capacity, sample_group);
   if (prc != RENET_OK) return prc;
   const int64_t Q = P.Q, S = P.S, G = P.G, N = P.N;
   for (int i = 0; i < 10; ++i) sizes[i] = 0;
@@ -365,6 +380,17 @@ extern "C" int renet_host_plan_batch(
   o_moff[G] = (int32_t)M;
   o_coff[G] = (int32_t)acc;
   return RENET_OK;
+}
+
+extern "C" int renet_host_plan_batch(
+    int64_t T, const int64_t* g_node_off, const int32_t* g_node_ent, const int64_t* g_edge_off,
+    const int64_t* h_samp_off, const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow,
+    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort,
+    int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
+    int64_t* sizes) {
+  return renet_host_plan_batch_grouped(T, g_node_off, g_node_ent, g_edge_off, h_samp_off, h_samp_entry, h_ent_graph, h_ent_srow,
+                                       h_ent_off, h_nbr_row, sample_idx, nullptr, B, sort, s_idx_out, out, out_capacity,
+                                       batch_sizes_out, max_len_capacity, sizes);
 }
 
 // ---- native loader: a pool of C++ worker threads that run batch jobs ahead of the consumer ------------------------------

@@ -343,6 +343,9 @@ __device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], flo
 //   EPI 5  grouped top-k candidates (renet_decoder_group_topk): p = row_w[row] * exp(logit - lse[row]); every p at or above
 //          its group's threshold is appended to the group's candidate buffer (an integer atomic picks the slot; the final
 //          select sorts, so no output depends on the slot order)
+//   EPI 6  rank counts (renet_decoder_rank): every logit is compared with the label's logit that the EPI 1 pass wrote to
+//          tlogit (the same tile, the same instructions: the label's own logit compares equal), raw and after the sigmoid
+//          with the row's exclusion list zeroed; each (row, half tile) adds its four counts with integer atomics
 // grid.x = min(units, SMs).  Batched GEMMs (the two GRU encoders) have per-batch operand offsets.  Split-K (long-K,
 // few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
 // partial product to C + s*split_c; the caller sums the partials.
@@ -508,7 +511,7 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     acc_store(acc, sC, P_CLD, wt);
     named_bar_sync(1 + g, 128);
     if (wt >= 64) continue;
-    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI == 3 || EPI == 4, SEL = EPI == 5;
+    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI == 3 || EPI == 4, SEL = EPI == 5, RANK = EPI == 6;
     const int64_t gr = w.row_base + 64 * g + wt;
     const float* srow = sC + wt * P_CLD;
     float run_m = -3.0e38f, run_s = 0.f;               // EPI 1, 3: running max / sum of exp of this (row, half tile)
@@ -519,7 +522,23 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     const int sel_base = SEL ? (int)(gr - sel_g * epi.sel_R) * N : 0;     // flat index of the row's column 0 in its group
     const float row_w = (SEL && gr < M) ? __ldg(epi.row_w + gr) : 0.f;
     const float sel_tau = (SEL && gr < M) ? __ldg(epi.tau + sel_g) : 0.f;
-    const float row_lse = (!FWD && gr < M) ? __ldg(epi.lse + gr) : 0.f;
+    const float row_lse = (!FWD && !RANK && gr < M) ? __ldg(epi.lse + gr) : 0.f;
+    // EPI 6: the label's logit and sigmoid, the four counts, and the cursor into the row's exclusion list at the first
+    // entry >= the unit's first column
+    const float lab_z = (RANK && gr < M) ? __ldg(epi.tlogit + gr) : 0.f;
+    const float lab_p = RANK ? torch_sigmoid(lab_z) : 0.f;
+    const bool filt = RANK && epi.excl_col != nullptr;
+    int n_gt = 0, n_eq = 0, n_fgt = 0, n_feq = 0;
+    int xb = 0, xe = 0;
+    if (filt && gr < M) {
+      xb = __ldg(epi.excl_begin + gr);
+      xe = __ldg(epi.excl_end + gr);
+      const int first = n0 + cb;
+      for (int hi = xe; xb < hi;) {
+        const int mid = (xb + hi) >> 1;
+        if (__ldg(epi.excl_col + mid) < first) xb = mid + 1; else hi = mid;
+      }
+    }
     const float row_mass = (EPI == 4 && gr < M) ? __ldg(epi.rowmass + gr) : 0.f;
     const float gscale = (!FWD) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
     const float* prow = SOFT ? epi.soft + gr * epi.ldp + n0 : nullptr;   // read only for gr < M
@@ -568,6 +587,21 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
                 }
               }
             }
+        } else if (RANK) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            if (i < nv) {
+              n_gt += o[i] > lab_z;
+              n_eq += o[i] == lab_z;
+              if (filt) {
+                const int col = n0 + cc + i;
+                while (xb < xe && __ldg(epi.excl_col + xb) < col) ++xb;
+                const bool zeroed = xb < xe && __ldg(epi.excl_col + xb) == col && col != tgt;
+                const float p = zeroed ? 0.f : torch_sigmoid(o[i]);
+                n_fgt += p > lab_p;
+                n_feq += p == lab_p;
+              }
+            }
         } else {
           float* dp = Cz + gr * ldc + n0 + cc;
 #pragma unroll
@@ -580,6 +614,13 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
             }
         }
       }
+    }
+    if (RANK && gr < M) {
+      int32_t* rc = epi.rank_counts + 4 * gr;
+      if (n_gt) atomicAdd(rc, n_gt);
+      if (n_eq) atomicAdd(rc + 1, n_eq);
+      if (n_fgt) atomicAdd(rc + 2, n_fgt);
+      if (n_feq) atomicAdd(rc + 3, n_feq);
     }
     if (FWD && gr < M) {
       const int64_t pi = (int64_t)(w.nt * 2 + w.half) * M + gr;
@@ -911,6 +952,7 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(3)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(4)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(5)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(6)));
     attr2 = true;
   }
   const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
@@ -926,6 +968,7 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
   else if (epi_mode == 3) RENET_UMMA_LAUNCH(false, 3);
   else if (epi_mode == 4) RENET_UMMA_LAUNCH(false, 4);
   else if (epi_mode == 5) RENET_UMMA_LAUNCH(false, 5);
+  else if (epi_mode == 6) RENET_UMMA_LAUNCH(false, 6);
   else if (a_index) RENET_UMMA_LAUNCH(true, 0);
   else RENET_UMMA_LAUNCH(false, 0);
 #undef RENET_UMMA_LAUNCH
@@ -1058,7 +1101,7 @@ static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, 
 }
 
 // C[b] (+)= A[b] @ Bpacked[b] (+bias[b]) for b < batch; strides in elements (A, C) / bytes (Bp).
-// epi_mode 1-4: fused cross-entropy epilogues, 5: grouped top-k candidates (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
+// epi_mode 1-4: fused cross-entropy epilogues, 5: grouped top-k candidates, 6: rank counts (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,

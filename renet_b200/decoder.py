@@ -8,7 +8,10 @@ the forward pass.  ``nn.Linear`` modules stay the parameter holders (state_dict 
 (utils.py:287-290, fp64 log-softmax, mean over rows), returned as a float64 scalar like the reference's.
 
 ``decoder_group_topk(x, weight, bias, row_weight, R, k)`` is the test-time roll-over's candidate scoring on the same engine
-(renet_decoder_group_topk): per group of R rows, the k largest row_weight * softmax(F.linear(x, weight, bias)) entries."""
+(renet_decoder_group_topk): per group of R rows, the k largest row_weight * softmax(F.linear(x, weight, bias)) entries.
+
+``decoder_rank(x, weight, bias, label, exclude)`` is the test-time scoring on the same engine (renet_decoder_rank): per row
+the cross-entropy loss and the label's raw and filtered ranks by the reference's tie rule (model.py:373-379, 403-418)."""
 import torch
 
 from . import _lib
@@ -137,3 +140,47 @@ def decoder_group_topk(x, weight, bias, row_weight, R, k, order=ORDER_INDEX, cap
         if need == 0:
             return values, indices.long()
         cap = need
+
+
+def decoder_rank_counts(x, weight, bias, label, exclude=None):
+    """renet_decoder_rank: for z = x @ weight^T + bias and the labels ``label`` [M], returns (loss_rows float32 [M],
+    counts int32 [M, 4]) with counts[m] = (#z > z_l, #z == z_l, #p > p_l, #p == p_l) where p = torch.sigmoid(z) with the
+    columns of row m's exclusion list other than its label set to 0.  ``exclude`` = (col, begin, end): int32 device
+    tensors, row m's list being col[begin[m]:end[m]] in ascending order; None leaves the last two counts 0."""
+    L, P = _lib.lib(), _lib.ptr
+    _lib.require_cuda(x, weight, label)
+    x, weight = x.contiguous(), weight.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    lab = label.to(torch.int32).contiguous()
+    M, K = x.shape
+    N = weight.shape[0]
+    if lab.numel() != M:
+        raise ValueError('decoder_rank: %d rows but %d labels' % (M, lab.numel()))
+    col = begin = end = None
+    if exclude is not None:
+        col, begin, end = (t.to(torch.int32).contiguous() for t in exclude)
+        _lib.require_cuda(col, begin, end)
+        if begin.numel() != M or end.numel() != M:
+            raise ValueError('decoder_rank: exclusion ranges need one (begin, end) per row')
+    dev = x.device
+    loss_rows = torch.empty(M, device=dev)
+    counts = torch.empty(M, 4, dtype=torch.int32, device=dev)
+    nbytes = int(L.renet_decoder_rank_workspace_bytes(M, N, K))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    _lib.check(L.renet_decoder_rank(P(x), P(weight), P(bias), P(lab), P(col), P(begin), P(end), P(loss_rows), P(counts), M, N, K,
+                                    P(ws), nbytes, _lib.stream()), 'renet_decoder_rank')
+    return loss_rows, counts
+
+
+def ranks_from_counts(greater, equal):
+    """The reference's tie rule (model.py:373-379): #greater + (#equal - 1) / 2 + 1, in float64."""
+    return greater.double() + (equal.double() - 1.0) / 2 + 1
+
+
+def decoder_rank(x, weight, bias, label, exclude=None):
+    """(loss_rows float32 [M], raw ranks float64 [M], filtered ranks float64 [M] or None when ``exclude`` is None) of the
+    labels among the rows of x @ weight^T + bias; see decoder_rank_counts."""
+    loss_rows, c = decoder_rank_counts(x, weight, bias, label, exclude)
+    raw = ranks_from_counts(c[:, 0], c[:, 1])
+    filt = ranks_from_counts(c[:, 2], c[:, 3]) if exclude is not None else None
+    return loss_rows, raw, filt

@@ -180,15 +180,25 @@ class HistoryStore:
             self.nbr_row = np.zeros(0, np.int32)
         self._keepalive = hist        # array identities are the entry keys: keep the arrays alive
 
-    def select(self, sample_idx):
-        return HistoryView(self, np.ascontiguousarray(sample_idx, dtype=np.int64))
+    def select(self, sample_idx, groups=None):
+        return HistoryView(self, np.ascontiguousarray(sample_idx, dtype=np.int64), groups)
 
 
 class HistoryView:
-    """A batch = indices into a HistoryStore.  Passed where the reference passes (s_hist, s_hist_t)."""
+    """A batch = indices into a HistoryStore.  Passed where the reference passes (s_hist, s_hist_t).
 
-    def __init__(self, store, sample_idx):
+    ``groups`` (optional, one int per selected sample): isolation groups.  The batched history graph then has one component
+    per distinct (group, timestamp) instead of one per timestamp, so the samples of a group are encoded exactly as if they
+    were batched alone (renet_host_plan_batch_grouped); the reference's predict encodes every (entity, relation) history
+    alone.  Only the device batcher takes groups."""
+
+    def __init__(self, store, sample_idx, groups=None):
         self.store, self.sample_idx = store, sample_idx
+        self.groups = None
+        if groups is not None:
+            self.groups = np.ascontiguousarray(groups, dtype=np.int64).reshape(-1)
+            if len(self.groups) != len(sample_idx):
+                raise ValueError('HistoryView: %d samples but %d groups' % (len(sample_idx), len(self.groups)))
 
     def __len__(self):
         return len(self.sample_idx)
@@ -239,6 +249,8 @@ def reserve_pinned(n, words=1 << 21):
 def assemble_view_raw(view, out, sort=True):
     """Run the C++ batcher into the int32 numpy buffer ``out`` (host only, no CUDA).  Returns None when
     the buffer is too small (sizes[6] words are needed), else a dict of sizes + small host arrays."""
+    if view.groups is not None:
+        raise ValueError('isolation groups need the device batcher (device_edges=True)')
     L = _lib.lib()
     hs, gs = view.store, view.store.gs
     B = len(view.sample_idx)
@@ -274,17 +286,19 @@ def split_raw(buf, r):
 
 
 def plan_view_raw(view, out, sort=True):
-    """Host half of the device batcher (renet_host_plan_batch) into the int32 numpy buffer ``out``."""
+    """Host half of the device batcher (renet_host_plan_batch_grouped, with the view's isolation groups if it has any)
+    into the int32 numpy buffer ``out``."""
     L = _lib.lib()
     hs, gs = view.store, view.store.gs
     B = len(view.sample_idx)
     s_idx = np.empty(B, dtype=np.int64)
     bsz = np.zeros(MAX_LEN, dtype=np.int32)
     sizes = np.zeros(10, dtype=np.int64)
-    rc = L.renet_host_plan_batch(
+    groups = _p(view.groups) if view.groups is not None else None
+    rc = L.renet_host_plan_batch_grouped(
         len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(hs.samp_off), _p(hs.samp_entry), _p(hs.ent_graph),
-        _p(hs.ent_srow), _p(hs.ent_off), _p(hs.nbr_row), _p(view.sample_idx), B, int(sort), _p(s_idx), _p(out), out.size,
-        _p(bsz), MAX_LEN, _p(sizes))
+        _p(hs.ent_srow), _p(hs.ent_off), _p(hs.nbr_row), _p(view.sample_idx), groups, B, int(sort), _p(s_idx), _p(out),
+        out.size, _p(bsz), MAX_LEN, _p(sizes))
     if rc == 1:
         return {'need_words': int(sizes[6])}
     _lib.check(rc, 'renet_host_plan_batch')
@@ -328,6 +342,8 @@ class NativeLoader:
     def submit(self, view, out, sort, device_edges):
         """Enqueue the host work of one batch into the int32 numpy buffer ``out``; returns the job record that finish()
         takes (it keeps every array the C++ job writes alive)."""
+        if view.groups is not None:
+            raise ValueError('NativeLoader: isolation groups are not supported; use assemble_view')
         hs, gs = view.store, view.store.gs
         B = len(view.sample_idx)
         job = dict(view=view, out=out, sort=sort, device_edges=device_edges, B=B, s_idx=np.empty(B, dtype=np.int64),
@@ -528,9 +544,11 @@ DEVICE_EDGES = True      # build the batched CSR on the GPU (renet_induce_edges)
 
 def assemble_view(view, device, sort=True, device_edges=None):
     """HistoryView -> HistoryBatch on ``device``: host plan + one pinned H2D copy + renet_induce_edges on the GPU
-    (default), or the all-host C++ batcher + one pinned H2D copy (device_edges=False)."""
+    (default), or the all-host C++ batcher + one pinned H2D copy (device_edges=False; not for views with groups)."""
     if device_edges is None:
         device_edges = DEVICE_EDGES
+    if view.groups is not None and not device_edges:
+        raise ValueError('isolation groups need the device batcher (device_edges=True)')
     st = _staging.get(str(device))
     if st is None:
         st = _staging[str(device)] = _Staging()

@@ -23,6 +23,11 @@ from .graph import get_big_graph
 ROLLOVER_SEQ_BUDGET = 16384
 
 
+#: distinct (entity, timestamp) components evaluate_stream_batched batches per chunk are bounded by their summed node and
+#: candidate-edge counts: the plan's mark_off / cand_off are int32, and 2^28 keeps them far from overflow
+EVAL_PLAN_BUDGET = 1 << 28
+
+
 def rank_with_ties(scores, label):
     """model.py:373-379: rank = #(strictly greater) + (#equal - 1)/2 + 1."""
     ref = scores[label]
@@ -46,6 +51,65 @@ def history_triples(s_cache, o_cache):
     if not rows:
         return None
     return np.unique(torch.cat(rows).numpy(), axis=0)
+
+
+def stream_metrics(ranks, total_loss):
+    """test.py:140-150: MRR / MR / Hits@{1,3,10} over all ranks, the summed loss and the ranks themselves."""
+    ranks = np.concatenate(ranks) if ranks else np.zeros(0)
+    out = {'mrr': float(np.mean(1.0 / ranks)) if len(ranks) else float('nan'),
+           'mr': float(np.mean(ranks)) if len(ranks) else float('nan'), 'loss': total_loss, 'ranks': ranks}
+    for k in (1, 3, 10):
+        out['hits@%d' % k] = float(np.mean(ranks <= k)) if len(ranks) else float('nan')
+    return out
+
+
+class FilterIndex:
+    """The known answers of every (subject, relation) and (object, relation) pair of a set of triples, built once: what
+    evaluate_filter (model.py:384-419) finds by scanning all triples for every test triple.  For direction ``objects``
+    (the answers o of (s, r, ?)) and ``subjects`` (the answers s of (?, r, o)): one int32 column array of the sorted
+    distinct answers, grouped by pair, and the pairs' keys sorted ascending."""
+
+    def __init__(self, triples):
+        t = np.asarray(torch.as_tensor(triples).cpu().numpy()[:, :3], dtype=np.int64)
+        self.R = int(t[:, 1].max()) + 1 if len(t) else 1
+        self.dirs = {}
+        for name, fix, ans in (('objects', 0, 2), ('subjects', 2, 0)):
+            u = np.unique(np.stack((t[:, fix] * self.R + t[:, 1], t[:, ans]), 1), axis=0) if len(t) else np.zeros((0, 2), np.int64)
+            self.dirs[name] = (u[:, 0].copy(), np.ascontiguousarray(u[:, 1], dtype=np.int32))
+
+    def ranges(self, direction, fixed, r):
+        """(begin, end) int64 arrays: the answers of pair i are col(direction)[begin[i]:end[i]]."""
+        keys, _ = self.dirs[direction]
+        k = np.asarray(fixed, dtype=np.int64) * self.R + np.asarray(r, dtype=np.int64)
+        k = np.where((np.asarray(r) >= 0) & (np.asarray(r) < self.R), k, -1)
+        return np.searchsorted(keys, k, 'left'), np.searchsorted(keys, k, 'right')
+
+    def col(self, direction):
+        return self.dirs[direction][1]
+
+
+def rank_counts_torch(z, label, exclude=None):
+    """What renet_decoder_rank counts, on materialised logits z [M, N] with torch: int64 [M, 4] = (#z > z_l, #z == z_l,
+    #p > p_l, #p == p_l), p = torch.sigmoid(z) with row m's excluded columns other than its label set to 0 (the last two
+    are 0 without ``exclude`` = (col, begin, end))."""
+    M = z.shape[0]
+    idx = torch.arange(M, device=z.device)
+    zl = z[idx, label].view(-1, 1)
+    out = torch.zeros(M, 4, dtype=torch.long, device=z.device)
+    out[:, 0] = (z > zl).sum(1)
+    out[:, 1] = (z == zl).sum(1)
+    if exclude is not None:
+        col, begin, end = (torch.as_tensor(x).long().cpu() for x in exclude)
+        p = torch.sigmoid(z)
+        for m in range(M):
+            cols = col[begin[m]:end[m]].to(z.device)
+            ground = p[m, label[m]].clone()
+            p[m, cols] = 0
+            p[m, label[m]] = ground
+        pl = p[idx, label].view(-1, 1)
+        out[:, 2] = (p > pl).sum(1)
+        out[:, 3] = (p == pl).sum(1)
+    return out
 
 
 class RENetInference:
@@ -140,14 +204,27 @@ class RENetInference:
         p_r = torch.softmax(ob_pred_r.view(-1), dim=0)
         return p_o * p_r.view(R, 1)
 
+    def _grouped_view(self, entities, samples, subject):
+        """A HistoryView over the current test-time histories of ``entities`` (all non-empty): one store entry per entity,
+        the view's samples = ``samples`` (positions in ``entities``), each sample isolated in the group of its entity, over
+        a GraphStore of the timestamps those histories reference.  Returns (view, graph store)."""
+        from .hoststore import GraphStore, HistoryStore
+        hist = self.s_hist_test if subject else self.o_hist_test
+        hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
+        times = sorted({int(t) for e in entities for t in hist_t[e]})
+        gs = GraphStore({t: self.graph_dict[t] for t in times})
+        store = HistoryStore([hist[e] for e in entities], [hist_t[e] for e in entities], entities, gs, dedupe=False)
+        samples = np.asarray(samples, dtype=np.int64)
+        return store.select(samples, groups=samples), gs
+
     def pred_r_topk(self, entities, weights, k, subject=True, capacity=None):
         """pred_r_rank2 followed by torch.topk for many entities at once (model.py:168-213, 236-240).  For entity
         entities[i]: the k largest entries of weights[i] * pred_r_rank2([entities[i]] * R, arange(R), subject).view(-1)
         and their codes r * in_dim + o, as (values float32 [n, k], codes int64 [n, k]) on the model's device.
 
         The test-time histories of a chunk of entities are encoded in one batched call (one store entry per entity, each
-        repeated once per relation, through the C++ / device batcher, over a graph store built for the chunk in which
-        every entity has its own copies of its history's graphs); entities without history get zero s_h / s_q as in
+        repeated once per relation, through the C++ / device batcher with one isolation group per entity, so that every
+        entity gets components of its own); entities without history get zero s_h / s_q as in
         pred_r_rank2.  The joint distribution is never materialised: renet_decoder_group_topk scores
         [ent_e | s_h(e, r) | rel_r] against ``linear`` with the row weights weights[i] * softmax_r(linear_r([ent_e | s_q_e]))
         and selects each entity's k best in one pass.  A group's k entries come in the order torch.topk(sorted=False) gives
@@ -155,7 +232,6 @@ class RENetInference:
         to it; measured on an H100 with PyTorch 2.11 from R * in_dim = 9 600 to 5.9 M), since the roll-over's final
         selection and the order of its cache updates depend on that layout."""
         from .decoder import ORDER_INDEX, decoder_group_topk
-        from .hoststore import GraphStore, HistoryStore
         R, h, N = self.num_rels, self.h_dim, self.in_dim
         dev = self.ent_embeds.device
         ents = torch.as_tensor(entities).reshape(-1).long().cpu().numpy()
@@ -167,7 +243,6 @@ class RENetInference:
         codes = torch.empty(n, k, dtype=torch.long, device=dev)
         rel_embeds, reverse = self._direction(subject)
         hist = self.s_hist_test if subject else self.o_hist_test
-        hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
         per = max(1, ROLLOVER_SEQ_BUDGET // R)
         rel_rows = torch.arange(R, device=dev)
         for c0 in range(0, n, per):
@@ -179,22 +254,14 @@ class RENetInference:
             if len(has):
                 he = ce[has]
                 # The batched history graph has one component per timestamp, induced by the nodes of every sample in
-                # the batch (utils.py:158-181), so an entity's encoding depends on what it is batched with.  Each entity
-                # gets its own copies of its history's graphs, under keys of its own, to encode exactly what
-                # pred_r_rank2 encodes alone.
-                span = max(len(hist_t[e]) for e in he)
-                keys = [[j * span + i for i in range(len(hist_t[e]))] for j, e in enumerate(he)]
-                graphs, glob = {}, {}
-                for e, ks in zip(he, keys):
-                    for v, t in zip(ks, hist_t[e]):
-                        graphs[v], glob[v] = self.graph_dict[int(t)], self.global_emb[int(t)]
-                gs = GraphStore(graphs)
-                store = HistoryStore([hist[e] for e in he], keys, he, gs, dedupe=False)
-                view = store.select(np.repeat(np.arange(len(he)), R))
+                # the batch (utils.py:158-181), so an entity's encoding depends on what it is batched with.  One isolation
+                # group per entity gives every entity components of its own, to encode exactly what pred_r_rank2 encodes
+                # alone.
+                view, gs = self._grouped_view(he, np.repeat(np.arange(len(he)), R), subject)
                 s_dev = torch.from_numpy(np.repeat(he, R)).to(dev)
                 r_dev = rel_rows.repeat(len(he))
-                sh, sq, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, glob, reverse,
-                                                    self.encoder, self.encoder_r)
+                sh, sq, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, self.global_emb,
+                                                    reverse, self.encoder, self.encoder_r)
                 # the encoder returns the sequences length-sorted: row j is sample sample_order[j] of the view
                 idx = hb.sample_order(dev)
                 sh_v, sq_v = torch.empty_like(sh), torch.empty_like(sq)
@@ -336,11 +403,7 @@ class RENetInference:
         (test.py:100-106), ranks every test triple in stream order (``evaluate`` when ``raw`` else ``evaluate_filter``
         against ``total_data``), and returns MRR / MR / Hits@{1,3,10} over subject and object ranks together, the summed
         loss and the ranks.  ``s_history`` / ``o_history`` = (lists, timestamp lists) of the test split."""
-        for hist, hist_t in ((self.s_hist_test, self.s_hist_test_t), (self.o_hist_test, self.o_hist_test_t)):
-            for ee in range(self.in_dim):
-                while len(hist[ee]) > self.seq_len:
-                    hist[ee].pop(0)
-                    hist_t[ee].pop(0)
+        self._trim_test_histories()
         test_data = torch.as_tensor(test_data)
         if not raw:
             if total_data is None:
@@ -357,10 +420,166 @@ class RENetInference:
                     r, loss = self.evaluate_filter(trip, sh, oh, global_model, total_data)
                 ranks.append(r)
                 total_loss += float(loss)
-        ranks = np.concatenate(ranks) if ranks else np.zeros(0)
-        out = {'mrr': float(np.mean(1.0 / ranks)) if len(ranks) else float('nan'),
-               'mr': float(np.mean(ranks)) if len(ranks) else float('nan'), 'loss': total_loss, 'ranks': ranks}
-        for k in (1, 3, 10):
-            out['hits@%d' % k] = float(np.mean(ranks <= k)) if len(ranks) else float('nan')
+        return stream_metrics(ranks, total_loss)
+
+    def _trim_test_histories(self):
+        """test.py:100-106: keep the last seq_len entries of every per-entity test-time history."""
+        for hist, hist_t in ((self.s_hist_test, self.s_hist_test_t), (self.o_hist_test, self.o_hist_test_t)):
+            for ee in range(self.in_dim):
+                while len(hist[ee]) > self.seq_len:
+                    hist[ee].pop(0)
+                    hist_t[ee].pop(0)
+
+    # ---- batched evaluation -------------------------------------------------------------------------------------------
+    def evaluate_stream_batched(self, test_data, s_history, o_history, global_model, total_data=None, raw=False):
+        """evaluate_stream, one timestamp at a time: same arguments, same result dict, same state afterwards (histories,
+        caches, graph_dict, global_emb, latest_time, torch's RNG stream).  All triples of a timestamp are scored against the
+        same state -- predict changes it only at the first triple of a new timestamp, through the roll-over -- so for each
+        maximal run of equal timestamps the roll-over runs once, as predict runs it, and then every query of the run is
+        encoded in one batched pass (one isolation group per entity, so each history is encoded as if alone) and every
+        triple is scored and ranked by one renet_decoder_rank call.  The known answers come from a FilterIndex built once
+        from ``total_data``.  A model on the host has no kernels: it encodes each query through _encode_one and ranks the
+        materialised logits with torch, with the same grouping, rebinding and filter index."""
+        self._trim_test_histories()
+        test_data = torch.as_tensor(test_data)
+        fidx = None
+        if not raw:
+            if total_data is None:
+                raise ValueError('filtered evaluation needs total_data (all known triples)')
+            fidx = FilterIndex(total_data)
+        quads = test_data.cpu().numpy().astype(np.int64)
+        s_empty = np.asarray([len(x) == 0 for x in s_history[0]], dtype=bool)
+        o_empty = np.asarray([len(x) == 0 for x in o_history[0]], dtype=bool)
+        ranks, total_loss = [], 0.0
+        with torch.no_grad():
+            i0, n = 0, len(quads)
+            while i0 < n:
+                i1 = i0 + 1
+                while i1 < n and quads[i1, 3] == quads[i0, 3]:
+                    i1 += 1
+                t = test_data[i0][3].cpu()
+                rebind = None
+                if self.latest_time != t:                                   # predict's roll-over (model.py:222-330)
+                    last_s, last_o = self._roll_over(t, global_model)
+                    if self.reference_rebinding:
+                        rebind = (last_s, last_o)
+                r, loss = self._score_run(quads[i0:i1], s_empty[i0:i1], o_empty[i0:i1], rebind, fidx)
+                ranks.append(r)
+                total_loss += float(np.sum(loss.astype(np.float64)))
+                i0 = i1
+        return stream_metrics(ranks, total_loss)
+
+    def _score_run(self, quads, s_empty, o_empty, rebind, fidx):
+        """Scores the triples of one timestamp against the current state: (ranks float64 [2n] as [sub, ob] per triple,
+        loss float32 [n] = predict's two cross-entropies per triple).  rebind = (s, o) of the roll-over that the run's first
+        triple is scored with (model.py:279,290) or None; its rank labels and filter keys stay its own."""
+        R, h = self.num_rels, self.h_dim
+        dev = self.ent_embeds.device
+        n = len(quads)
+        s, r, o = quads[:, 0].copy(), quads[:, 1].copy(), quads[:, 2].copy()
+        si, oi = s.copy(), o.copy()
+        if rebind is not None:
+            si[0], oi[0] = rebind
+        has_s = ~s_empty & np.asarray([len(self.s_hist_test[e]) != 0 for e in si], dtype=bool)
+        has_o = ~o_empty & np.asarray([len(self.o_hist_test[e]) != 0 for e in oi], dtype=bool)
+        s_h = self._encode_queries(si, r, has_s, True)
+        o_h = self._encode_queries(oi, r, has_o, False)
+        to_dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(dev)    # noqa: E731
+        si_d, oi_d, r_d = to_dev(si), to_dev(oi), to_dev(r)
+        x = torch.cat((torch.cat((self.ent_embeds[si_d], s_h, self.rel_embeds[:R][r_d]), dim=1),
+                       torch.cat((self.ent_embeds[oi_d], o_h, self.rel_embeds[R:][r_d]), dim=1)), dim=0)
+        rank_lab = np.concatenate((o, s))                        # ob rows rank the triple's object, sub rows its subject
+        loss_row = np.concatenate((np.arange(n), n + np.arange(n)))
+        if rebind is not None and (si[0] != s[0] or oi[0] != o[0]):
+            # predict's loss for the rebound triple takes the rebound labels: two extra rows carry them
+            x = torch.cat((x, x[[0, n]]), dim=0)
+            rank_lab = np.concatenate((rank_lab, [oi[0], si[0]]))
+            loss_row[0], loss_row[n] = 2 * n, 2 * n + 1
+        exclude = None
+        if fidx is not None:
+            m = len(rank_lab)
+            fix = np.concatenate((s, o, [s[0], o[0]]))[:m]
+            rr = np.concatenate((r, r, [r[0], r[0]]))[:m]
+            direction = np.concatenate((np.zeros(n, bool), np.ones(n, bool), [False, True]))[:m]
+            b_ob, e_ob = fidx.ranges('objects', fix, rr)
+            b_sb, e_sb = fidx.ranges('subjects', fix, rr)
+            off = len(fidx.col('objects'))
+            col = np.concatenate((fidx.col('objects'), fidx.col('subjects')))
+            begin = np.where(direction, b_sb + off, b_ob)
+            end = np.where(direction, e_sb + off, e_ob)
+            exclude = (col, begin, end)
+        loss_rows, raw_rank, filt_rank = self._rank_rows(x, rank_lab, exclude)
+        rk = (filt_rank if exclude is not None else raw_rank).cpu().numpy()
+        ranks = np.stack((rk[n:2 * n], rk[:n]), axis=1).reshape(-1)
+        lr = loss_rows.cpu().numpy().astype(np.float32)
+        return ranks, lr[loss_row[:n]] + lr[loss_row[n:]]
+
+    def _rank_rows(self, x, label, exclude):
+        """(loss_rows, raw ranks, filtered ranks or None) of the rows of x against ``linear``: renet_decoder_rank on the
+        GPU; on the host, row by row through ``linear`` as predict computes them, counted with torch."""
+        from .decoder import decoder_rank, ranks_from_counts
+        dev = x.device
+        lab = torch.from_numpy(np.ascontiguousarray(label, dtype=np.int64)).to(dev)
+        if x.is_cuda:
+            ex = None
+            if exclude is not None:
+                ex = tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev) for a in exclude)
+            return decoder_rank(x, self.linear.weight, self.linear.bias, lab, ex)
+        z = torch.stack([self.linear(row) for row in x])
+        loss_rows = torch.stack([self.criterion(z[m].view(1, -1), lab[m].view(1)) for m in range(len(lab))])
+        c = rank_counts_torch(z, lab, exclude)
+        filt = ranks_from_counts(c[:, 2], c[:, 3]) if exclude is not None else None
+        return loss_rows, ranks_from_counts(c[:, 0], c[:, 1]), filt
+
+    def _encode_queries(self, ents, rels, has, subject):
+        """s_h [n, h] of the queries (ents[i], rels[i]) against the current test-time histories; rows where ``has`` is
+        False stay zero (predict's empty-history rule).  Equal queries are encoded once.  On the GPU the distinct queries go
+        through the device batcher in chunks, one isolation group per entity, so that each equals _encode_one's encoding
+        of it alone; on the host, through _encode_one."""
+        h, R = self.h_dim, self.num_rels
+        dev = self.ent_embeds.device
+        out = torch.zeros(len(ents), h, device=dev)
+        sel = np.flatnonzero(has)
+        if len(sel) == 0:
+            return out
+        keys, inverse = np.unique(np.asarray(ents)[sel].astype(np.int64) * R + np.asarray(rels)[sel], return_inverse=True)
+        q_e, q_r = keys // R, keys % R
+        hist = self.s_hist_test if subject else self.o_hist_test
+        hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
+        enc = torch.empty(len(keys), h, device=dev)
+        if not self.ent_embeds.is_cuda:
+            for j, (e, rr) in enumerate(zip(q_e.tolist(), q_r.tolist())):
+                enc[j] = self._encode_one(e, rr, hist[e], hist_t[e], subject)
+        else:
+            rel_embeds, reverse = self._direction(subject)
+            sizes = {}
+            for t in {int(t) for e in np.unique(q_e) for t in hist_t[e]}:
+                g = self.graph_dict[t]
+                sizes[t] = g.number_of_nodes() + g.number_of_edges()
+            j0 = 0
+            while j0 < len(keys):
+                # a chunk: whole entities (keys are sorted by entity), within both budgets
+                cost, j1 = 0, j0
+                while j1 < len(keys) and j1 - j0 < ROLLOVER_SEQ_BUDGET:
+                    e = q_e[j1]
+                    if j1 == j0 or e != q_e[j1 - 1]:
+                        c = sum(sizes[int(t)] for t in hist_t[e])
+                        if j1 > j0 and cost + c > EVAL_PLAN_BUDGET:
+                            break
+                        cost += c
+                    j1 += 1
+                ue, pos = np.unique(q_e[j0:j1], return_inverse=True)
+                view, gs = self._grouped_view(ue, pos, subject)
+                s_dev = torch.from_numpy(q_e[j0:j1]).to(dev)
+                r_dev = torch.from_numpy(q_r[j0:j1]).to(dev)
+                sh, _, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, self.global_emb,
+                                                   reverse, self.encoder, self.encoder_r)
+                # the encoder returns the sequences length-sorted: row k is sample sample_order[k] of the view
+                idx = hb.sample_order(dev)
+                part = torch.empty_like(sh)
+                part[idx] = sh
+                enc[j0:j1] = part
+                j0 = j1
+        out[torch.from_numpy(sel).to(dev)] = enc[torch.from_numpy(inverse.reshape(-1)).to(dev)]
         return out
 
