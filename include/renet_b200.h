@@ -357,13 +357,9 @@ int renet_segment_pool_bwd(const float* dout, const int32_t* seg_ptr, const int3
  * Output: s_idx_out [B] (sample order: history length descending, stable, when sort != 0), the batched
  * graph in CSR form + bookkeeping packed into `out` (int32 words, one H2D copy):
  *   node_ent[N] row_ptr[N+1] col_src[E] col_type_s[E] col_type_o[E] norm[N](float bits)
- *   readout[S] row_comp[S] row_seq[S] seq_start[Q] seq_len[Q] packed_row[S]
- *   comp_ptr[G+1] comp_order[G] rel_slot_s[R2] hot_s[n_hot_max] rel_slot_o[R2] hot_o[n_hot_max]
- *   s_idx[B] comp_graph[G]
- * (the comp/rel line feeds renet_rgcn_gather_comp: components largest-first, and the n_hot_max most frequent
- * edge types of the batch for each type column).  comp_graph_out [G] (graph index of every component,
- * first-appearance order), batch_sizes_out [max_len],
- * sizes [10] = {N, E, S, Q, G, max_len, words_used, n_hot_s, n_hot_o, 0}.
+ *   readout[S] row_comp[S] row_seq[S] seq_start[Q] seq_len[Q] packed_row[S] s_idx[B] comp_graph[G]
+ * (comp_graph: graph index of every component, first-appearance order), batch_sizes_out [max_len],
+ * sizes [10] = {N, E, S, Q, G, max_len, words_used, 0, 0, 0}.
  * Returns 0, or 1 when out_capacity < words_used (sizes is filled: grow and call again), <0 on error.
  * ---------------------------------------------------------------------------------------------- */
 /* Threads renet_host_assemble_batch may use per call (default 8; use 1 when many calls run concurrently, e.g.
@@ -374,8 +370,7 @@ int renet_host_assemble_batch(
     const int32_t* g_src, const int32_t* g_dst, const int32_t* g_type_s, const int32_t* g_type_o,
     const int64_t* h_samp_off, const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow,
     const int64_t* h_ent_off, const int32_t* h_nbr_row,
-    const int64_t* sample_idx, int64_t B, int32_t sort, int32_t R2, int32_t n_hot_max,
-    int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* comp_graph_out,
+    const int64_t* sample_idx, int64_t B, int32_t sort, int64_t* s_idx_out, int32_t* out, int64_t out_capacity,
     int32_t* batch_sizes_out, int32_t max_len_capacity, int64_t* sizes);
 
 /* ------------------------------------------------------------------------------------------------
@@ -438,9 +433,9 @@ int64_t renet_loader_submit_assemble(
     void* loader, int64_t T, const int64_t* g_node_off, const int32_t* g_node_ent, const int64_t* g_edge_off,
     const int32_t* g_src, const int32_t* g_dst, const int32_t* g_type_s, const int32_t* g_type_o,
     const int64_t* h_samp_off, const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow,
-    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort, int32_t R2,
-    int32_t n_hot_max, int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* comp_graph_out,
-    int32_t* batch_sizes_out, int32_t max_len_capacity, int64_t* sizes);
+    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort,
+    int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
+    int64_t* sizes);
 int renet_loader_wait(void* loader, int64_t ticket);
 
 /* Sequence ids of a batch in processing order, on the device, in one launch (model.py:81-84, utils.py:224-225):

@@ -54,7 +54,7 @@ SIGNATURES = {
     'renet_segment_pool_fwd': (ctypes.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
     'renet_segment_pool_bwd': (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i32, _i32, _vp, _vp]),
     'renet_set_host_threads': (ctypes.c_int, [ctypes.c_int]),
-    'renet_host_assemble_batch': (ctypes.c_int, [_i64] + [_vp] * 13 + [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _vp, _vp, _i32, _vp]),
+    'renet_host_assemble_batch': (ctypes.c_int, [_i64] + [_vp] * 14 + [_i64, _i32, _vp, _vp, _i64, _vp, _i32, _vp]),
     'renet_host_plan_batch': (ctypes.c_int, [_i64] + [_vp] * 10 + [_i64, _i32, _vp, _vp, _i64, _vp, _i32, _vp]),
     'renet_host_plan_batch_grouped': (ctypes.c_int, [_i64] + [_vp] * 11 + [_i64, _i32, _vp, _vp, _i64, _vp, _i32, _vp]),
     'renet_induce_workspace_bytes': (_i64, [_i64]),
@@ -64,7 +64,7 @@ SIGNATURES = {
     'renet_loader_create': (_vp, [_i32]),
     'renet_loader_destroy': (None, [_vp]),
     'renet_loader_submit_plan': (_i64, [_vp, _i64] + [_vp] * 10 + [_i64, _i32, _vp, _vp, _i64, _vp, _i32, _vp]),
-    'renet_loader_submit_assemble': (_i64, [_vp, _i64] + [_vp] * 13 + [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _vp, _vp, _i32, _vp]),
+    'renet_loader_submit_assemble': (_i64, [_vp, _i64] + [_vp] * 14 + [_i64, _i32, _vp, _vp, _i64, _vp, _i32, _vp]),
     'renet_loader_wait': (ctypes.c_int, [_vp, _i64]),
     'renet_prepare_sequences': (ctypes.c_int, [_vp, _i32, _i32, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     'renet_pack_inputs': (ctypes.c_int, [_vp] * 12 + [_i64, _i32, _vp]),

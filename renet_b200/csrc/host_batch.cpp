@@ -212,20 +212,19 @@ extern "C" int renet_host_assemble_batch(
     const int64_t* h_samp_off, const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow, const int64_t* h_ent_off,
     const int32_t* h_nbr_row,
     // ---- batch --------------------------------------------------------------------------------------
-    const int64_t* sample_idx, int64_t B, int32_t sort, int32_t R2, int32_t n_hot_max,
+    const int64_t* sample_idx, int64_t B, int32_t sort,
     // ---- outputs --------------------------------------------------------------------------------------
-    int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* comp_graph_out, int32_t* batch_sizes_out,
-    int32_t max_len_capacity,
-    int64_t* sizes /* [10]: N, E, S, Q, G, max_len, words_used, n_hot_s, n_hot_o, 0 */) {
-  if (B < 0 || !sizes || R2 < 0 || n_hot_max < 0) { renet::set_error("renet_host_assemble_batch: bad arguments"); return RENET_ERR_INVALID_ARG; }
+    int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
+    int64_t* sizes /* [10]: N, E, S, Q, G, max_len, words_used, 0, 0, 0 */) {
+  if (B < 0 || !sizes) { renet::set_error("renet_host_assemble_batch: bad arguments"); return RENET_ERR_INVALID_ARG; }
   Plan P;
   int prc = build_plan(P, "renet_host_assemble_batch", T, g_node_off, g_node_ent, h_samp_off, h_samp_entry, h_ent_graph, h_ent_srow,
                        h_ent_off, h_nbr_row, sample_idx, B, sort, s_idx_out, max_len_capacity);
   if (prc != RENET_OK) return prc;
   const int64_t Q = P.Q, S = P.S, G = P.G, N = P.N;
-  const int max_len = P.max_len;
-  sizes[2] = S; sizes[3] = Q; sizes[5] = max_len;
-  if (S == 0) { sizes[0] = sizes[1] = sizes[4] = sizes[6] = 0; return RENET_OK; }
+  for (int i = 0; i < 10; ++i) sizes[i] = 0;
+  sizes[2] = S; sizes[3] = Q; sizes[5] = P.max_len;
+  if (S == 0) return RENET_OK;
   const std::vector<int32_t>& comp_graph = P.comp_graph;
   const int32_t* newid = P.nid;
   const std::vector<int64_t>& mark_off = P.mark_off;
@@ -244,9 +243,8 @@ extern "C" int renet_host_assemble_batch(
   // layout of `out` (int32 words):
   //  node_ent[N] row_ptr[N+1] col_src[E] col_type_s[E] col_type_o[E] norm[N](f32 bits)
   //  readout[S] row_comp[S] row_seq[S] seq_start[Q] seq_len[Q] packed_row[S]
-  //  comp_ptr[G+1] comp_order[G] rel_slot_s[R2] hot_s[n_hot_max] rel_slot_o[R2] hot_o[n_hot_max]
-  //  s_idx[B] comp_graph[G]      (device copies of the two small host outputs, so no separate H2D is needed)
-  const int64_t words = N + (N + 1) + 3 * E + N + 3 * S + 2 * Q + S + (G + 1) + G + 2 * (int64_t)(R2 + n_hot_max) + B + G;
+  //  s_idx[B] comp_graph[G]      (s_idx: device copy of s_idx_out, so no separate H2D is needed)
+  const int64_t words = N + (N + 1) + 3 * E + N + 3 * S + 2 * Q + S + B + G;
   sizes[0] = N; sizes[1] = E; sizes[4] = G; sizes[6] = words;
   if (words > out_capacity) return 1;   // caller grows the staging buffer and retries
   int32_t* o_node = out;
@@ -284,36 +282,7 @@ extern "C" int renet_host_assemble_batch(
   }
   // ---- 6. read-out rows + sequence bookkeeping ------------------------------------------------------------------
   emit_sequences(P, s_idx_out, o_readout, o_rowcomp, o_rowseq, o_seqstart, o_seqlen, o_packed, batch_sizes_out);
-  for (int64_t c = 0; c < G; ++c) comp_graph_out[c] = comp_graph[c];
-  // ---- 7. component table (largest first) and the hottest relations of this batch, for renet_rgcn_gather_comp ----
-  int32_t* o_cptr = o_packed + S;
-  int32_t* o_corder = o_cptr + G + 1;
-  for (int64_t c = 0; c <= G; ++c) o_cptr[c] = (int32_t)comp_start[c];
-  for (int64_t c = 0; c < G; ++c) o_corder[c] = (int32_t)c;
-  std::stable_sort(o_corder, o_corder + G, [&](int32_t a, int32_t b) {
-    return comp_estart[a + 1] - comp_estart[a] > comp_estart[b + 1] - comp_estart[b];
-  });
-  int32_t* o_hot = o_corder + G;
-  const int32_t* cols[2] = {o_ts, o_to};
-  std::vector<int64_t> cnt(R2);
-  std::vector<int32_t> ids(R2);
-  for (int w = 0; w < 2; ++w) {
-    int32_t* slot = o_hot + w * (R2 + n_hot_max);
-    int32_t* hot = slot + R2;
-    std::fill(cnt.begin(), cnt.end(), 0);
-    for (int64_t k = 0; k < E; ++k) {
-      const int32_t t = cols[w][k];
-      if ((uint32_t)t >= (uint32_t)R2) { renet::set_error("renet_host_assemble_batch: edge type %d out of range [0,%d)", t, R2); return RENET_ERR_INVALID_ARG; }
-      cnt[t]++;
-    }
-    for (int32_t i = 0; i < R2; ++i) { ids[i] = i; slot[i] = -1; }
-    std::stable_sort(ids.begin(), ids.end(), [&](int32_t a, int32_t b) { return cnt[a] > cnt[b]; });
-    int32_t nh = 0;
-    for (; nh < n_hot_max && nh < R2 && cnt[ids[nh]] > 0; ++nh) { hot[nh] = ids[nh]; slot[ids[nh]] = nh; }
-    for (int32_t i = nh; i < n_hot_max; ++i) hot[i] = 0;
-    sizes[7 + w] = nh;
-  }
-  int32_t* o_sidx = o_hot + 2 * (R2 + n_hot_max);
+  int32_t* o_sidx = o_packed + S;
   for (int64_t i = 0; i < B; ++i) o_sidx[i] = (int32_t)s_idx_out[i];
   int32_t* o_cg = o_sidx + B;
   for (int64_t c = 0; c < G; ++c) o_cg[c] = comp_graph[c];
@@ -479,15 +448,14 @@ extern "C" int64_t renet_loader_submit_assemble(
     void* loader, int64_t T, const int64_t* g_node_off, const int32_t* g_node_ent, const int64_t* g_edge_off,
     const int32_t* g_src, const int32_t* g_dst, const int32_t* g_type_s, const int32_t* g_type_o,
     const int64_t* h_samp_off, const int64_t* h_samp_entry, const int32_t* h_ent_graph, const int32_t* h_ent_srow,
-    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort, int32_t R2,
-    int32_t n_hot_max, int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* comp_graph_out,
-    int32_t* batch_sizes_out, int32_t max_len_capacity, int64_t* sizes) {
+    const int64_t* h_ent_off, const int32_t* h_nbr_row, const int64_t* sample_idx, int64_t B, int32_t sort,
+    int64_t* s_idx_out, int32_t* out, int64_t out_capacity, int32_t* batch_sizes_out, int32_t max_len_capacity,
+    int64_t* sizes) {
   if (!loader) return -1;
   return static_cast<Loader*>(loader)->submit([=]() {
     return renet_host_assemble_batch(T, g_node_off, g_node_ent, g_edge_off, g_src, g_dst, g_type_s, g_type_o, h_samp_off,
-                                     h_samp_entry, h_ent_graph, h_ent_srow, h_ent_off, h_nbr_row, sample_idx, B, sort, R2,
-                                     n_hot_max, s_idx_out, out, out_capacity, comp_graph_out, batch_sizes_out,
-                                     max_len_capacity, sizes);
+                                     h_samp_entry, h_ent_graph, h_ent_srow, h_ent_off, h_nbr_row, sample_idx, B, sort,
+                                     s_idx_out, out, out_capacity, batch_sizes_out, max_len_capacity, sizes);
   });
 }
 

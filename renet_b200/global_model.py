@@ -56,8 +56,8 @@ def whole_graph_arrays(graphs):
 
 def batch_whole_graphs(graphs, device):
     """dgl.batch + move_dgl_to_cuda of whole graphs: BatchedHistoryGraph + node offsets [G+1] on the device."""
-    node_ent, norm, row_ptr, src, ts, to, sizes, off = whole_graph_arrays(graphs)
-    bg = BatchedHistoryGraph(node_ent, norm, row_ptr, src, ts, to, sizes, device)
+    node_ent, norm, row_ptr, src, ts, to, _, off = whole_graph_arrays(graphs)
+    bg = BatchedHistoryGraph(node_ent, norm, row_ptr, src, ts, to, device)
     seg = torch.from_numpy(off.astype(np.int32)).to(device)
     return bg, seg
 

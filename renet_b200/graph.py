@@ -141,16 +141,12 @@ class BatchedHistoryGraph:
 
     Equivalent of ``dgl.batch(g_list)`` + ``move_dgl_to_cuda`` (reference utils.py:237-241)."""
 
-    def __init__(self, node_ent, norm, row_ptr, col_src, col_type_s, col_type_o, comp_sizes, device, extras=None):
+    def __init__(self, node_ent, norm, row_ptr, col_src, col_type_s, col_type_o, device):
         self.device = torch.device(device)
         self.N = int(len(node_ent))
         self.E = int(len(col_src))
-        self.comp_sizes = comp_sizes
         # one pinned staging buffer -> one H2D copy
         parts = [node_ent, row_ptr, col_src, col_type_s, col_type_o]
-        names = ['comp_ptr', 'comp_order', 'rel_slot_s', 'hot_s', 'rel_slot_o', 'hot_o']
-        if extras is not None:
-            parts += [extras[k] for k in names]
         i32 = np.concatenate([np.asarray(p).astype(np.int32) for p in parts])
         dev = _to_device(torch.from_numpy(i32), self.device)
         o = 0
@@ -158,41 +154,13 @@ class BatchedHistoryGraph:
         self.row_ptr = dev[o:o + self.N + 1]; o += self.N + 1
         self.col_src = dev[o:o + self.E]; o += self.E
         self.col_type_s = dev[o:o + self.E]; o += self.E
-        self.col_type_o = dev[o:o + self.E]; o += self.E
-        self.comp, self.G = None, 0
-        if extras is not None:
-            t = {}
-            for k in names:
-                n = len(extras[k])
-                t[k] = dev[o:o + n]; o += n
-            self.G = len(extras['comp_order'])
-            self.comp = {False: (t['comp_ptr'], t['comp_order'], t['rel_slot_s'], t['hot_s'], int(extras['n_hot_s'])),
-                         True: (t['comp_ptr'], t['comp_order'], t['rel_slot_o'], t['hot_o'], int(extras['n_hot_o']))}
+        self.col_type_o = dev[o:o + self.E]
         self.norm = _to_device(torch.from_numpy(np.ascontiguousarray(norm, dtype=np.float32)), self.device)
         self.h2d_bytes = i32.nbytes + self.N * 4
         self.ndata = _Frame(norm=self.norm.view(-1, 1), id=self.node_ent.view(-1, 1))
         self.h_index = None          # when set, ndata['h'] is virtual: H = table[h_index]
         self.h_table = None
         self._bwd = {}
-
-    @classmethod
-    def from_coo(cls, node_ent, norm, src, dst, type_s, type_o, device, comp_sizes=None):
-        """General entry (any edge order): builds the CSR on the GPU with renet_build_csr."""
-        n, e = len(node_ent), len(src)
-        g = cls.__new__(cls)
-        g.device = torch.device(device)
-        g.N, g.E, g.comp_sizes = n, e, comp_sizes
-        t = lambda a, dt: _to_device(torch.from_numpy(np.ascontiguousarray(a, dtype=dt)), g.device)
-        g.node_ent, g.norm = t(node_ent, np.int32), t(norm, np.float32)
-        d_src, d_dst, d_ts, d_to = t(src, np.int32), t(dst, np.int32), t(type_s, np.int32), t(type_o, np.int32)
-        g.row_ptr, g.col_src, g.col_type_s, perm = build_csr(d_dst, d_src, d_ts, n, want_perm=True)
-        g.col_type_o = d_to[perm.long()] if e else d_to
-        g.h2d_bytes = (n * 2 + e * 4) * 4
-        g.ndata = _Frame(norm=g.norm.view(-1, 1), id=g.node_ent.view(-1, 1))
-        g.h_index = g.h_table = None
-        g._bwd = {}
-        g.comp, g.G = None, 0
-        return g
 
     # ---- edge count: known on the host for host-assembled batches; for device-assembled ones (hoststore, device
     # batcher) it is produced on the GPU and read back lazily, so nothing on the forward path waits for it ------------

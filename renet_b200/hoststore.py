@@ -22,7 +22,6 @@ from .graph import BatchedHistoryGraph, PendingCount, _Frame, as_history_graph
 from .utils import HistoryBatch
 
 MAX_LEN = 16
-N_HOT = 40          # relation rows renet_rgcn_gather_comp keeps in shared memory (kHotRel)
 
 
 def _p(a):
@@ -36,7 +35,6 @@ class GraphStore:
     def __init__(self, graph_dict):
         self.graph_dict = graph_dict
         self.times = np.asarray(sorted(int(t) for t in graph_dict.keys()), dtype=np.int64)
-        self.index_of = {int(t): i for i, t in enumerate(self.times)}
         graphs = [as_history_graph(graph_dict[int(t)]) for t in self.times]
         for g in graphs:
             if not g._sorted:
@@ -49,6 +47,8 @@ class GraphStore:
         self.dst = cat([g.dst for g in graphs], np.int32)
         self.type_s = cat([g.type_s for g in graphs], np.int32)
         self.type_o = cat([g.type_o for g in graphs], np.int32)
+        if len(self.type_s) and min(self.type_s.min(), self.type_o.min()) < 0:
+            raise ValueError('GraphStore: edge types must be >= 0 (they index the relation weights)')
         self.graphs = graphs
         self.num_types = int(max(self.type_s.max(), self.type_o.max())) + 1 if len(self.type_s) else 1
         self._dev = {}
@@ -118,14 +118,6 @@ class GraphStore:
             bad = int(np.flatnonzero(missing)[0])
             raise KeyError('entity %d not present in the graph of timestamp %d' % (int(entities[bad]), int(self.times[gi[bad]])))
         return rows
-
-    def local_rows(self, gi, entities):
-        lo = self.node_off[gi]
-        ent = self.node_ent[lo:self.node_off[gi + 1]]
-        rows = np.searchsorted(ent, entities)
-        if np.any(rows >= len(ent)) or np.any(ent[np.minimum(rows, len(ent) - 1)] != entities):
-            raise KeyError('entity not present in the graph of timestamp %d' % int(self.times[gi]))
-        return rows.astype(np.int32)
 
 
 class HistoryStore:
@@ -246,28 +238,37 @@ def reserve_pinned(n, words=1 << 21):
         _PINNED_POOL.append(torch.empty(words, dtype=torch.int32).pin_memory())
 
 
+def _result(rc, name, plan, sizes, s_idx, bsz, out):
+    """What a batcher call into the int32 buffer ``out`` returns, from its return code and outputs: {'need_words': n}
+    when the buffer was too small, else the batch's sizes and small host arrays (sizes[] as renet_host_assemble_batch /
+    renet_host_plan_batch document them)."""
+    if rc == 1:
+        return {'need_words': int(sizes[6])}
+    _lib.check(rc, name)
+    N, E, S, Q, G, max_len, words, M = (int(x) for x in sizes[:8])
+    r = dict(N=N, S=S, Q=Q, G=G, max_len=max_len, words=words, s_idx=s_idx, batch_sizes=bsz[:max_len].copy(), B=len(s_idx))
+    if plan:
+        r.update(E_cand=E, M=M, plan=True)
+    else:      # the all-host layout ends with comp_graph[G]; copied, since the staging buffer is reused
+        r.update(E=E, comp_graph=out[words - G:words].copy())
+    return r
+
+
 def assemble_view_raw(view, out, sort=True):
-    """Run the C++ batcher into the int32 numpy buffer ``out`` (host only, no CUDA).  Returns None when
-    the buffer is too small (sizes[6] words are needed), else a dict of sizes + small host arrays."""
+    """Run the C++ batcher into the int32 numpy buffer ``out`` (host only, no CUDA); returns _result's dict."""
     if view.groups is not None:
         raise ValueError('isolation groups need the device batcher (device_edges=True)')
     L = _lib.lib()
     hs, gs = view.store, view.store.gs
     B = len(view.sample_idx)
     s_idx = np.empty(B, dtype=np.int64)
-    comp_graph = np.empty(len(gs.times), dtype=np.int32)
     bsz = np.zeros(MAX_LEN, dtype=np.int32)
     sizes = np.zeros(10, dtype=np.int64)
     rc = L.renet_host_assemble_batch(
         len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(gs.src), _p(gs.dst), _p(gs.type_s),
         _p(gs.type_o), _p(hs.samp_off), _p(hs.samp_entry), _p(hs.ent_graph), _p(hs.ent_srow), _p(hs.ent_off), _p(hs.nbr_row),
-        _p(view.sample_idx), B, int(sort), gs.num_types, N_HOT, _p(s_idx), _p(out), out.size, _p(comp_graph), _p(bsz), MAX_LEN, _p(sizes))
-    if rc == 1:
-        return {'need_words': int(sizes[6])}
-    _lib.check(rc, 'renet_host_assemble_batch')
-    N, E, S, Q, G, max_len, words = (int(x) for x in sizes[:7])
-    return dict(N=N, E=E, S=S, Q=Q, G=G, max_len=max_len, words=words, s_idx=s_idx, comp_graph=comp_graph[:G],
-                batch_sizes=bsz[:max_len].copy(), R2=gs.num_types, n_hot_s=int(sizes[7]), n_hot_o=int(sizes[8]), B=B)
+        _p(view.sample_idx), B, int(sort), _p(s_idx), _p(out), out.size, _p(bsz), MAX_LEN, _p(sizes))
+    return _result(rc, 'renet_host_assemble_batch', False, sizes, s_idx, bsz, out)
 
 
 def split_raw(buf, r):
@@ -277,9 +278,7 @@ def split_raw(buf, r):
     out = {}
     for name, n in (('node_ent', N), ('row_ptr', N + 1), ('col_src', E), ('col_type_s', E), ('col_type_o', E),
                     ('norm', N), ('readout', S), ('row_comp', S), ('row_seq', S), ('seq_start', Q), ('seq_len', Q),
-                    ('packed_row', S), ('comp_ptr', r['G'] + 1), ('comp_order', r['G']), ('rel_slot_s', r['R2']),
-                    ('hot_s', N_HOT), ('rel_slot_o', r['R2']), ('hot_o', N_HOT), ('s_idx', r['B']),
-                    ('comp_graph', r['G'])):
+                    ('packed_row', S), ('s_idx', r['B']), ('comp_graph', r['G'])):
         out[name] = buf[o:o + n]
         o += n
     return out
@@ -287,7 +286,7 @@ def split_raw(buf, r):
 
 def plan_view_raw(view, out, sort=True):
     """Host half of the device batcher (renet_host_plan_batch_grouped, with the view's isolation groups if it has any)
-    into the int32 numpy buffer ``out``."""
+    into the int32 numpy buffer ``out``; returns _result's dict."""
     L = _lib.lib()
     hs, gs = view.store, view.store.gs
     B = len(view.sample_idx)
@@ -299,12 +298,7 @@ def plan_view_raw(view, out, sort=True):
         len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(hs.samp_off), _p(hs.samp_entry), _p(hs.ent_graph),
         _p(hs.ent_srow), _p(hs.ent_off), _p(hs.nbr_row), _p(view.sample_idx), groups, B, int(sort), _p(s_idx), _p(out),
         out.size, _p(bsz), MAX_LEN, _p(sizes))
-    if rc == 1:
-        return {'need_words': int(sizes[6])}
-    _lib.check(rc, 'renet_host_plan_batch')
-    N, E_cand, S, Q, G, max_len, words, M = (int(x) for x in sizes[:8])
-    return dict(N=N, E_cand=E_cand, S=S, Q=Q, G=G, max_len=max_len, words=words, M=M, s_idx=s_idx,
-                batch_sizes=bsz[:max_len].copy(), B=B, plan=True)
+    return _result(rc, 'renet_host_plan_batch', True, sizes, s_idx, bsz, out)
 
 
 def split_plan(buf, r):
@@ -346,9 +340,8 @@ class NativeLoader:
             raise ValueError('NativeLoader: isolation groups are not supported; use assemble_view')
         hs, gs = view.store, view.store.gs
         B = len(view.sample_idx)
-        job = dict(view=view, out=out, sort=sort, device_edges=device_edges, B=B, s_idx=np.empty(B, dtype=np.int64),
-                   bsz=np.zeros(MAX_LEN, dtype=np.int32), sizes=np.zeros(10, dtype=np.int64),
-                   comp_graph=np.empty(len(gs.times), dtype=np.int32))
+        job = dict(view=view, out=out, sort=sort, device_edges=device_edges, s_idx=np.empty(B, dtype=np.int64),
+                   bsz=np.zeros(MAX_LEN, dtype=np.int32), sizes=np.zeros(10, dtype=np.int64))
         if device_edges:
             t = self.L.renet_loader_submit_plan(
                 self.h, len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(hs.samp_off), _p(hs.samp_entry),
@@ -358,8 +351,8 @@ class NativeLoader:
             t = self.L.renet_loader_submit_assemble(
                 self.h, len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(gs.src), _p(gs.dst), _p(gs.type_s),
                 _p(gs.type_o), _p(hs.samp_off), _p(hs.samp_entry), _p(hs.ent_graph), _p(hs.ent_srow), _p(hs.ent_off),
-                _p(hs.nbr_row), _p(view.sample_idx), B, int(sort), gs.num_types, N_HOT, _p(job['s_idx']), _p(out), out.size,
-                _p(job['comp_graph']), _p(job['bsz']), MAX_LEN, _p(job['sizes']))
+                _p(hs.nbr_row), _p(view.sample_idx), B, int(sort), _p(job['s_idx']), _p(out), out.size, _p(job['bsz']),
+                MAX_LEN, _p(job['sizes']))
         if t < 0:
             raise RuntimeError('renet_loader_submit failed')
         job['ticket'] = t
@@ -368,19 +361,7 @@ class NativeLoader:
     def finish(self, job):
         """Wait for the job; returns the dict plan_view_raw / assemble_view_raw return."""
         rc = self.L.renet_loader_wait(self.h, job['ticket'])
-        sizes = job['sizes']
-        if rc == 1:
-            return {'need_words': int(sizes[6])}
-        _lib.check(rc, 'renet_loader job')
-        if job['device_edges']:
-            N, E_cand, S, Q, G, max_len, words, M = (int(x) for x in sizes[:8])
-            return dict(N=N, E_cand=E_cand, S=S, Q=Q, G=G, max_len=max_len, words=words, M=M, s_idx=job['s_idx'],
-                        batch_sizes=job['bsz'][:max_len].copy(), B=job['B'], plan=True)
-        N, E, S, Q, G, max_len, words = (int(x) for x in sizes[:7])
-        gs = job['view'].store.gs
-        return dict(N=N, E=E, S=S, Q=Q, G=G, max_len=max_len, words=words, s_idx=job['s_idx'],
-                    comp_graph=job['comp_graph'][:G], batch_sizes=job['bsz'][:max_len].copy(), R2=gs.num_types,
-                    n_hot_s=int(sizes[7]), n_hot_o=int(sizes[8]), B=job['B'])
+        return _result(rc, 'renet_loader job', job['device_edges'], job['sizes'], job['s_idx'], job['bsz'], job['out'])
 
 
 _E_PINNED = __import__('collections').deque()       # pool of pinned int32[1] read-back slots
@@ -395,15 +376,38 @@ def _loader_stream(device):
     return st
 
 
-def _upload_plan(view, buf, r, device):
+def _fill(hb, view, r, d, h, csr, device):
+    """The fields both batchers set alike: ``hb`` and its BatchedHistoryGraph over the staged buffer's device views ``d``
+    (host views ``h``) and the CSR arrays ``csr``.  Returns the graph; its edge count is left to the caller."""
+    gs = view.store.gs
+    g = BatchedHistoryGraph.__new__(BatchedHistoryGraph)
+    g.device, g.N = torch.device(device), r['N']
+    g.node_ent, g.row_ptr = d['node_ent'], csr['row_ptr']
+    g.col_src, g.col_type_s, g.col_type_o = csr['col_src'], csr['col_type_s'], csr['col_type_o']
+    g.norm = csr['norm'].view(torch.float32)
+    g.h2d_bytes = r['words'] * 4
+    g.ndata = _Frame(norm=g.norm.view(-1, 1), id=g.node_ent.view(-1, 1))
+    g.h_index = g.h_table = None
+    g._bwd = {}
+    g.seq_len_dev = d['seq_len']
+    g.hot = gs.hot_relations(device)
+    hb.graph = g
+    hb.readout, hb.row_glob, hb.row_seq = d['readout'], d['row_comp'], d['row_seq']
+    hb.seq_start, hb.packed_row = d['seq_start'], d['packed_row']
+    hb.readout_host = h['readout'].astype(np.int64)
+    hb.seq_len = h['seq_len'].astype(np.int64)
+    hb.batch_sizes = r['batch_sizes']
+    hb.times = gs.times[h['comp_graph']]
+    hb.h2d_bytes = r['words'] * 4
+    hb.s_idx_dev, hb.comp_graph_dev = d['s_idx'], d['comp_graph']     # device copies: no pageable H2D later
+    hb.graph_store = gs
+    return g
+
+
+def _upload_plan(hb, view, buf, r, device):
     """Device part of the device batcher (caller's thread / current stream): one pinned H2D copy of the plan, then
     renet_induce_edges builds the CSR on the GPU from the resident graph store; the edge count comes back
     asynchronously (graph.E resolves it on demand)."""
-    hb = HistoryBatch()
-    hb.s_idx, hb.num_seq, hb.S = r['s_idx'], r['Q'], r['S']
-    if r['S'] == 0:
-        hb.graph, hb.seq_len = None, np.zeros(0, np.int64)
-        return hb, None
     L = _lib.lib()
     gs = view.store.gs
     ga = gs.device_arrays(device)
@@ -435,20 +439,8 @@ def _upload_plan(view, buf, r, device):
                                   P(parts['row_ptr']), P(parts['col_src']), P(parts['col_type_s']), P(parts['col_type_o']),
                                   P(parts['norm']), P(parts['e_count']), P(ws), ws.numel() * 4, _lib.stream())
         _lib.check(rc, 'renet_induce_edges')
-    g = BatchedHistoryGraph.__new__(BatchedHistoryGraph)
-    g.device, g.N = torch.device(device), N
+    g = _fill(hb, view, r, d, h, parts, device)
     g.E_cap = E_cand
-    g.node_ent, g.row_ptr = d['node_ent'], parts['row_ptr']
-    g.col_src, g.col_type_s, g.col_type_o = parts['col_src'], parts['col_type_s'], parts['col_type_o']
-    g.norm = parts['norm'].view(torch.float32)
-    g.comp_sizes = None
-    g.h2d_bytes = words * 4
-    g.ndata = _Frame(norm=g.norm.view(-1, 1), id=g.node_ent.view(-1, 1))
-    g.h_index = g.h_table = None
-    g._bwd = {}
-    g.G, g.comp = r['G'], None
-    g.seq_len_dev = d['seq_len']
-    g.hot = gs.hot_relations(device)
     g._keep = (blob, dev)
     with torch.cuda.stream(ls):
         rev = getattr(view.store, 'reverse', None)
@@ -472,16 +464,6 @@ def _upload_plan(view, buf, r, device):
         for t in sub._keep:
             t.record_stream(main)
     g._E_pending = PendingCount(e_ev, e_host, _E_PINNED.append)
-    hb.graph = g
-    hb.readout, hb.row_glob, hb.row_seq = d['readout'], d['row_comp'], d['row_seq']
-    hb.seq_start, hb.packed_row = d['seq_start'], d['packed_row']
-    hb.readout_host = h['readout'].astype(np.int64)
-    hb.seq_len = h['seq_len'].astype(np.int64)
-    hb.batch_sizes = r['batch_sizes']
-    hb.times = gs.times[h['comp_graph']]
-    hb.h2d_bytes = words * 4
-    hb.s_idx_dev, hb.comp_graph_dev = d['s_idx'], d['comp_graph']
-    hb.graph_store = gs
     return hb, ev
 
 
@@ -497,45 +479,20 @@ def _stage(view, buf_holder, sort, device_edges=False):
 
 
 def _upload(view, buf, r, device):
-    """Device part (caller's thread / current stream): one pinned H2D copy, then slice it into the batch."""
-    if r.get('plan'):
-        return _upload_plan(view, buf, r, device)
+    """Device part (caller's thread / current stream): one pinned H2D copy, then slice it into the batch.  Returns the
+    HistoryBatch and the event after which ``buf`` may be reused (None when nothing was copied)."""
     hb = HistoryBatch()
     hb.s_idx, hb.num_seq, hb.S = r['s_idx'], r['Q'], r['S']
     if r['S'] == 0:
         hb.graph, hb.seq_len = None, np.zeros(0, np.int64)
         return hb, None
-    words = r['words']
-    dev = buf[:words].to(device, non_blocking=True)
+    if r.get('plan'):
+        return _upload_plan(hb, view, buf, r, device)
+    dev = buf[:r['words']].to(device, non_blocking=True)
     ev = torch.cuda.Event()
     ev.record()
     d = split_raw(dev, r)
-    h = split_raw(buf.numpy(), r)
-    g = BatchedHistoryGraph.__new__(BatchedHistoryGraph)
-    g.device, g.N, g.E = torch.device(device), r['N'], r['E']
-    g.node_ent, g.row_ptr = d['node_ent'], d['row_ptr']
-    g.col_src, g.col_type_s, g.col_type_o = d['col_src'], d['col_type_s'], d['col_type_o']
-    g.norm = d['norm'].view(torch.float32)
-    g.comp_sizes = None
-    g.h2d_bytes = words * 4
-    g.ndata = _Frame(norm=g.norm.view(-1, 1), id=g.node_ent.view(-1, 1))
-    g.h_index = g.h_table = None
-    g._bwd = {}
-    g.G = r['G']
-    g.comp = {False: (d['comp_ptr'], d['comp_order'], d['rel_slot_s'], d['hot_s'], r['n_hot_s']),
-              True: (d['comp_ptr'], d['comp_order'], d['rel_slot_o'], d['hot_o'], r['n_hot_o'])}
-    g.seq_len_dev = d['seq_len']
-    g.hot = view.store.gs.hot_relations(device)
-    hb.graph = g
-    hb.readout, hb.row_glob, hb.row_seq = d['readout'], d['row_comp'], d['row_seq']
-    hb.seq_start, hb.packed_row = d['seq_start'], d['packed_row']
-    hb.readout_host = h['readout'].astype(np.int64)
-    hb.seq_len = h['seq_len'].astype(np.int64)
-    hb.batch_sizes = r['batch_sizes']
-    hb.times = view.store.gs.times[r['comp_graph']]
-    hb.h2d_bytes = words * 4
-    hb.s_idx_dev, hb.comp_graph_dev = d['s_idx'], d['comp_graph']     # device copies: no pageable H2D later
-    hb.graph_store = view.store.gs
+    _fill(hb, view, r, d, split_raw(buf.numpy(), r), d, device).E = r['E']
     return hb, ev
 
 

@@ -120,7 +120,6 @@ def assemble_history_batch_host(s_hist, s_hist_t, s_host, graph_dict, sort=True)
     type_s, type_o = np.concatenate(tss), np.concatenate(tos)
     hb.graph = dict(node_ent=node_ent, norm=norm, row_ptr=row_ptr, col_src=src, col_type_s=type_s,
                     col_type_o=type_o, comp_sizes=comp_sizes)
-    hb.graph['extras'] = component_extras(comp_start, np.asarray([len(x) for x in srcs]), type_s, type_o)
     # ---- sequence bookkeeping (pack_padded_sequence order, Aggregator.py:160-165) ------------------
     seq_start = np.concatenate(([0], np.cumsum(seq_len)[:-1]))
     max_len = int(seq_len[0]) if sort else int(seq_len.max())
@@ -133,29 +132,6 @@ def assemble_history_batch_host(s_hist, s_hist_t, s_host, graph_dict, sort=True)
     return hb
 
 
-N_HOT = 40     # relation rows renet_rgcn_gather_comp keeps in shared memory (kHotRel in rgcn_comp.cuh)
-
-
-def component_extras(comp_start, comp_edges, type_s, type_o, num_types=None):
-    """What renet_rgcn_gather_comp needs besides the CSR: component node offsets, components ordered by edge
-    count (largest first, stable), and per type column the N_HOT most frequent edge types of the batch
-    (rel_slot[type] = slot or -1; ties broken by type id).  Same rule as renet_host_assemble_batch."""
-    G = len(comp_edges)
-    order = np.argsort(-np.asarray(comp_edges, dtype=np.int64), kind='stable')
-    R2 = int(num_types) if num_types is not None else (int(max(type_s.max(), type_o.max())) + 1 if len(type_s) else 1)
-    out = dict(comp_ptr=np.asarray(comp_start, dtype=np.int32), comp_order=order.astype(np.int32))
-    for tag, col in (('s', type_s), ('o', type_o)):
-        cnt = np.bincount(col, minlength=R2)
-        ids = np.argsort(-cnt, kind='stable')
-        nh = int(min(N_HOT, np.count_nonzero(cnt)))
-        slot = np.full(R2, -1, dtype=np.int32)
-        slot[ids[:nh]] = np.arange(nh, dtype=np.int32)
-        hot = np.zeros(N_HOT, dtype=np.int32)
-        hot[:nh] = ids[:nh]
-        out['rel_slot_' + tag], out['hot_' + tag], out['n_hot_' + tag] = slot, hot, nh
-    return out
-
-
 def upload_history_batch(hb, device):
     """Device half: two pinned host->device copies (graph structure, sequence bookkeeping)."""
     if hb.graph is None:
@@ -163,7 +139,7 @@ def upload_history_batch(hb, device):
     g = hb.graph
     S, Q = hb.S, hb.num_seq
     hb.graph = BatchedHistoryGraph(g['node_ent'], g['norm'], g['row_ptr'], g['col_src'], g['col_type_s'],
-                                   g['col_type_o'], g['comp_sizes'], device, extras=g.get('extras'))
+                                   g['col_type_o'], device)
     i32 = np.concatenate(hb.readout).astype(np.int32)
     dev = torch.from_numpy(i32).pin_memory().to(device, non_blocking=True)
     o = 0

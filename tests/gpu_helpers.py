@@ -15,7 +15,7 @@ def d(x, dtype=None):
     return t.to(DEV)
 
 
-def csr_from_coo(src, dst, etype, N):
+def coo_to_csr(src, dst, etype, N):
     """device CSR by destination via renet_build_csr -> (row_ptr, col_src, col_type)"""
     rp, cs, ct, _ = build_csr(d(dst, torch.int32), d(src, torch.int32), d(etype, torch.int32), N)
     return rp, cs, ct

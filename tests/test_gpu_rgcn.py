@@ -32,7 +32,7 @@ def test_golden_layer_cases_forward(G):
         c = layer_case(blob, str(name))
         N, E = int(c['N']), len(c['src'])
         H, W, Wl, et = _case_tensors(G, c)
-        rp, cs, ct = G.csr_from_coo(c['src'], c['dst'], et, N)
+        rp, cs, ct = G.coo_to_csr(c['src'], c['dst'], et, N)
         out = G.layer_fwd(H, None, W, Wl, rp, cs, ct, G.d(c['ref_norm']), N, E, int(c['d_in']), int(c['d_out']),
                           int(c['nb']), bool(c['relu']))
         err = rel_err(out.cpu().numpy(), c['ref_out'])
@@ -47,7 +47,7 @@ def test_golden_layer_cases_backward(G):
         c = layer_case(blob, str(name))
         N, E = int(c['N']), len(c['src'])
         H, W, Wl, et = _case_tensors(G, c)
-        rp, cs, ct = G.csr_from_coo(c['src'], c['dst'], et, N)
+        rp, cs, ct = G.coo_to_csr(c['src'], c['dst'], et, N)
         norm = G.d(c['ref_norm'])
         out = G.layer_fwd(H, None, W, Wl, rp, cs, ct, norm, N, E, int(c['d_in']), int(c['d_out']), int(c['nb']),
                           bool(c['relu']))
@@ -163,7 +163,7 @@ def test_full_size_properties(G):
     H = torch.randn(N, 200, device=G.DEV)
     W = torch.randn(R2, 400, device=G.DEV) * 0.1
     Wl = torch.randn(200, 200, device=G.DEV) * 0.07
-    rp, cs, ct = G.csr_from_coo(src, dst, et, N)
+    rp, cs, ct = G.coo_to_csr(src, dst, et, N)
     # device CSR == host CSR (stable)
     order = np.argsort(dst, kind='stable')
     np.testing.assert_array_equal(cs.cpu().numpy(), src[order])
@@ -173,7 +173,7 @@ def test_full_size_properties(G):
     b = G.layer_fwd(H * 3.0, None, W, Wl, rp, cs, ct, norm, N, E, 200, 200, 100, False)
     assert rel_err(b.cpu().numpy(), (a * 3.0).cpu().numpy()) < 1e-5
     perm = rng.permutation(E)
-    rp2, cs2, ct2 = G.csr_from_coo(src[perm], dst[perm], et[perm], N)
+    rp2, cs2, ct2 = G.coo_to_csr(src[perm], dst[perm], et[perm], N)
     c = G.layer_fwd(H, None, W, Wl, rp2, cs2, ct2, norm, N, E, 200, 200, 100, False)
     assert rel_err(c.cpu().numpy(), a.cpu().numpy()) < 1e-5
     # the gather hands partial sums between warps in a fixed order (no atomics): bitwise reproducible, so
@@ -214,7 +214,7 @@ def test_batch_scale_kernel_edge_cases_fwd_bwd_vs_oracle(G, N, E, heavy, empty_f
         pre = restate.rgcn_block_layer(H, W, Wl, t(src), t(dst), t(et), t(norm), False, 100)
     Gout = torch.randn(ref.shape) * (pre.abs() > 1e-4)
     (ref * Gout).sum().backward()
-    rp, cs, ct = G.csr_from_coo(src, dst, et, N)
+    rp, cs, ct = G.coo_to_csr(src, dst, et, N)
     Hd, Wd, Wld, nd = H.to(G.DEV), W.to(G.DEV), Wl.to(G.DEV), G.d(norm)
     out = G.layer_fwd(Hd, None, Wd, Wld, rp, cs, ct, nd, N, E, 200, 200, 100, True)
     assert rel_err(out.cpu().numpy(), ref.detach().numpy()) < TOL
@@ -236,7 +236,7 @@ def test_hot_relation_list_only_changes_where_rows_are_read_from(G):
     dst = rng.zipf(1.4, E) % N
     et = (rng.zipf(1.3, E) % R2).astype(np.int64)                  # skewed relation frequencies, as in the datasets
     deg = np.bincount(dst, minlength=N).astype(np.float32); deg[deg == 0] = 1
-    rp, cs, ct = G.csr_from_coo(src, dst, et, N)
+    rp, cs, ct = G.coo_to_csr(src, dst, et, N)
     torch.manual_seed(1)
     H = torch.randn(N, 200, device=G.DEV)
     W = torch.randn(R2, 400, device=G.DEV) * 0.1
