@@ -584,6 +584,18 @@ int renet_decoder_rank(const float* X, const float* W, const float* bias, const 
                        const int32_t* excl_begin, const int32_t* excl_end, float* loss_rows, int32_t* counts, int64_t M, int32_t N,
                        int32_t K, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Several filters in one pass: renet_decoder_rank with n_lists (0, 1 or 2) exclusion lists per row, all indexing one
+ * shared column array.  List j of row m is excl_col[excl_begin[j*M + m] .. excl_end[j*M + m]) (ascending per range).
+ *   counts [M, 2 + 2*n_lists]:  counts[m, 0], counts[m, 1] = renet_decoder_rank's raw pair;
+ *   counts[m, 2 + 2j], counts[m, 3 + 2j] = its filtered pair with list j as the exclusion list.
+ * The sigmoid of each logit is computed once and shared by the lists.  With one list the counts and loss_rows equal
+ * renet_decoder_rank's bit for bit.  Workspace: renet_decoder_rank_workspace_bytes(M, N, K).  Rejected before any launch:
+ * n_lists outside 0..2, a null excl_col, excl_begin or excl_end with n_lists > 0, K % 4 != 0, a workspace too small. */
+int renet_decoder_rank_multi(const float* X, const float* W, const float* bias, const int32_t* label, int32_t n_lists,
+                             const int32_t* excl_col, const int32_t* excl_begin, const int32_t* excl_end, float* loss_rows,
+                             int32_t* counts, int64_t M, int32_t N, int32_t K, void* workspace, int64_t workspace_bytes,
+                             void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Optimiser step of the reference training loop on FLAT fp32 buffers (reference train.py:140-142:
  * torch.nn.utils.clip_grad_norm_(model.parameters(), grad_norm); Adam(lr, weight_decay).step()).  The data-parallel

@@ -82,6 +82,7 @@ SIGNATURES = {
                                  [_i64, _vp]),
     'renet_decoder_rank_workspace_bytes': (_i64, [_i64, _i32, _i32]),
     'renet_decoder_rank': (ctypes.c_int, [_vp] * 9 + [_i64, _i32, _i32, _vp, _i64, _vp]),
+    'renet_decoder_rank_multi': (ctypes.c_int, [_vp] * 4 + [_i32] + [_vp] * 5 + [_i64, _i32, _i32, _vp, _i64, _vp]),
     'renet_grad_sumsq_workspace_bytes': (_i64, []),
     'renet_grad_sumsq': (ctypes.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _vp]),
     'renet_adam_step': (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64] + [ctypes.c_float] * 5 + [_i64, _vp, ctypes.c_float, ctypes.c_float, _vp]),

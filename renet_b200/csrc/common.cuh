@@ -160,6 +160,10 @@ struct EpiArgs {
   const int32_t* excl_begin;
   const int32_t* excl_end;
   int32_t* rank_counts;
+  // rank counting against n_lists (0..2) lists (EPI 7): list j of row `row` is excl_col[excl_begin[j * M + row] ..
+  // excl_end[j * M + row]) (sorted; the lists share excl_col), and rank_counts[(2 + 2 * n_lists) * row + {0, 1}] += EPI 6's
+  // raw pair, rank_counts[(2 + 2 * n_lists) * row + 2 + 2 * j + {0, 1}] += list j's filtered pair
+  int n_lists;
 };
 // p = w * exp(z - lse), rounded the same way wherever the grouped top-k forms it (decoder.cu, umma_gemm.cu)
 __device__ __forceinline__ float topk_prob(float z, float lse, float w) { return __fmul_rn(w, expf(__fsub_rn(z, lse))); }

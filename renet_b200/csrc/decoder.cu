@@ -38,6 +38,9 @@
 //   2. the EPI 6 pass recomputes the logits with the same packed W, bias and tile mapping, so the label's own logit equals
 //      tlogit bit for bit, and counts the logits above / equal to it, and the sigmoids above / equal to the label's with the
 //      row's exclusion list zeroed.  The counts are integers added with integer atomics: the output is reproducible.
+// renet_decoder_rank_multi runs the same two passes with EPI 7 in place of EPI 6: up to two exclusion lists per row (the
+// static and the time-aware filter of evaluate_stream(time_aware=True)), each with its own cursor and filtered pair, the
+// sigmoid of each logit computed once for both.  Its first pass is renet_decoder_rank's, so the loss rows are the same bits.
 #include "common.cuh"
 
 namespace renet {
@@ -535,6 +538,44 @@ int renet_decoder_rank(const float* X, const float* W, const float* bias, const 
   cnt.target = label; cnt.tlogit = w.fwd.tlogit; cnt.excl_col = excl_col; cnt.excl_begin = excl_begin; cnt.excl_end = excl_end;
   cnt.rank_counts = counts;
   rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 6, cnt, 1, 0, stream);
+  if (rc < 0) return rc;
+  return RENET_OK;
+}
+
+int renet_decoder_rank_multi(const float* X, const float* W, const float* bias, const int32_t* label, int32_t n_lists,
+                             const int32_t* excl_col, const int32_t* excl_begin, const int32_t* excl_end, float* loss_rows,
+                             int32_t* counts, int64_t M, int32_t N, int32_t K, void* workspace, int64_t workspace_bytes,
+                             void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  RENET_CHECK_ARG(M >= 0 && N > 0 && K > 0 && K % 4 == 0, "renet_decoder_rank_multi: bad shape (K must be a multiple of 4)");
+  RENET_CHECK_ARG(n_lists >= 0 && n_lists <= 2, "renet_decoder_rank_multi: n_lists = %d outside 0..2", n_lists);
+  RENET_CHECK_ARG(n_lists == 0 || excl_col != nullptr, "renet_decoder_rank_multi: n_lists = %d needs excl_col", n_lists);
+  RENET_CHECK_ARG(n_lists == 0 || (excl_begin != nullptr && excl_end != nullptr),
+                  "renet_decoder_rank_multi: n_lists = %d needs excl_begin and excl_end", n_lists);
+  if (M == 0) return RENET_OK;
+  RENET_CHECK_ARG(X && W && label && loss_rows && counts && workspace, "renet_decoder_rank_multi: null pointer");
+  RENET_CHECK_ARG(workspace_bytes >= renet_decoder_rank_workspace_bytes(M, N, K), "renet_decoder_rank_multi: workspace too small");
+  RENET_CHECK_ARG(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
+                  "renet_decoder_rank_multi: X and W must be 16-byte aligned");
+  void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
+  RankWs w = carve_rank(base, M, N, K);
+  RENET_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)M * (2 + 2 * n_lists) * 4, stream));
+  // 1. lse, loss and the label's logit: the cross-entropy forward epilogue, as in renet_decoder_rank
+  int rc = umma_pack_b(W, 1, K, N, K, w.fwd.Wp, 0, stream);          // logical B[k][n] = W[n*K + k]
+  if (rc) return rc;
+  EpiArgs epi{};
+  epi.target = label; epi.pmax = w.fwd.pmax; epi.psum = w.fwd.psum; epi.tlogit = w.fwd.tlogit;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 1, epi, 1, 0, stream);
+  if (rc < 0) return rc;
+  const int n_part = 2 * ((N + 199) / 200);
+  ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.fwd.pmax, w.fwd.psum, w.fwd.tlogit, n_part, M, w.lse,
+                                                                      loss_rows);
+  RENET_CHECK_LAUNCH("ce_reduce_kernel");
+  // 2. the counts against the label's logit, one filtered pair per list
+  EpiArgs cnt{};
+  cnt.target = label; cnt.tlogit = w.fwd.tlogit; cnt.excl_col = excl_col; cnt.excl_begin = excl_begin; cnt.excl_end = excl_end;
+  cnt.rank_counts = counts; cnt.n_lists = n_lists;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 7, cnt, 1, 0, stream);
   if (rc < 0) return rc;
   return RENET_OK;
 }

@@ -346,6 +346,9 @@ __device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], flo
 //   EPI 6  rank counts (renet_decoder_rank): every logit is compared with the label's logit that the EPI 1 pass wrote to
 //          tlogit (the same tile, the same instructions: the label's own logit compares equal), raw and after the sigmoid
 //          with the row's exclusion list zeroed; each (row, half tile) adds its four counts with integer atomics
+//   EPI 7  rank counts against up to two exclusion lists per row (renet_decoder_rank_multi): EPI 6's raw counts, then per
+//          list its own cursor and its pair of sigmoid counts; the sigmoid of each logit is computed once and shared by the
+//          lists; each (row, half tile) adds its 2 + 2 * n_lists counts with integer atomics
 // grid.x = min(units, SMs).  Batched GEMMs (the two GRU encoders) have per-batch operand offsets.  Split-K (long-K,
 // few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
 // partial product to C + s*split_c; the caller sums the partials.
@@ -511,7 +514,8 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     acc_store(acc, sC, P_CLD, wt);
     named_bar_sync(1 + g, 128);
     if (wt >= 64) continue;
-    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI == 3 || EPI == 4, SEL = EPI == 5, RANK = EPI == 6;
+    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI == 3 || EPI == 4, SEL = EPI == 5, MULTI = EPI == 7;
+    constexpr bool RANK = EPI == 6 || MULTI;
     const int64_t gr = w.row_base + 64 * g + wt;
     const float* srow = sC + wt * P_CLD;
     float run_m = -3.0e38f, run_s = 0.f;               // EPI 1, 3: running max / sum of exp of this (row, half tile)
@@ -527,7 +531,7 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     // entry >= the unit's first column
     const float lab_z = (RANK && gr < M) ? __ldg(epi.tlogit + gr) : 0.f;
     const float lab_p = RANK ? torch_sigmoid(lab_z) : 0.f;
-    const bool filt = RANK && epi.excl_col != nullptr;
+    const bool filt = RANK && !MULTI && epi.excl_col != nullptr;
     int n_gt = 0, n_eq = 0, n_fgt = 0, n_feq = 0;
     int xb = 0, xe = 0;
     if (filt && gr < M) {
@@ -538,6 +542,27 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
         const int mid = (xb + hi) >> 1;
         if (__ldg(epi.excl_col + mid) < first) xb = mid + 1; else hi = mid;
       }
+    }
+    // EPI 7: list j of the row is excl_col[excl_begin[j * M + row] .. excl_end[j * M + row]); each list keeps a cursor, the
+    // column at the cursor in a register (0x7fffffff past the end) and a pair of counts of its own
+    const int n_lists = MULTI ? epi.n_lists : 0;
+    int mxb[2] = {0, 0}, mxe[2] = {0, 0}, m_gt[2] = {0, 0}, m_eq[2] = {0, 0};
+    int m_next[2] = {0x7fffffff, 0x7fffffff};
+    if (MULTI && gr < M) {
+      const int first = n0 + cb;
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (j < n_lists) {
+          int b = __ldg(epi.excl_begin + j * M + gr);
+          const int e = __ldg(epi.excl_end + j * M + gr);
+          for (int hi = e; b < hi;) {
+            const int mid = (b + hi) >> 1;
+            if (__ldg(epi.excl_col + mid) < first) b = mid + 1; else hi = mid;
+          }
+          mxb[j] = b;
+          mxe[j] = e;
+          if (b < e) m_next[j] = __ldg(epi.excl_col + b);
+        }
     }
     const float row_mass = (EPI == 4 && gr < M) ? __ldg(epi.rowmass + gr) : 0.f;
     const float gscale = (!FWD) ? epi.scale * (epi.dscale != nullptr ? __ldg(epi.dscale) : 1.f) : 0.f;
@@ -593,7 +618,19 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
             if (i < nv) {
               n_gt += o[i] > lab_z;
               n_eq += o[i] == lab_z;
-              if (filt) {
+              if (MULTI && n_lists > 0) {
+                const int col = n0 + cc + i;
+                const float p = torch_sigmoid(o[i]);
+#pragma unroll
+                for (int j = 0; j < 2; ++j)
+                  if (j < n_lists) {
+                    while (m_next[j] < col) m_next[j] = ++mxb[j] < mxe[j] ? __ldg(epi.excl_col + mxb[j]) : 0x7fffffff;
+                    const bool zeroed = m_next[j] == col && col != tgt;
+                    const float pj = zeroed ? 0.f : p;
+                    m_gt[j] += pj > lab_p;
+                    m_eq[j] += pj == lab_p;
+                  }
+              } else if (filt) {
                 const int col = n0 + cc + i;
                 while (xb < xe && __ldg(epi.excl_col + xb) < col) ++xb;
                 const bool zeroed = xb < xe && __ldg(epi.excl_col + xb) == col && col != tgt;
@@ -615,12 +652,23 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
         }
       }
     }
-    if (RANK && gr < M) {
+    if (RANK && !MULTI && gr < M) {
       int32_t* rc = epi.rank_counts + 4 * gr;
       if (n_gt) atomicAdd(rc, n_gt);
       if (n_eq) atomicAdd(rc + 1, n_eq);
       if (n_fgt) atomicAdd(rc + 2, n_fgt);
       if (n_feq) atomicAdd(rc + 3, n_feq);
+    }
+    if (MULTI && gr < M) {
+      int32_t* rc = epi.rank_counts + (2 + 2 * n_lists) * gr;
+      if (n_gt) atomicAdd(rc, n_gt);
+      if (n_eq) atomicAdd(rc + 1, n_eq);
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (j < n_lists) {
+          if (m_gt[j]) atomicAdd(rc + 2 + 2 * j, m_gt[j]);
+          if (m_eq[j]) atomicAdd(rc + 3 + 2 * j, m_eq[j]);
+        }
     }
     if (FWD && gr < M) {
       const int64_t pi = (int64_t)(w.nt * 2 + w.half) * M + gr;
@@ -953,6 +1001,7 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(4)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(5)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(6)));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 7>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(7)));
     attr2 = true;
   }
   const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
@@ -969,6 +1018,7 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
   else if (epi_mode == 4) RENET_UMMA_LAUNCH(false, 4);
   else if (epi_mode == 5) RENET_UMMA_LAUNCH(false, 5);
   else if (epi_mode == 6) RENET_UMMA_LAUNCH(false, 6);
+  else if (epi_mode == 7) RENET_UMMA_LAUNCH(false, 7);
   else if (a_index) RENET_UMMA_LAUNCH(true, 0);
   else RENET_UMMA_LAUNCH(false, 0);
 #undef RENET_UMMA_LAUNCH
@@ -1101,7 +1151,7 @@ static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, 
 }
 
 // C[b] (+)= A[b] @ Bpacked[b] (+bias[b]) for b < batch; strides in elements (A, C) / bytes (Bp).
-// epi_mode 1-4: fused cross-entropy epilogues, 5: grouped top-k candidates, 6: rank counts (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
+// epi_mode 1-4: fused cross-entropy epilogues, 5: grouped top-k candidates, 6, 7: rank counts (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,

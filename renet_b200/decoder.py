@@ -11,7 +11,9 @@ the forward pass.  ``nn.Linear`` modules stay the parameter holders (state_dict 
 (renet_decoder_group_topk): per group of R rows, the k largest row_weight * softmax(F.linear(x, weight, bias)) entries.
 
 ``decoder_rank(x, weight, bias, label, exclude)`` is the test-time scoring on the same engine (renet_decoder_rank): per row
-the cross-entropy loss and the label's raw and filtered ranks by the reference's tie rule (model.py:373-379, 403-418)."""
+the cross-entropy loss and the label's raw and filtered ranks by the reference's tie rule (model.py:373-379, 403-418).
+``decoder_rank_counts_multi(x, weight, bias, label, excludes)`` counts against up to two filters in the same pass
+(renet_decoder_rank_multi): the static and the time-aware filter of ``evaluate_stream(time_aware=True)``."""
 import torch
 
 from . import _lib
@@ -169,6 +171,47 @@ def decoder_rank_counts(x, weight, bias, label, exclude=None):
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     _lib.check(L.renet_decoder_rank(P(x), P(weight), P(bias), P(lab), P(col), P(begin), P(end), P(loss_rows), P(counts), M, N, K,
                                     P(ws), nbytes, _lib.stream()), 'renet_decoder_rank')
+    return loss_rows, counts
+
+
+def decoder_rank_counts_multi(x, weight, bias, label, excludes):
+    """renet_decoder_rank_multi: decoder_rank_counts against several filters in one pass.  ``excludes`` is a list of up to
+    two (col, begin, end) exclusion lists as in decoder_rank_counts.  Returns (loss_rows float32 [M], counts int32
+    [M, 2 + 2L]): counts[m, :2] is the raw pair and counts[m, 2 + 2j : 4 + 2j] the filtered pair against list j, each
+    equal to what decoder_rank_counts gives with that list alone."""
+    L, P = _lib.lib(), _lib.ptr
+    _lib.require_cuda(x, weight, label)
+    x, weight = x.contiguous(), weight.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    lab = label.to(torch.int32).contiguous()
+    M, K = x.shape
+    N = weight.shape[0]
+    if lab.numel() != M:
+        raise ValueError('decoder_rank_counts_multi: %d rows but %d labels' % (M, lab.numel()))
+    excludes = list(excludes)
+    n = len(excludes)
+    if n > 2:
+        raise ValueError('decoder_rank_counts_multi: at most two exclusion lists, got %d' % n)
+    col = begin = end = None
+    if n:
+        cols, begins, ends, off = [], [], [], 0
+        for ex in excludes:
+            c, b, e = (t.to(torch.int32).contiguous() for t in ex)
+            _lib.require_cuda(c, b, e)
+            if b.numel() != M or e.numel() != M:
+                raise ValueError('decoder_rank_counts_multi: exclusion ranges need one (begin, end) per row')
+            cols.append(c)
+            begins.append(b + off)                   # into the shared column array
+            ends.append(e + off)
+            off += c.numel()
+        col, begin, end = torch.cat(cols), torch.cat(begins), torch.cat(ends)
+    dev = x.device
+    loss_rows = torch.empty(M, device=dev)
+    counts = torch.empty(M, 2 + 2 * n, dtype=torch.int32, device=dev)
+    nbytes = int(L.renet_decoder_rank_workspace_bytes(M, N, K))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    _lib.check(L.renet_decoder_rank_multi(P(x), P(weight), P(bias), P(lab), n, P(col), P(begin), P(end), P(loss_rows), P(counts),
+                                          M, N, K, P(ws), nbytes, _lib.stream()), 'renet_decoder_rank_multi')
     return loss_rows, counts
 
 

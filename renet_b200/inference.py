@@ -4,6 +4,8 @@
 ``init_history``, ``pred_r_rank2``, ``predict``, ``evaluate``, ``evaluate_filter``, ``update_cache`` -- with the same
 arguments, return values and state attributes (``s_hist_test``, ``s_his_cache``, ``latest_time``, ``graph_dict``,
 ``global_emb`` ...), so the reference's ``test.py`` / validation loop (train.py:151-185) drive it unchanged.
+``evaluate_filter_time`` and ``time_aware=True`` on ``evaluate_stream`` / ``evaluate_stream_batched`` add the time-aware
+filter of the TKG forecasting literature: a query (s, r, ?, t) loses only the answers true at t.
 
 Per-triple scoring runs history batching -> fused RGCN layers -> fused read-out + GRU through
 ``RGCNAggregator.encode`` (the same CUDA path as training); ranks use the reference's tie rule
@@ -63,6 +65,38 @@ def stream_metrics(ranks, total_loss):
     return out
 
 
+#: the protocols evaluate_stream(time_aware=True) reports: raw (model.py:365-381), filtered by every answer known at any
+#: time (model.py:384-419), and time-aware filtered by the answers known at the query's own timestamp only
+PROTOCOLS = ('raw', 'filtered', 'time_filtered')
+
+
+def _quadruples(total_data):
+    """total_data as the time-aware filter needs it: known quadruples (s, r, o, t)."""
+    if total_data is None:
+        raise ValueError('time-aware evaluation needs total_data (all known quadruples)')
+    q = torch.as_tensor(total_data)
+    if q.dim() != 2 or q.shape[1] < 4:
+        raise ValueError('time-aware evaluation needs total_data with a time column (s, r, o, t)')
+    return q
+
+
+def _same_time(all_triplets, triplet):
+    """The rows of all_triplets at triplet's timestamp (column 3)."""
+    allt = torch.as_tensor(all_triplets)
+    return allt[allt[:, 3] == int(triplet[3])]
+
+
+def _exclusion_lists(index, direction, *key):
+    """(col, begin, end) of per-row exclusion lists from a FilterIndex / TimeFilterIndex: row i's list is the answers of
+    key i ((fixed, r) or (fixed, r, t)) in direction 'subjects' where direction[i], else 'objects'; col holds both
+    directions' columns."""
+    b_ob, e_ob = index.ranges('objects', *key)
+    b_sb, e_sb = index.ranges('subjects', *key)
+    off = len(index.col('objects'))
+    col = np.concatenate((index.col('objects'), index.col('subjects')))
+    return col, np.where(direction, b_sb + off, b_ob), np.where(direction, e_sb + off, e_ob)
+
+
 class FilterIndex:
     """The known answers of every (subject, relation) and (object, relation) pair of a set of triples, built once: what
     evaluate_filter (model.py:384-419) finds by scanning all triples for every test triple.  For direction ``objects``
@@ -82,6 +116,53 @@ class FilterIndex:
         keys, _ = self.dirs[direction]
         k = np.asarray(fixed, dtype=np.int64) * self.R + np.asarray(r, dtype=np.int64)
         k = np.where((np.asarray(r) >= 0) & (np.asarray(r) < self.R), k, -1)
+        return np.searchsorted(keys, k, 'left'), np.searchsorted(keys, k, 'right')
+
+    def col(self, direction):
+        return self.dirs[direction][1]
+
+
+class TimeFilterIndex:
+    """FilterIndex keyed by (fixed entity, relation, timestamp), built once from quadruples: the answers the time-aware
+    filter removes for a query (s, r, ?, t) or (?, r, o, t) -- those true at the query's own timestamp t only.  The same
+    interface as FilterIndex, with the timestamp as one more key: ``ranges(direction, fixed, r, t)`` and
+    ``col(direction)``.  Timestamps are replaced by their position among the distinct timestamps of the data, so the
+    composite key (fixed * R + r) * T + position stays far inside int64 (1 M entities x 500 relations x T < 2^63 for any T up
+    to 1.8e10)."""
+
+    def __init__(self, quads):
+        q = np.asarray(torch.as_tensor(quads).cpu().numpy(), dtype=np.int64)
+        if q.ndim != 2 or q.shape[1] < 4:
+            raise ValueError('TimeFilterIndex needs quadruples (s, r, o, t)')
+        self.E = int(max(q[:, 0].max(), q[:, 2].max())) + 1 if len(q) else 1
+        self.R = int(q[:, 1].max()) + 1 if len(q) else 1
+        self.times = np.unique(q[:, 3])
+        self.T = max(len(self.times), 1)
+        if self.E * self.R * self.T >= 1 << 63:
+            raise ValueError('TimeFilterIndex: %d entities x %d relations x %d timestamps overflow int64 keys'
+                             % (self.E, self.R, self.T))
+        pos = np.searchsorted(self.times, q[:, 3])
+        self.dirs = {}
+        for name, fix, ans in (('objects', 0, 2), ('subjects', 2, 0)):
+            key = (q[:, fix] * self.R + q[:, 1]) * self.T + pos
+            order = np.lexsort((q[:, ans], key))
+            k, a = key[order], q[order, ans]
+            keep = np.ones(len(k), dtype=bool)
+            keep[1:] = (k[1:] != k[:-1]) | (a[1:] != a[:-1])           # distinct (key, answer) pairs
+            self.dirs[name] = (k[keep], np.ascontiguousarray(a[keep], dtype=np.int32))
+
+    def ranges(self, direction, fixed, r, t):
+        """(begin, end) int64 arrays: the answers of query i are col(direction)[begin[i]:end[i]]; keys that are absent or
+        out of range (entity, relation or timestamp) give empty ranges."""
+        keys, _ = self.dirs[direction]
+        fixed, r, t = (np.asarray(a, dtype=np.int64) for a in (fixed, r, t))
+        fixed, r, t = np.broadcast_arrays(fixed, r, t)
+        if len(self.times) == 0:
+            z = np.zeros(fixed.shape, dtype=np.int64)
+            return z, z
+        pos = np.minimum(np.searchsorted(self.times, t), len(self.times) - 1)
+        ok = (fixed >= 0) & (fixed < self.E) & (r >= 0) & (r < self.R) & (self.times[pos] == t)
+        k = np.where(ok, (np.where(ok, fixed, 0) * self.R + np.where(ok, r, 0)) * self.T + pos, -1)
         return np.searchsorted(keys, k, 'left'), np.searchsorted(keys, k, 'right')
 
     def col(self, direction):
@@ -398,29 +479,70 @@ class RENetInference:
             ranks.append(rank_with_ties(pred, label))
         return np.array(ranks), loss
 
-    def evaluate_stream(self, test_data, s_history, o_history, global_model, total_data=None, raw=False):
+    def evaluate_filter_time(self, triplet, s_hist, o_hist, global_model, all_triplets):
+        """evaluate_filter with the time-aware filter: only the answers known at the triple's own timestamp -- the rows of
+        ``all_triplets`` whose column 3 equals triplet[3] -- are zeroed after the sigmoid.  Answers true at other times
+        stay ranked, as a forecaster should rank them.  One predict call, as evaluate_filter."""
+        loss, sub_pred, ob_pred = self.predict(triplet, s_hist, o_hist, global_model)
+        return self._filtered_ranks(triplet, sub_pred, ob_pred, _same_time(all_triplets, triplet)), loss
+
+    def _filtered_ranks(self, triplet, sub_pred, ob_pred, known):
+        """evaluate_filter's ranking step (model.py:403-418) against the known triples ``known``: [subject, object] ranks."""
+        s, r, o = int(triplet[0]), int(triplet[1]), int(triplet[2])
+        sub_pred, ob_pred = torch.sigmoid(sub_pred), torch.sigmoid(ob_pred)
+        allt = torch.as_tensor(known).to(ob_pred.device)
+        ranks = []
+        for pred, label, col_fix, col_out, fix in ((sub_pred, s, 2, 0, o), (ob_pred, o, 0, 2, s)):
+            ground = pred[label].clone()
+            ans = allt[(allt[:, col_fix] == fix) & (allt[:, 1] == r)][:, col_out].long()
+            pred = pred.clone()
+            pred[ans] = 0
+            pred[label] = ground
+            ranks.append(rank_with_ties(pred, label))
+        return np.array(ranks)
+
+    def evaluate_stream(self, test_data, s_history, o_history, global_model, total_data=None, raw=False, time_aware=False):
         """The reference's test loop (test.py:98-150) as a method: trims the per-entity histories to ``seq_len``
         (test.py:100-106), ranks every test triple in stream order (``evaluate`` when ``raw`` else ``evaluate_filter``
         against ``total_data``), and returns MRR / MR / Hits@{1,3,10} over subject and object ranks together, the summed
-        loss and the ranks.  ``s_history`` / ``o_history`` = (lists, timestamp lists) of the test split."""
+        loss and the ranks.  ``s_history`` / ``o_history`` = (lists, timestamp lists) of the test split.
+
+        ``time_aware=True`` (``total_data`` = quadruples) scores each triple with one predict call and ranks its scores
+        under all three protocols -- raw, filtered and time-aware filtered (evaluate_filter_time) -- returned as
+        result['protocols'] = {'raw', 'filtered', 'time_filtered'}, each a dict like the result; the top-level keys stay
+        the protocol ``raw`` selects.  (Calling evaluate, evaluate_filter and evaluate_filter_time in turn would run three
+        predicts per triple, and the first triple after a roll-over is scored differently by the later ones.)"""
         self._trim_test_histories()
         test_data = torch.as_tensor(test_data)
+        if time_aware:
+            total_data = _quadruples(total_data)
         if not raw:
             if total_data is None:
                 raise ValueError('filtered evaluation needs total_data (all known triples)')
+        if not raw or time_aware:
             total_data = torch.as_tensor(total_data).to(self.ent_embeds.device)
         ranks, total_loss = [], 0.0
+        protocols = {k: [] for k in PROTOCOLS}
         with torch.no_grad():
             for i in range(len(test_data)):
                 trip = test_data[i].to(self.ent_embeds.device)
                 sh, oh = (s_history[0][i], s_history[1][i]), (o_history[0][i], o_history[1][i])
-                if raw:
+                if time_aware:
+                    loss, sub_pred, ob_pred = self.predict(trip, sh, oh, global_model)
+                    protocols['raw'].append(np.array([rank_with_ties(sub_pred, int(trip[0])), rank_with_ties(ob_pred, int(trip[2]))]))
+                    protocols['filtered'].append(self._filtered_ranks(trip, sub_pred, ob_pred, total_data))
+                    protocols['time_filtered'].append(self._filtered_ranks(trip, sub_pred, ob_pred, _same_time(total_data, trip)))
+                    r = protocols['raw' if raw else 'filtered'][-1]
+                elif raw:
                     r, loss = self.evaluate(trip, sh, oh, global_model)
                 else:
                     r, loss = self.evaluate_filter(trip, sh, oh, global_model, total_data)
                 ranks.append(r)
                 total_loss += float(loss)
-        return stream_metrics(ranks, total_loss)
+        out = stream_metrics(ranks, total_loss)
+        if time_aware:
+            out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
+        return out
 
     def _trim_test_histories(self):
         """test.py:100-106: keep the last seq_len entries of every per-entity test-time history."""
@@ -431,7 +553,8 @@ class RENetInference:
                     hist_t[ee].pop(0)
 
     # ---- batched evaluation -------------------------------------------------------------------------------------------
-    def evaluate_stream_batched(self, test_data, s_history, o_history, global_model, total_data=None, raw=False):
+    def evaluate_stream_batched(self, test_data, s_history, o_history, global_model, total_data=None, raw=False,
+                                time_aware=False):
         """evaluate_stream, one timestamp at a time: same arguments, same result dict, same state afterwards (histories,
         caches, graph_dict, global_emb, latest_time, torch's RNG stream).  All triples of a timestamp are scored against the
         same state -- predict changes it only at the first triple of a new timestamp, through the roll-over -- so for each
@@ -439,14 +562,21 @@ class RENetInference:
         encoded in one batched pass (one isolation group per entity, so each history is encoded as if alone) and every
         triple is scored and ranked by one renet_decoder_rank call.  The known answers come from a FilterIndex built once
         from ``total_data``.  A model on the host has no kernels: it encodes each query through _encode_one and ranks the
-        materialised logits with torch, with the same grouping, rebinding and filter index."""
+        materialised logits with torch, with the same grouping, rebinding and filter index.
+
+        ``time_aware=True``: each run is ranked by one renet_decoder_rank_multi call against two lists per row, the static
+        filter and the time-aware one (a TimeFilterIndex built once from the quadruples ``total_data``), and the result
+        gets result['protocols'] as evaluate_stream(time_aware=True) returns it."""
         self._trim_test_histories()
         test_data = torch.as_tensor(test_data)
-        fidx = None
-        if not raw:
+        fidx = tfidx = None
+        if time_aware:
+            tfidx = TimeFilterIndex(_quadruples(total_data))
+        if not raw or time_aware:
             if total_data is None:
                 raise ValueError('filtered evaluation needs total_data (all known triples)')
             fidx = FilterIndex(total_data)
+        protocols = {k: [] for k in PROTOCOLS}
         quads = test_data.cpu().numpy().astype(np.int64)
         s_empty = np.asarray([len(x) == 0 for x in s_history[0]], dtype=bool)
         o_empty = np.asarray([len(x) == 0 for x in o_history[0]], dtype=bool)
@@ -463,16 +593,25 @@ class RENetInference:
                     last_s, last_o = self._roll_over(t, global_model)
                     if self.reference_rebinding:
                         rebind = (last_s, last_o)
-                r, loss = self._score_run(quads[i0:i1], s_empty[i0:i1], o_empty[i0:i1], rebind, fidx)
+                r, loss = self._score_run(quads[i0:i1], s_empty[i0:i1], o_empty[i0:i1], rebind, fidx, tfidx)
+                if time_aware:
+                    for k in PROTOCOLS:
+                        protocols[k].append(r[k])
+                    r = r['raw' if raw else 'filtered']
                 ranks.append(r)
                 total_loss += float(np.sum(loss.astype(np.float64)))
                 i0 = i1
-        return stream_metrics(ranks, total_loss)
+        out = stream_metrics(ranks, total_loss)
+        if time_aware:
+            out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
+        return out
 
-    def _score_run(self, quads, s_empty, o_empty, rebind, fidx):
+    def _score_run(self, quads, s_empty, o_empty, rebind, fidx, tfidx=None):
         """Scores the triples of one timestamp against the current state: (ranks float64 [2n] as [sub, ob] per triple,
         loss float32 [n] = predict's two cross-entropies per triple).  rebind = (s, o) of the roll-over that the run's first
-        triple is scored with (model.py:279,290) or None; its rank labels and filter keys stay its own."""
+        triple is scored with (model.py:279,290) or None; its rank labels and filter keys stay its own.  With a
+        TimeFilterIndex ``tfidx`` (and ``fidx``) the ranks are a dict of the three PROTOCOLS, the time-aware keys taking the
+        run's timestamp."""
         R, h = self.num_rels, self.h_dim
         dev = self.ent_embeds.device
         n = len(quads)
@@ -495,22 +634,22 @@ class RENetInference:
             x = torch.cat((x, x[[0, n]]), dim=0)
             rank_lab = np.concatenate((rank_lab, [oi[0], si[0]]))
             loss_row[0], loss_row[n] = 2 * n, 2 * n + 1
-        exclude = None
+        exclude = t_exclude = None
         if fidx is not None:
             m = len(rank_lab)
             fix = np.concatenate((s, o, [s[0], o[0]]))[:m]
             rr = np.concatenate((r, r, [r[0], r[0]]))[:m]
             direction = np.concatenate((np.zeros(n, bool), np.ones(n, bool), [False, True]))[:m]
-            b_ob, e_ob = fidx.ranges('objects', fix, rr)
-            b_sb, e_sb = fidx.ranges('subjects', fix, rr)
-            off = len(fidx.col('objects'))
-            col = np.concatenate((fidx.col('objects'), fidx.col('subjects')))
-            begin = np.where(direction, b_sb + off, b_ob)
-            end = np.where(direction, e_sb + off, e_ob)
-            exclude = (col, begin, end)
-        loss_rows, raw_rank, filt_rank = self._rank_rows(x, rank_lab, exclude)
-        rk = (filt_rank if exclude is not None else raw_rank).cpu().numpy()
-        ranks = np.stack((rk[n:2 * n], rk[:n]), axis=1).reshape(-1)
+            exclude = _exclusion_lists(fidx, direction, fix, rr)
+            if tfidx is not None:
+                t_exclude = _exclusion_lists(tfidx, direction, fix, rr, np.full(m, quads[0, 3]))
+        pair = lambda rk: np.stack((rk[n:2 * n], rk[:n]), axis=1).reshape(-1)    # noqa: E731
+        if tfidx is None:
+            loss_rows, raw_rank, filt_rank = self._rank_rows(x, rank_lab, exclude)
+            ranks = pair((filt_rank if exclude is not None else raw_rank).cpu().numpy())
+        else:
+            loss_rows, rks = self._rank_rows_multi(x, rank_lab, [exclude, t_exclude])
+            ranks = {k: pair(rk.cpu().numpy()) for k, rk in zip(PROTOCOLS, rks)}
         lr = loss_rows.cpu().numpy().astype(np.float32)
         return ranks, lr[loss_row[:n]] + lr[loss_row[n:]]
 
@@ -530,6 +669,23 @@ class RENetInference:
         c = rank_counts_torch(z, lab, exclude)
         filt = ranks_from_counts(c[:, 2], c[:, 3]) if exclude is not None else None
         return loss_rows, ranks_from_counts(c[:, 0], c[:, 1]), filt
+
+    def _rank_rows_multi(self, x, label, excludes):
+        """(loss_rows, [raw ranks, then the filtered ranks against each list of ``excludes``]) of the rows of x against
+        ``linear``: one renet_decoder_rank_multi call on the GPU; on the host, as _rank_rows, counted with torch once per
+        list."""
+        from .decoder import decoder_rank_counts_multi, ranks_from_counts
+        dev = x.device
+        lab = torch.from_numpy(np.ascontiguousarray(label, dtype=np.int64)).to(dev)
+        if x.is_cuda:
+            ex = [tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev) for a in e) for e in excludes]
+            loss_rows, c = decoder_rank_counts_multi(x, self.linear.weight, self.linear.bias, lab, ex)
+        else:
+            z = torch.stack([self.linear(row) for row in x])
+            loss_rows = torch.stack([self.criterion(z[m].view(1, -1), lab[m].view(1)) for m in range(len(lab))])
+            cs = [rank_counts_torch(z, lab, e) for e in excludes]
+            c = torch.cat([rank_counts_torch(z, lab)[:, :2]] + [ci[:, 2:] for ci in cs], dim=1)
+        return loss_rows, [ranks_from_counts(c[:, 2 * j], c[:, 2 * j + 1]) for j in range(len(excludes) + 1)]
 
     def _encode_queries(self, ents, rels, has, subject):
         """s_h [n, h] of the queries (ents[i], rels[i]) against the current test-time histories; rows where ``has`` is
