@@ -374,6 +374,8 @@ int renet_decoder_ce_bwd(const float* X, const float* W, const float* bias, cons
   if (M == 0) return RENET_OK;
   RENET_CHECK_ARG(X && W && target && lse && dX && dW && workspace, "renet_decoder_ce_bwd: null pointer");
   RENET_CHECK_ARG(workspace_bytes >= renet_decoder_ce_bwd_workspace_bytes(M, N, K), "renet_decoder_ce_bwd: workspace too small");
+  RENET_CHECK_ARG(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
+                  "renet_decoder_ce_bwd: X and W must be 16-byte aligned");
   void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
   DecBwdWs w = carve_bwd(base, M, N, K);
   int rc;

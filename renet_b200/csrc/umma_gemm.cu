@@ -302,7 +302,10 @@ struct GemmStamps {
 };
 
 // EPI 0 straight from a warpgroup's m64n104 fragment: thread wt holds rows r0, r0 + 8 of the 64 rows at row_base and, per
-// 8-column group i, columns 8i + c0, +1 of the 104 at tile column cb; the 4 threads of a quad cover 32 contiguous bytes
+// 8-column group i, columns 8i + c0, +1 of the 104 at tile column cb; the 4 threads of a quad cover 32 contiguous bytes.
+// tile_n is even (N % 4 == 0 for every caller), so each column pair is wholly inside or wholly past the tile; the pairs
+// past it are skipped one by one: the decoder's gradient products have N = its K, where K % 8 == 4 ends the tile
+// half-way through an 8-column group, and a store there would land on the next row's first columns.
 __device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], float* __restrict__ Cz, int64_t ldc,
                                                const float* __restrict__ bz, int64_t row_base, int64_t M, int n0, int cb,
                                                int tile_n, int accumulate, int wt) {
@@ -314,7 +317,7 @@ __device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], flo
 #pragma unroll
     for (int i = 0; i < P_UN / 8; ++i) {
       const int cc = cb + 8 * i;
-      if (cc >= tile_n) continue;
+      if (cc + c0 >= tile_n) continue;
       float o0 = acc[4 * i + 2 * h], o1 = acc[4 * i + 2 * h + 1];
       float* cp = Cz + gr * ldc + n0 + cc + c0;
       if (bz != nullptr) {

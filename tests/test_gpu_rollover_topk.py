@@ -61,7 +61,12 @@ SHAPES = [(3, 1, 1000, 64, 10),            # R = 1
           (3, 2, 150, 24, 20),             # R * n_part = 4 < k: the threshold is 0, every entry is a candidate
           (2, 256, 23033, 600, 1),         # ICEWS18: R = 256 relations, |E| = 23 033, K = 3h
           (2, 256, 23033, 600, 10),
-          (2, 256, 23033, 600, 1000)]
+          (2, 256, 23033, 600, 1000),
+          (3, 240, 7691, 600, 1000),       # GDELT: groups of 240 rows cross the 128-row tiles and the CTAs
+          (40, 3, 1001, 200, 50),          # many groups inside one row tile
+          (2, 64, 2000, 64, 1500),         # k above 1024 and not a power of two: several pairs per thread per sort stage
+          (2, 16, 2000, 200, 4096),
+          (1, 16, 1024, 64, 16384)]        # k = R * N = RENET_TOPK_MAX_K
 
 
 @pytest.mark.parametrize('G,R,N,K,k', SHAPES)
@@ -92,7 +97,7 @@ def test_group_topk_vs_fp64(G, R, N, K, k):
     _check_layout(v2, i2, ORDER_VALUE)
 
 
-@pytest.mark.parametrize('G,R,N,K,k', [SHAPES[1], SHAPES[5]])
+@pytest.mark.parametrize('G,R,N,K,k', [SHAPES[1], SHAPES[5], SHAPES[6], SHAPES[8]])
 def test_group_topk_capacity_retry(G, R, N, K, k):
     """A candidate buffer too small for a group is reported, never truncated; the wrapper repeats the call with the size
     reported and returns what a large enough buffer gives."""
