@@ -577,7 +577,8 @@ int renet_decoder_group_topk(const float* X, const float* W, const float* bias, 
  * The reference's rank is counts[gt] + (counts[eq] - 1) / 2 + 1.  3xTF32 wgmma GEMM in two passes (logsumexp and the
  * label's logit, then the counts); the logits never reach memory, the label's logit is the same bits in both passes.  No
  * float atomics; the output is bitwise reproducible.  K % 4 == 0; X [M,K], W [N,K] row-major, 16-byte aligned; bias [N]
- * may be NULL; counts int32 [M,4].
+ * may be NULL; counts int32 [M,4].  This is the one-list (excl_col != NULL) or no-list case of renet_decoder_rank_multi
+ * below, with the counts always laid out [M,4].
  * ---------------------------------------------------------------------------------------------- */
 int64_t renet_decoder_rank_workspace_bytes(int64_t M, int32_t N, int32_t K);
 int renet_decoder_rank(const float* X, const float* W, const float* bias, const int32_t* label, const int32_t* excl_col,

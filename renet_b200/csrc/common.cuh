@@ -152,18 +152,17 @@ struct EpiArgs {
   float* sel_val;          // [G, sel_cap]
   int32_t* sel_idx;        // [G, sel_cap]
   int sel_R, sel_cap;
-  // rank counting (EPI 6): every logit of row `row` is compared with tlogit[row] (the label's logit from the EPI 1 pass)
-  // and rank_counts[4 * row + {0, 1, 2, 3}] += {#greater, #equal, #filtered greater, #filtered equal} (integer atomics).
-  // Filtered: sigmoid, with the columns of excl_col[excl_begin[row] .. excl_end[row]) (sorted) other than target[row]
-  // set to 0; excl_col == nullptr skips the filtered counts.
+  // rank counting (EPI 6): every logit of row `row` is compared with tlogit[row] (the label's logit from the EPI 1 pass),
+  // and rank_counts[rank_ld * row + {0, 1}] += {#greater, #equal} (integer atomics).  Per exclusion list j < n_lists (0..2):
+  // the sigmoid, with the columns of excl_col[excl_begin[j * M + row] .. excl_end[j * M + row]) (sorted; the lists share
+  // excl_col) other than target[row] set to 0, is compared with the label's, and rank_counts[rank_ld * row + 2 + 2 * j +
+  // {0, 1}] += {#greater, #equal}.  rank_ld >= 2 + 2 * n_lists; the columns past the lists' are not written.
   const int32_t* excl_col;
   const int32_t* excl_begin;
   const int32_t* excl_end;
   int32_t* rank_counts;
-  // rank counting against n_lists (0..2) lists (EPI 7): list j of row `row` is excl_col[excl_begin[j * M + row] ..
-  // excl_end[j * M + row]) (sorted; the lists share excl_col), and rank_counts[(2 + 2 * n_lists) * row + {0, 1}] += EPI 6's
-  // raw pair, rank_counts[(2 + 2 * n_lists) * row + 2 + 2 * j + {0, 1}] += list j's filtered pair
   int n_lists;
+  int rank_ld;
 };
 // p = w * exp(z - lse), rounded the same way wherever the grouped top-k forms it (decoder.cu, umma_gemm.cu)
 __device__ __forceinline__ float topk_prob(float z, float lse, float w) { return __fmul_rn(w, expf(__fsub_rn(z, lse))); }

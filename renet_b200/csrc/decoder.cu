@@ -31,16 +31,17 @@
 //      the lower index, and bitonic-sorts the k winners into the output order in shared memory.
 // Every step is either a fixed-order computation or an integer count, so the output is bitwise reproducible.
 //
-// Rank counts (renet_decoder_rank; test-time scoring, reference model.py:365-419): per row, the label's rank among the row's
-// logits, raw and filtered, by the tie rule #greater + (#equal - 1) / 2 + 1, without writing the [M, N] logits:
+// Rank counts (test-time scoring, reference model.py:365-419): per row, the label's rank among the row's logits, raw and
+// filtered against each of 0-2 exclusion lists (the static and the time-aware filter of evaluate_stream(time_aware=True)),
+// by the tie rule #greater + (#equal - 1) / 2 + 1, without writing the [M, N] logits.  One rank pass (rank_counts below):
 //   1. the EPI 1 pass with the label as target gives the partials and the label's logit tlogit; ce_reduce_kernel turns
 //      them into lse and loss_rows;
 //   2. the EPI 6 pass recomputes the logits with the same packed W, bias and tile mapping, so the label's own logit equals
-//      tlogit bit for bit, and counts the logits above / equal to it, and the sigmoids above / equal to the label's with the
-//      row's exclusion list zeroed.  The counts are integers added with integer atomics: the output is reproducible.
-// renet_decoder_rank_multi runs the same two passes with EPI 7 in place of EPI 6: up to two exclusion lists per row (the
-// static and the time-aware filter of evaluate_stream(time_aware=True)), each with its own cursor and filtered pair, the
-// sigmoid of each logit computed once for both.  Its first pass is renet_decoder_rank's, so the loss rows are the same bits.
+//      tlogit bit for bit, and counts the logits above / equal to it and, per list, the sigmoids above / equal to the
+//      label's with that list zeroed (the sigmoid of each logit computed once for all lists).  The counts are integers
+//      added with integer atomics: the output is reproducible.
+// Two entry points run it: renet_decoder_rank with at most one list and rows of 4 counts, renet_decoder_rank_multi with
+// 0-2 lists and rows of 2 + 2 * n_lists.
 #include "common.cuh"
 
 namespace renet {
@@ -332,6 +333,34 @@ RankWs carve_rank(void* base, int64_t M, int N, int K) {
   return w;
 }
 
+// The rank pass of both rank entry points, after their argument checks: loss_rows, and counts [M, rank_ld] zeroed, then
+// the raw pair and one filtered pair per list added (the columns past 2 + 2 * n_lists stay 0)
+int rank_counts(const float* X, const float* W, const float* bias, const int32_t* label, int n_lists, const int32_t* excl_col,
+                const int32_t* excl_begin, const int32_t* excl_end, float* loss_rows, int32_t* counts, int rank_ld, int64_t M,
+                int N, int K, void* workspace, cudaStream_t stream) {
+  void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
+  RankWs w = carve_rank(base, M, N, K);
+  RENET_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)M * rank_ld * 4, stream));
+  // 1. lse, loss and the label's logit: the cross-entropy forward epilogue
+  int rc = umma_pack_b(W, 1, K, N, K, w.fwd.Wp, 0, stream);          // logical B[k][n] = W[n*K + k]
+  if (rc) return rc;
+  EpiArgs epi{};
+  epi.target = label; epi.pmax = w.fwd.pmax; epi.psum = w.fwd.psum; epi.tlogit = w.fwd.tlogit;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 1, epi, 1, 0, stream);
+  if (rc < 0) return rc;
+  const int n_part = 2 * ((N + 199) / 200);
+  ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.fwd.pmax, w.fwd.psum, w.fwd.tlogit, n_part, M, w.lse,
+                                                                      loss_rows);
+  RENET_CHECK_LAUNCH("ce_reduce_kernel");
+  // 2. the counts against the label's logit, one filtered pair per list
+  EpiArgs cnt{};
+  cnt.target = label; cnt.tlogit = w.fwd.tlogit; cnt.excl_col = excl_col; cnt.excl_begin = excl_begin; cnt.excl_end = excl_end;
+  cnt.rank_counts = counts; cnt.n_lists = n_lists; cnt.rank_ld = rank_ld;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 6, cnt, 1, 0, stream);
+  if (rc < 0) return rc;
+  return RENET_OK;
+}
+
 }  // namespace
 }  // namespace renet
 
@@ -521,27 +550,9 @@ int renet_decoder_rank(const float* X, const float* W, const float* bias, const 
   RENET_CHECK_ARG(workspace_bytes >= renet_decoder_rank_workspace_bytes(M, N, K), "renet_decoder_rank: workspace too small");
   RENET_CHECK_ARG(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
                   "renet_decoder_rank: X and W must be 16-byte aligned");
-  void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
-  RankWs w = carve_rank(base, M, N, K);
-  RENET_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)M * 16, stream));
-  // 1. lse, loss and the label's logit: the cross-entropy forward epilogue
-  int rc = umma_pack_b(W, 1, K, N, K, w.fwd.Wp, 0, stream);          // logical B[k][n] = W[n*K + k]
-  if (rc) return rc;
-  EpiArgs epi{};
-  epi.target = label; epi.pmax = w.fwd.pmax; epi.psum = w.fwd.psum; epi.tlogit = w.fwd.tlogit;
-  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 1, epi, 1, 0, stream);
-  if (rc < 0) return rc;
-  const int n_part = 2 * ((N + 199) / 200);
-  ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.fwd.pmax, w.fwd.psum, w.fwd.tlogit, n_part, M, w.lse,
-                                                                      loss_rows);
-  RENET_CHECK_LAUNCH("ce_reduce_kernel");
-  // 2. the counts against the label's logit
-  EpiArgs cnt{};
-  cnt.target = label; cnt.tlogit = w.fwd.tlogit; cnt.excl_col = excl_col; cnt.excl_begin = excl_begin; cnt.excl_end = excl_end;
-  cnt.rank_counts = counts;
-  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 6, cnt, 1, 0, stream);
-  if (rc < 0) return rc;
-  return RENET_OK;
+  // always 4 counts per row: without a list the filtered pair stays 0
+  return rank_counts(X, W, bias, label, excl_col != nullptr ? 1 : 0, excl_col, excl_begin, excl_end, loss_rows, counts, 4, M, N,
+                     K, workspace, stream);
 }
 
 int renet_decoder_rank_multi(const float* X, const float* W, const float* bias, const int32_t* label, int32_t n_lists,
@@ -559,27 +570,8 @@ int renet_decoder_rank_multi(const float* X, const float* W, const float* bias, 
   RENET_CHECK_ARG(workspace_bytes >= renet_decoder_rank_workspace_bytes(M, N, K), "renet_decoder_rank_multi: workspace too small");
   RENET_CHECK_ARG(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
                   "renet_decoder_rank_multi: X and W must be 16-byte aligned");
-  void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
-  RankWs w = carve_rank(base, M, N, K);
-  RENET_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)M * (2 + 2 * n_lists) * 4, stream));
-  // 1. lse, loss and the label's logit: the cross-entropy forward epilogue, as in renet_decoder_rank
-  int rc = umma_pack_b(W, 1, K, N, K, w.fwd.Wp, 0, stream);          // logical B[k][n] = W[n*K + k]
-  if (rc) return rc;
-  EpiArgs epi{};
-  epi.target = label; epi.pmax = w.fwd.pmax; epi.psum = w.fwd.psum; epi.tlogit = w.fwd.tlogit;
-  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 1, epi, 1, 0, stream);
-  if (rc < 0) return rc;
-  const int n_part = 2 * ((N + 199) / 200);
-  ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.fwd.pmax, w.fwd.psum, w.fwd.tlogit, n_part, M, w.lse,
-                                                                      loss_rows);
-  RENET_CHECK_LAUNCH("ce_reduce_kernel");
-  // 2. the counts against the label's logit, one filtered pair per list
-  EpiArgs cnt{};
-  cnt.target = label; cnt.tlogit = w.fwd.tlogit; cnt.excl_col = excl_col; cnt.excl_begin = excl_begin; cnt.excl_end = excl_end;
-  cnt.rank_counts = counts; cnt.n_lists = n_lists;
-  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.fwd.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 7, cnt, 1, 0, stream);
-  if (rc < 0) return rc;
-  return RENET_OK;
+  return rank_counts(X, W, bias, label, n_lists, excl_col, excl_begin, excl_end, loss_rows, counts, 2 + 2 * n_lists, M, N, K,
+                     workspace, stream);
 }
 
 }  // extern "C"

@@ -346,12 +346,11 @@ __device__ __forceinline__ void store_fragment(const float (&acc)[P_UN / 2], flo
 //   EPI 5  grouped top-k candidates (renet_decoder_group_topk): p = row_w[row] * exp(logit - lse[row]); every p at or above
 //          its group's threshold is appended to the group's candidate buffer (an integer atomic picks the slot; the final
 //          select sorts, so no output depends on the slot order)
-//   EPI 6  rank counts (renet_decoder_rank): every logit is compared with the label's logit that the EPI 1 pass wrote to
-//          tlogit (the same tile, the same instructions: the label's own logit compares equal), raw and after the sigmoid
-//          with the row's exclusion list zeroed; each (row, half tile) adds its four counts with integer atomics
-//   EPI 7  rank counts against up to two exclusion lists per row (renet_decoder_rank_multi): EPI 6's raw counts, then per
-//          list its own cursor and its pair of sigmoid counts; the sigmoid of each logit is computed once and shared by the
-//          lists; each (row, half tile) adds its 2 + 2 * n_lists counts with integer atomics
+//   EPI 6  rank counts (renet_decoder_rank, renet_decoder_rank_multi): every logit is compared with the label's logit that
+//          the EPI 1 pass wrote to tlogit (the same tile, the same instructions: the label's own logit compares equal), raw
+//          and, per exclusion list of the row (0..2), after the sigmoid with the list zeroed; each list has its own cursor,
+//          the sigmoid of each logit is computed once and shared by the lists, and each (row, half tile) adds its
+//          2 + 2 * n_lists counts with integer atomics
 // grid.x = min(units, SMs).  Batched GEMMs (the two GRU encoders) have per-batch operand offsets.  Split-K (long-K,
 // few-tile products such as dX = dlogits @ W of the decoder): split s owns the chunks [s*cps, (s+1)*cps) and writes its
 // partial product to C + s*split_c; the caller sums the partials.
@@ -517,8 +516,7 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     acc_store(acc, sC, P_CLD, wt);
     named_bar_sync(1 + g, 128);
     if (wt >= 64) continue;
-    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI == 3 || EPI == 4, SEL = EPI == 5, MULTI = EPI == 7;
-    constexpr bool RANK = EPI == 6 || MULTI;
+    constexpr bool FWD = EPI == 1 || EPI == 3, SOFT = EPI == 3 || EPI == 4, SEL = EPI == 5, RANK = EPI == 6;
     const int64_t gr = w.row_base + 64 * g + wt;
     const float* srow = sC + wt * P_CLD;
     float run_m = -3.0e38f, run_s = 0.f;               // EPI 1, 3: running max / sum of exp of this (row, half tile)
@@ -530,28 +528,16 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
     const float row_w = (SEL && gr < M) ? __ldg(epi.row_w + gr) : 0.f;
     const float sel_tau = (SEL && gr < M) ? __ldg(epi.tau + sel_g) : 0.f;
     const float row_lse = (!FWD && !RANK && gr < M) ? __ldg(epi.lse + gr) : 0.f;
-    // EPI 6: the label's logit and sigmoid, the four counts, and the cursor into the row's exclusion list at the first
-    // entry >= the unit's first column
+    // EPI 6: the label's logit and sigmoid and the raw pair of counts.  List j of the row is excl_col[excl_begin[j * M + row]
+    // .. excl_end[j * M + row]); each list keeps a cursor (first placed at the first entry >= the unit's first column), the
+    // column at the cursor in a register (0x7fffffff past the end) and a pair of counts of its own
     const float lab_z = (RANK && gr < M) ? __ldg(epi.tlogit + gr) : 0.f;
     const float lab_p = RANK ? torch_sigmoid(lab_z) : 0.f;
-    const bool filt = RANK && !MULTI && epi.excl_col != nullptr;
-    int n_gt = 0, n_eq = 0, n_fgt = 0, n_feq = 0;
-    int xb = 0, xe = 0;
-    if (filt && gr < M) {
-      xb = __ldg(epi.excl_begin + gr);
-      xe = __ldg(epi.excl_end + gr);
-      const int first = n0 + cb;
-      for (int hi = xe; xb < hi;) {
-        const int mid = (xb + hi) >> 1;
-        if (__ldg(epi.excl_col + mid) < first) xb = mid + 1; else hi = mid;
-      }
-    }
-    // EPI 7: list j of the row is excl_col[excl_begin[j * M + row] .. excl_end[j * M + row]); each list keeps a cursor, the
-    // column at the cursor in a register (0x7fffffff past the end) and a pair of counts of its own
-    const int n_lists = MULTI ? epi.n_lists : 0;
-    int mxb[2] = {0, 0}, mxe[2] = {0, 0}, m_gt[2] = {0, 0}, m_eq[2] = {0, 0};
-    int m_next[2] = {0x7fffffff, 0x7fffffff};
-    if (MULTI && gr < M) {
+    int n_gt = 0, n_eq = 0;
+    const int n_lists = RANK ? epi.n_lists : 0;
+    int xb[2] = {0, 0}, xe[2] = {0, 0}, f_gt[2] = {0, 0}, f_eq[2] = {0, 0};
+    int x_next[2] = {0x7fffffff, 0x7fffffff};
+    if (RANK && gr < M) {
       const int first = n0 + cb;
 #pragma unroll
       for (int j = 0; j < 2; ++j)
@@ -562,9 +548,9 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
             const int mid = (b + hi) >> 1;
             if (__ldg(epi.excl_col + mid) < first) b = mid + 1; else hi = mid;
           }
-          mxb[j] = b;
-          mxe[j] = e;
-          if (b < e) m_next[j] = __ldg(epi.excl_col + b);
+          xb[j] = b;
+          xe[j] = e;
+          if (b < e) x_next[j] = __ldg(epi.excl_col + b);
         }
     }
     const float row_mass = (EPI == 4 && gr < M) ? __ldg(epi.rowmass + gr) : 0.f;
@@ -621,25 +607,18 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
             if (i < nv) {
               n_gt += o[i] > lab_z;
               n_eq += o[i] == lab_z;
-              if (MULTI && n_lists > 0) {
+              if (n_lists > 0) {
                 const int col = n0 + cc + i;
                 const float p = torch_sigmoid(o[i]);
 #pragma unroll
                 for (int j = 0; j < 2; ++j)
                   if (j < n_lists) {
-                    while (m_next[j] < col) m_next[j] = ++mxb[j] < mxe[j] ? __ldg(epi.excl_col + mxb[j]) : 0x7fffffff;
-                    const bool zeroed = m_next[j] == col && col != tgt;
+                    while (x_next[j] < col) x_next[j] = ++xb[j] < xe[j] ? __ldg(epi.excl_col + xb[j]) : 0x7fffffff;
+                    const bool zeroed = x_next[j] == col && col != tgt;
                     const float pj = zeroed ? 0.f : p;
-                    m_gt[j] += pj > lab_p;
-                    m_eq[j] += pj == lab_p;
+                    f_gt[j] += pj > lab_p;
+                    f_eq[j] += pj == lab_p;
                   }
-              } else if (filt) {
-                const int col = n0 + cc + i;
-                while (xb < xe && __ldg(epi.excl_col + xb) < col) ++xb;
-                const bool zeroed = xb < xe && __ldg(epi.excl_col + xb) == col && col != tgt;
-                const float p = zeroed ? 0.f : torch_sigmoid(o[i]);
-                n_fgt += p > lab_p;
-                n_feq += p == lab_p;
               }
             }
         } else {
@@ -655,22 +634,15 @@ umma_gemm_packed_kernel(const float* __restrict__ A, const int32_t* __restrict__
         }
       }
     }
-    if (RANK && !MULTI && gr < M) {
-      int32_t* rc = epi.rank_counts + 4 * gr;
-      if (n_gt) atomicAdd(rc, n_gt);
-      if (n_eq) atomicAdd(rc + 1, n_eq);
-      if (n_fgt) atomicAdd(rc + 2, n_fgt);
-      if (n_feq) atomicAdd(rc + 3, n_feq);
-    }
-    if (MULTI && gr < M) {
-      int32_t* rc = epi.rank_counts + (2 + 2 * n_lists) * gr;
+    if (RANK && gr < M) {
+      int32_t* rc = epi.rank_counts + epi.rank_ld * gr;
       if (n_gt) atomicAdd(rc, n_gt);
       if (n_eq) atomicAdd(rc + 1, n_eq);
 #pragma unroll
       for (int j = 0; j < 2; ++j)
         if (j < n_lists) {
-          if (m_gt[j]) atomicAdd(rc + 2 + 2 * j, m_gt[j]);
-          if (m_eq[j]) atomicAdd(rc + 3 + 2 * j, m_eq[j]);
+          if (f_gt[j]) atomicAdd(rc + 2 + 2 * j, f_gt[j]);
+          if (f_eq[j]) atomicAdd(rc + 3 + 2 * j, f_eq[j]);
         }
     }
     if (FWD && gr < M) {
@@ -1004,7 +976,6 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(4)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(5)));
     RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(6)));
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(umma_gemm_packed_kernel<false, 7>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem(7)));
     attr2 = true;
   }
   const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
@@ -1021,7 +992,6 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
   else if (epi_mode == 4) RENET_UMMA_LAUNCH(false, 4);
   else if (epi_mode == 5) RENET_UMMA_LAUNCH(false, 5);
   else if (epi_mode == 6) RENET_UMMA_LAUNCH(false, 6);
-  else if (epi_mode == 7) RENET_UMMA_LAUNCH(false, 7);
   else if (a_index) RENET_UMMA_LAUNCH(true, 0);
   else RENET_UMMA_LAUNCH(false, 0);
 #undef RENET_UMMA_LAUNCH
@@ -1154,7 +1124,7 @@ static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, 
 }
 
 // C[b] (+)= A[b] @ Bpacked[b] (+bias[b]) for b < batch; strides in elements (A, C) / bytes (Bp).
-// epi_mode 1-4: fused cross-entropy epilogues, 5: grouped top-k candidates, 6, 7: rank counts (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
+// epi_mode 1-4: fused cross-entropy epilogues, 5: grouped top-k candidates, 6: rank counts (EpiArgs); k_splits > 1: split-K partial products at C + s*split_c.
 int umma_gemm_prepacked_ex(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, bool accumulate, int batch, int64_t batch_a,
                            int64_t batch_bp, int64_t batch_c, int epi_mode, const EpiArgs& epi, int k_splits, int64_t split_c,

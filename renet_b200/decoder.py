@@ -144,26 +144,43 @@ def decoder_group_topk(x, weight, bias, row_weight, R, k, order=ORDER_INDEX, cap
         cap = need
 
 
+def _rank_operands(name, x, weight, bias, label, excludes):
+    """The operands of a rank call, as its C entry takes them: (x, weight, bias, int32 labels, col, begin, end) with the
+    exclusion lists ``excludes`` (up to two (col, begin, end)) in one column array, begin / end [len(excludes) * M] indexing
+    it (col, begin, end are None without a list).  ValueErrors name the caller ``name``."""
+    _lib.require_cuda(x, weight, label)
+    x, weight = x.contiguous(), weight.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    lab = label.to(torch.int32).contiguous()
+    M = x.shape[0]
+    if lab.numel() != M:
+        raise ValueError('%s: %d rows but %d labels' % (name, M, lab.numel()))
+    if len(excludes) > 2:
+        raise ValueError('%s: at most two exclusion lists, got %d' % (name, len(excludes)))
+    lists, off = [], 0
+    for ex in excludes:
+        c, b, e = (t.to(torch.int32).contiguous() for t in ex)
+        _lib.require_cuda(c, b, e)
+        if b.numel() != M or e.numel() != M:
+            raise ValueError('%s: exclusion ranges need one (begin, end) per row' % name)
+        lists.append((c, b + off, e + off) if off else (c, b, e))      # into the shared column array
+        off += c.numel()
+    if len(lists) == 2:
+        lists = [tuple(torch.cat(t) for t in zip(*lists))]
+    col, begin, end = lists[0] if lists else (None, None, None)
+    return x, weight, bias, lab, col, begin, end
+
+
 def decoder_rank_counts(x, weight, bias, label, exclude=None):
     """renet_decoder_rank: for z = x @ weight^T + bias and the labels ``label`` [M], returns (loss_rows float32 [M],
     counts int32 [M, 4]) with counts[m] = (#z > z_l, #z == z_l, #p > p_l, #p == p_l) where p = torch.sigmoid(z) with the
     columns of row m's exclusion list other than its label set to 0.  ``exclude`` = (col, begin, end): int32 device
     tensors, row m's list being col[begin[m]:end[m]] in ascending order; None leaves the last two counts 0."""
     L, P = _lib.lib(), _lib.ptr
-    _lib.require_cuda(x, weight, label)
-    x, weight = x.contiguous(), weight.contiguous()
-    bias = bias.contiguous() if bias is not None else None
-    lab = label.to(torch.int32).contiguous()
+    x, weight, bias, lab, col, begin, end = _rank_operands('decoder_rank', x, weight, bias, label,
+                                                           [] if exclude is None else [exclude])
     M, K = x.shape
     N = weight.shape[0]
-    if lab.numel() != M:
-        raise ValueError('decoder_rank: %d rows but %d labels' % (M, lab.numel()))
-    col = begin = end = None
-    if exclude is not None:
-        col, begin, end = (t.to(torch.int32).contiguous() for t in exclude)
-        _lib.require_cuda(col, begin, end)
-        if begin.numel() != M or end.numel() != M:
-            raise ValueError('decoder_rank: exclusion ranges need one (begin, end) per row')
     dev = x.device
     loss_rows = torch.empty(M, device=dev)
     counts = torch.empty(M, 4, dtype=torch.int32, device=dev)
@@ -180,31 +197,11 @@ def decoder_rank_counts_multi(x, weight, bias, label, excludes):
     [M, 2 + 2L]): counts[m, :2] is the raw pair and counts[m, 2 + 2j : 4 + 2j] the filtered pair against list j, each
     equal to what decoder_rank_counts gives with that list alone."""
     L, P = _lib.lib(), _lib.ptr
-    _lib.require_cuda(x, weight, label)
-    x, weight = x.contiguous(), weight.contiguous()
-    bias = bias.contiguous() if bias is not None else None
-    lab = label.to(torch.int32).contiguous()
-    M, K = x.shape
-    N = weight.shape[0]
-    if lab.numel() != M:
-        raise ValueError('decoder_rank_counts_multi: %d rows but %d labels' % (M, lab.numel()))
     excludes = list(excludes)
     n = len(excludes)
-    if n > 2:
-        raise ValueError('decoder_rank_counts_multi: at most two exclusion lists, got %d' % n)
-    col = begin = end = None
-    if n:
-        cols, begins, ends, off = [], [], [], 0
-        for ex in excludes:
-            c, b, e = (t.to(torch.int32).contiguous() for t in ex)
-            _lib.require_cuda(c, b, e)
-            if b.numel() != M or e.numel() != M:
-                raise ValueError('decoder_rank_counts_multi: exclusion ranges need one (begin, end) per row')
-            cols.append(c)
-            begins.append(b + off)                   # into the shared column array
-            ends.append(e + off)
-            off += c.numel()
-        col, begin, end = torch.cat(cols), torch.cat(begins), torch.cat(ends)
+    x, weight, bias, lab, col, begin, end = _rank_operands('decoder_rank_counts_multi', x, weight, bias, label, excludes)
+    M, K = x.shape
+    N = weight.shape[0]
     dev = x.device
     loss_rows = torch.empty(M, device=dev)
     counts = torch.empty(M, 2 + 2 * n, dtype=torch.int32, device=dev)

@@ -465,19 +465,8 @@ class RENetInference:
     def evaluate_filter(self, triplet, s_hist, o_hist, global_model, all_triplets):
         """model.py:384-419: filtered ranks -- other known true answers of (s, r, ?) / (?, r, o) are zeroed after the
         sigmoid before ranking."""
-        s, r, o = int(triplet[0]), int(triplet[1]), int(triplet[2])
         loss, sub_pred, ob_pred = self.predict(triplet, s_hist, o_hist, global_model)
-        sub_pred, ob_pred = torch.sigmoid(sub_pred), torch.sigmoid(ob_pred)
-        allt = torch.as_tensor(all_triplets).to(ob_pred.device)
-        ranks = []
-        for pred, label, col_fix, col_out, fix in ((sub_pred, s, 2, 0, o), (ob_pred, o, 0, 2, s)):
-            ground = pred[label].clone()
-            known = allt[(allt[:, col_fix] == fix) & (allt[:, 1] == r)][:, col_out].long()
-            pred = pred.clone()
-            pred[known] = 0
-            pred[label] = ground
-            ranks.append(rank_with_ties(pred, label))
-        return np.array(ranks), loss
+        return self._filtered_ranks(triplet, sub_pred, ob_pred, all_triplets), loss
 
     def evaluate_filter_time(self, triplet, s_hist, o_hist, global_model, all_triplets):
         """evaluate_filter with the time-aware filter: only the answers known at the triple's own timestamp -- the rows of
@@ -560,13 +549,14 @@ class RENetInference:
         same state -- predict changes it only at the first triple of a new timestamp, through the roll-over -- so for each
         maximal run of equal timestamps the roll-over runs once, as predict runs it, and then every query of the run is
         encoded in one batched pass (one isolation group per entity, so each history is encoded as if alone) and every
-        triple is scored and ranked by one renet_decoder_rank call.  The known answers come from a FilterIndex built once
-        from ``total_data``.  A model on the host has no kernels: it encodes each query through _encode_one and ranks the
-        materialised logits with torch, with the same grouping, rebinding and filter index.
+        triple is scored and ranked by one renet_decoder_rank_multi call, with no exclusion list (``raw``) or one per row
+        whose known answers come from a FilterIndex built once from ``total_data``.  A model on the host has no kernels: it
+        encodes each query through _encode_one and ranks the materialised logits with torch, with the same grouping,
+        rebinding and filter index.
 
-        ``time_aware=True``: each run is ranked by one renet_decoder_rank_multi call against two lists per row, the static
-        filter and the time-aware one (a TimeFilterIndex built once from the quadruples ``total_data``), and the result
-        gets result['protocols'] as evaluate_stream(time_aware=True) returns it."""
+        ``time_aware=True``: the call takes two lists per row, the static filter and the time-aware one (a TimeFilterIndex
+        built once from the quadruples ``total_data``), and the result gets result['protocols'] as
+        evaluate_stream(time_aware=True) returns it."""
         self._trim_test_histories()
         test_data = torch.as_tensor(test_data)
         fidx = tfidx = None
@@ -634,46 +624,28 @@ class RENetInference:
             x = torch.cat((x, x[[0, n]]), dim=0)
             rank_lab = np.concatenate((rank_lab, [oi[0], si[0]]))
             loss_row[0], loss_row[n] = 2 * n, 2 * n + 1
-        exclude = t_exclude = None
+        excludes = []                                            # the static filter, then the time-aware one
         if fidx is not None:
             m = len(rank_lab)
             fix = np.concatenate((s, o, [s[0], o[0]]))[:m]
             rr = np.concatenate((r, r, [r[0], r[0]]))[:m]
             direction = np.concatenate((np.zeros(n, bool), np.ones(n, bool), [False, True]))[:m]
-            exclude = _exclusion_lists(fidx, direction, fix, rr)
+            excludes.append(_exclusion_lists(fidx, direction, fix, rr))
             if tfidx is not None:
-                t_exclude = _exclusion_lists(tfidx, direction, fix, rr, np.full(m, quads[0, 3]))
+                excludes.append(_exclusion_lists(tfidx, direction, fix, rr, np.full(m, quads[0, 3])))
+        loss_rows, rks = self._rank_rows(x, rank_lab, excludes)
         pair = lambda rk: np.stack((rk[n:2 * n], rk[:n]), axis=1).reshape(-1)    # noqa: E731
         if tfidx is None:
-            loss_rows, raw_rank, filt_rank = self._rank_rows(x, rank_lab, exclude)
-            ranks = pair((filt_rank if exclude is not None else raw_rank).cpu().numpy())
+            ranks = pair(rks[-1].cpu().numpy())                  # filtered with a filter index, else raw
         else:
-            loss_rows, rks = self._rank_rows_multi(x, rank_lab, [exclude, t_exclude])
             ranks = {k: pair(rk.cpu().numpy()) for k, rk in zip(PROTOCOLS, rks)}
         lr = loss_rows.cpu().numpy().astype(np.float32)
         return ranks, lr[loss_row[:n]] + lr[loss_row[n:]]
 
-    def _rank_rows(self, x, label, exclude):
-        """(loss_rows, raw ranks, filtered ranks or None) of the rows of x against ``linear``: renet_decoder_rank on the
-        GPU; on the host, row by row through ``linear`` as predict computes them, counted with torch."""
-        from .decoder import decoder_rank, ranks_from_counts
-        dev = x.device
-        lab = torch.from_numpy(np.ascontiguousarray(label, dtype=np.int64)).to(dev)
-        if x.is_cuda:
-            ex = None
-            if exclude is not None:
-                ex = tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev) for a in exclude)
-            return decoder_rank(x, self.linear.weight, self.linear.bias, lab, ex)
-        z = torch.stack([self.linear(row) for row in x])
-        loss_rows = torch.stack([self.criterion(z[m].view(1, -1), lab[m].view(1)) for m in range(len(lab))])
-        c = rank_counts_torch(z, lab, exclude)
-        filt = ranks_from_counts(c[:, 2], c[:, 3]) if exclude is not None else None
-        return loss_rows, ranks_from_counts(c[:, 0], c[:, 1]), filt
-
-    def _rank_rows_multi(self, x, label, excludes):
-        """(loss_rows, [raw ranks, then the filtered ranks against each list of ``excludes``]) of the rows of x against
-        ``linear``: one renet_decoder_rank_multi call on the GPU; on the host, as _rank_rows, counted with torch once per
-        list."""
+    def _rank_rows(self, x, label, excludes):
+        """(loss_rows, [raw ranks, then the filtered ranks against each of the 0-2 exclusion lists ``excludes``]) of the
+        rows of x against ``linear``: one renet_decoder_rank_multi call on the GPU; on the host, row by row through
+        ``linear`` as predict computes them, counted with torch once per list."""
         from .decoder import decoder_rank_counts_multi, ranks_from_counts
         dev = x.device
         lab = torch.from_numpy(np.ascontiguousarray(label, dtype=np.int64)).to(dev)

@@ -1,7 +1,6 @@
 """not gpu: the time-aware filter (evaluate_stream(time_aware=True), renet_b200/inference.py) -- the TimeFilterIndex against
 brute-force masks, an oracle anchored on the reference's own scores, the host flow against that oracle and against the
-per-triple path, the counting epilogue's SASS, and renet_decoder_rank_multi's argument checks."""
-import re
+per-triple path, and renet_decoder_rank_multi's argument checks (the counting epilogue's SASS: test_rank_decoder_sass.py)."""
 import threading
 
 import numpy as np
@@ -9,7 +8,6 @@ import pytest
 import torch
 
 from helpers import load_npz, rel_err
-from test_deterministic_sass import FLOAT_ATOMIC, _matching, sass  # noqa: F401  (sass is a fixture)
 from test_eval_batched_host import _assert_same_state, _ctx, _state
 
 
@@ -191,13 +189,6 @@ def test_time_aware_needs_quadruples():
 
 
 # ---- the kernel, without a GPU ----------------------------------------------------------------------------------------------
-def test_rank_multi_epilogue_has_integer_atomics_only(sass):  # noqa: F811
-    for name, body in _matching(sass, r'umma_gemm_packed_kernel<\(bool\)0, \(int\)7>').items():
-        hits = [ln.strip() for ln in body.split('\n') if FLOAT_ATOMIC.search(ln)]
-        assert not hits, '%s: %s' % (name, hits[:3])
-        assert re.search(r'\b(RED|REDG|ATOM|ATOMG)\.E\.ADD', body), name
-
-
 def test_decoder_rank_multi_rejects_bad_arguments():
     """Every case returns -1 with its message before anything is launched (the fake addresses are never dereferenced).  The
     library's last-error string is per thread: the calls run on a thread of their own and leave this one's empty."""

@@ -10,7 +10,7 @@ rolls over once.
       first test timestamp (no roll-over), in ms per triple;
   (b) new: evaluate_stream_batched over the whole test split, filtered: ms per timestamp in all, the roll-over per
       roll-over, and per timestamp the rest, batching + encode (_encode_queries, both directions) and the rank call
-      (_rank_rows: renet_decoder_rank with its inputs' uploads); each part ends in a device synchronise;
+      (_rank_rows: renet_decoder_rank_multi with its inputs' uploads); each part ends in a device synchronise;
   (c) the rank kernel alone (renet_decoder_rank) on one timestamp's rows, timed with CUDA events: logical GEMM TFLOP/s of its
       two passes = 2 x 2 * rows * |E| * 3h over the call's time.
 (a) and (b) alternate --reps times; every (b) starts from a fresh copy of the state.  The model has seeded parameters (h =

@@ -11,8 +11,9 @@ TimeFilterIndex of the whole stream):
       from a fresh copy of the state: ms per timestamp without the roll-over (host clock after a device synchronise);
   (c) building the TimeFilterIndex (and, for scale, the FilterIndex) from an ICEWS18-sized stream of about 470 k
       quadruples, host clock.
---compare-tree DIR: the static call of (a) alone, in alternating processes importing renet_b200 from this tree and from DIR
-(another checkout with its library built), --ab-rounds times each.  --static-only: one such process (used by the above)."""
+--compare-tree DIR: renet_decoder_rank alone, with the static list of (a) and with no list, in alternating processes
+importing renet_b200 from this tree and from DIR (another checkout with its library built), --ab-rounds times each.
+--static-only: one such process (used by the above)."""
 import argparse
 import json
 import os
@@ -107,14 +108,20 @@ def gpu_info():
 
 
 def static_only(datasets, rounds, calls):
+    """{'<dataset>/static' and '<dataset>/no_list': ms per call per round} of renet_decoder_rank in the two forms it serves,
+    the static filter's list and no list, alternated round by round."""
     out = {}
     with torch.no_grad():
         for ds in datasets:
             k = kernel_inputs(ds)
-            fn = lambda: decoder_rank_counts(k['x'], k['w'], k['b'], k['lab'], k['ex'][0])   # noqa: E731
-            for _ in range(3):
-                fn()
-            out[ds] = [round(time_calls(fn, calls), 4) for _ in range(rounds)]
+            forms = {form: (lambda ex=ex: decoder_rank_counts(k['x'], k['w'], k['b'], k['lab'], ex))
+                     for form, ex in (('static', k['ex'][0]), ('no_list', None))}
+            for fn in forms.values():
+                for _ in range(3):
+                    fn()
+            for _ in range(rounds):
+                for form, fn in forms.items():
+                    out.setdefault('%s/%s' % (ds, form), []).append(round(time_calls(fn, calls), 4))
     return out
 
 
@@ -198,15 +205,15 @@ def main():
         res[ds] = {'kernel': kernel_ab(ds, A.rounds, A.calls), 'stream': stream_ab(ds, A.num_k, A.stream_reps)}
     res['index_build'] = index_build()
     if A.compare_tree:
-        ab = {'this': {d: [] for d in datasets}, 'other': {d: [] for d in datasets}}
+        ab = {'this': {}, 'other': {}}
         for _ in range(A.ab_rounds):
             for arm, tree in (('this', A.tree), ('other', A.compare_tree)):
                 cmd = [sys.executable, os.path.abspath(__file__), '--static-only', '--tree', tree, '--datasets', A.datasets,
                        '--rounds', str(A.rounds), '--calls', str(A.calls)]
                 got = json.loads(subprocess.run(cmd, capture_output=True, text=True, check=True).stdout.strip().split('\n')[-1])
-                for d in datasets:
-                    ab[arm][d].extend(got[d])
-        res['static_call_ms_this_vs_other_tree'] = ab
+                for key, times in got.items():
+                    ab[arm].setdefault(key, []).extend(times)
+        res['rank_call_ms_this_vs_other_tree'] = ab
     print(json.dumps(res))
 
 
