@@ -312,92 +312,142 @@ class RENetInference:
         on a CUDA tensor of R * in_dim values (ORDER_INDEX: the values above the k-th one in index order, then those equal
         to it; measured on an H100 with PyTorch 2.11 from R * in_dim = 9 600 to 5.9 M), since the roll-over's final
         selection and the order of its cache updates depend on that layout."""
-        from .decoder import ORDER_INDEX, decoder_group_topk
-        R, h, N = self.num_rels, self.h_dim, self.in_dim
-        dev = self.ent_embeds.device
-        ents = torch.as_tensor(entities).reshape(-1).long().cpu().numpy()
-        wts = torch.as_tensor(weights).reshape(-1).to(device=dev, dtype=torch.float32)
+        ents, wts = self._topk_operands(entities, weights)
         n = len(ents)
-        if wts.numel() != n:
-            raise ValueError('pred_r_topk: %d entities but %d weights' % (n, wts.numel()))
+        dev = self.ent_embeds.device
         values = torch.empty(n, k, device=dev)
         codes = torch.empty(n, k, dtype=torch.long, device=dev)
-        rel_embeds, reverse = self._direction(subject)
-        hist = self.s_hist_test if subject else self.o_hist_test
-        per = max(1, ROLLOVER_SEQ_BUDGET // R)
-        rel_rows = torch.arange(R, device=dev)
-        for c0 in range(0, n, per):
-            ce = ents[c0:c0 + per]
-            nc = len(ce)
-            s_h = torch.zeros(nc, R, h, device=dev)
-            s_q = torch.zeros(nc, h, device=dev)
-            has = np.flatnonzero([len(hist[e]) != 0 for e in ce])
-            if len(has):
-                he = ce[has]
-                # The batched history graph has one component per timestamp, induced by the nodes of every sample in
-                # the batch (utils.py:158-181), so an entity's encoding depends on what it is batched with.  One isolation
-                # group per entity gives every entity components of its own, to encode exactly what pred_r_rank2 encodes
-                # alone.
-                view, gs = self._grouped_view(he, np.repeat(np.arange(len(he)), R), subject)
-                s_dev = torch.from_numpy(np.repeat(he, R)).to(dev)
-                r_dev = rel_rows.repeat(len(he))
-                sh, sq, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, self.global_emb,
-                                                    reverse, self.encoder, self.encoder_r)
-                # the encoder returns the sequences length-sorted: row j is sample sample_order[j] of the view
-                idx = hb.sample_order(dev)
-                sh_v, sq_v = torch.empty_like(sh), torch.empty_like(sq)
-                sh_v[idx], sq_v[idx] = sh, sq
-                has_dev = torch.from_numpy(has).to(dev)
-                s_h[has_dev] = sh_v.view(len(he), R, h)
-                s_q[has_dev] = sq_v.view(len(he), R, h)[:, 0]                 # s_q does not depend on r (model.py:96)
-            ent = self.ent_embeds[torch.from_numpy(ce).to(dev)]
-            p_r = torch.softmax(self.linear_r(torch.cat((ent, s_q), dim=1)), dim=1)                    # [nc, R]
-            row_w = (wts[c0:c0 + nc].view(-1, 1) * p_r).reshape(-1)
-            x = torch.cat((ent.repeat_interleave(R, dim=0), s_h.view(nc * R, h), rel_embeds.repeat(nc, 1)), dim=1)
-            v, i = decoder_group_topk(x, self.linear.weight, self.linear.bias, row_w, R, k, ORDER_INDEX, capacity)
-            values[c0:c0 + nc] = v
-            codes[c0:c0 + nc] = i
+        for c0, c1 in self._topk_chunks(n):
+            values[c0:c1], codes[c0:c1] = self._topk_chunk(ents[c0:c1], wts[c0:c1], k, subject, capacity)
         return values, codes
 
-    def _pick_candidates(self, picks, prob, subject):
-        """The num_k most probable (relation, entity) continuations of every pick (model.py:236-240): host tensors
-        (joint probabilities [n_picks, num_k], codes r * in_dim + o [n_picks, num_k]) in picks order.  On the GPU every
-        distinct entity is scored once, all of them in one batched pass (pred_r_topk: its scores depend on the entity
-        only), and its list is repeated for each pick of it.  A model on the host has no kernels to run (the host-logic
-        checks substitute a host encoder): its picks are scored one by one through pred_r_rank2, as the reference does."""
-        K, R = self.num_k, self.num_rels
-        if self.ent_embeds.is_cuda:
-            uniq, inverse = torch.unique(picks, return_inverse=True)
-            top_p, top_i = self.pred_r_topk(uniq, prob[uniq], K, subject=subject)
-            inverse = inverse.cpu()
-            return top_p.cpu()[inverse], top_i.cpu()[inverse]
-        lists, inds = [], []
-        for e, p_e in zip(picks, prob[picks]):
-            ee = torch.full((R,), int(e), dtype=torch.long)
-            joint = float(p_e) * self.pred_r_rank2(ee, torch.arange(R), subject=subject)
-            top_p, top_i = torch.topk(joint.view(-1), K, sorted=False)
-            lists.append(top_p.view(-1).cpu())
-            inds.append(top_i.view(-1).cpu())
-        return torch.stack(lists), torch.stack(inds)
+    def _topk_operands(self, entities, weights):
+        """pred_r_topk's entities as a host int64 array and its weights as float32 on the model's device."""
+        ents = torch.as_tensor(entities).reshape(-1).long().cpu().numpy()
+        wts = torch.as_tensor(weights).reshape(-1).to(device=self.ent_embeds.device, dtype=torch.float32)
+        if wts.numel() != len(ents):
+            raise ValueError('pred_r_topk: %d entities but %d weights' % (len(ents), wts.numel()))
+        return ents, wts
 
-    def _roll_over(self, t, global_model):
+    def _topk_chunks(self, n):
+        """[c0, c1) of pred_r_topk's chunks of n entities: ROLLOVER_SEQ_BUDGET // R entities each."""
+        per = max(1, ROLLOVER_SEQ_BUDGET // self.num_rels)
+        return [(c0, min(c0 + per, n)) for c0 in range(0, n, per)]
+
+    def _topk_chunk(self, ce, wc, k, subject, capacity=None):
+        """pred_r_topk of one chunk: host entities ``ce`` with device weights ``wc``, encoded and scored in one pass."""
+        from .decoder import ORDER_INDEX, decoder_group_topk
+        R, h = self.num_rels, self.h_dim
+        dev = self.ent_embeds.device
+        rel_embeds, reverse = self._direction(subject)
+        hist = self.s_hist_test if subject else self.o_hist_test
+        rel_rows = torch.arange(R, device=dev)
+        nc = len(ce)
+        s_h = torch.zeros(nc, R, h, device=dev)
+        s_q = torch.zeros(nc, h, device=dev)
+        has = np.flatnonzero([len(hist[e]) != 0 for e in ce])
+        if len(has):
+            he = ce[has]
+            # The batched history graph has one component per timestamp, induced by the nodes of every sample in
+            # the batch (utils.py:158-181), so an entity's encoding depends on what it is batched with.  One isolation
+            # group per entity gives every entity components of its own, to encode exactly what pred_r_rank2 encodes
+            # alone.
+            view, gs = self._grouped_view(he, np.repeat(np.arange(len(he)), R), subject)
+            s_dev = torch.from_numpy(np.repeat(he, R)).to(dev)
+            r_dev = rel_rows.repeat(len(he))
+            sh, sq, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, self.global_emb,
+                                                reverse, self.encoder, self.encoder_r)
+            # the encoder returns the sequences length-sorted: row j is sample sample_order[j] of the view
+            idx = hb.sample_order(dev)
+            sh_v, sq_v = torch.empty_like(sh), torch.empty_like(sq)
+            sh_v[idx], sq_v[idx] = sh, sq
+            has_dev = torch.from_numpy(has).to(dev)
+            s_h[has_dev] = sh_v.view(len(he), R, h)
+            s_q[has_dev] = sq_v.view(len(he), R, h)[:, 0]                 # s_q does not depend on r (model.py:96)
+        ent = self.ent_embeds[torch.from_numpy(ce).to(dev)]
+        p_r = torch.softmax(self.linear_r(torch.cat((ent, s_q), dim=1)), dim=1)                    # [nc, R]
+        row_w = (wc.view(-1, 1) * p_r).reshape(-1)
+        x = torch.cat((ent.repeat_interleave(R, dim=0), s_h.view(nc * R, h), rel_embeds.repeat(nc, 1)), dim=1)
+        return decoder_group_topk(x, self.linear.weight, self.linear.bias, row_w, R, k, ORDER_INDEX, capacity)
+
+    def _pick_candidates(self, draws, shard=None):
+        """The num_k most probable (relation, entity) continuations of every pick (model.py:236-240), for each direction's
+        draw (picks, prob, subject) of ``draws``: host tensors (joint probabilities [n_picks, num_k], codes r * in_dim + o
+        [n_picks, num_k]) in picks order.  On the GPU every distinct entity of a draw is scored once, in pred_r_topk's
+        chunks (its scores depend on the entity only), and its list is repeated for each pick of it.  A model on the host
+        has no kernels to run (the host-logic checks substitute a host encoder): its picks are scored one by one through
+        pred_r_rank2, as the reference does.
+
+        The units of work -- the chunks of both directions on the GPU, the picks on the host -- are independent, and each
+        gets exactly the operands it gets alone; with a ``shard`` (parallel.Shard) unit j runs on rank j mod world and
+        every rank all-gathers the lists, so every rank returns what one process returns, bit for bit."""
+        K, R = self.num_k, self.num_rels
+        dev = self.ent_embeds.device
+        jobs, done, inverse = [], [], []               # jobs: (draw, first row, end row) per unit, in unit order
+        if self.ent_embeds.is_cuda:
+            work = []
+            for d, (picks, prob, subject) in enumerate(draws):
+                uniq, inv = torch.unique(picks, return_inverse=True)
+                work.append(self._topk_operands(uniq, prob[uniq]))
+                inverse.append(inv.cpu())
+                jobs += [(d, c0, c1) for c0, c1 in self._topk_chunks(len(uniq))]
+            for j in (range(len(jobs)) if shard is None else shard.units(len(jobs))):
+                d, c0, c1 = jobs[j]
+                ents, wts = work[d]
+                done.append(self._topk_chunk(ents[c0:c1], wts[c0:c1], K, draws[d][2]))
+        else:
+            jobs = [(d, i, i + 1) for d, (picks, _, _) in enumerate(draws) for i in range(len(picks))]
+            inverse = [None] * len(draws)
+            p_picks = [prob[picks] for picks, prob, _ in draws]          # each pick's probability
+            for j in (range(len(jobs)) if shard is None else shard.units(len(jobs))):
+                d, i, _ = jobs[j]
+                picks, _, subject = draws[d]
+                ee = torch.full((R,), int(picks[i]), dtype=torch.long)
+                joint = float(p_picks[d][i]) * self.pred_r_rank2(ee, torch.arange(R), subject=subject)
+                top_p, top_i = torch.topk(joint.view(-1), K, sorted=False)
+                done.append((top_p.view(1, -1), top_i.view(1, -1)))
+        vals, codes = [v for v, _ in done], [c for _, c in done]
+        if shard is not None:
+            sizes = [c1 - c0 for _, c0, c1 in jobs]
+            vals = shard.gather_units(vals, sizes, torch.empty(0, K, device=dev))
+            codes = shard.gather_units(codes, sizes, torch.empty(0, K, dtype=torch.long, device=dev))
+        out = []
+        for d in range(len(draws)):
+            js = [j for j, job in enumerate(jobs) if job[0] == d]
+            v, c = torch.cat([vals[j] for j in js]).cpu(), torch.cat([codes[j] for j in js]).cpu()
+            out.append((v, c) if inverse[d] is None else (v[inverse[d]], c[inverse[d]]))
+        return out
+
+    def _roll_over(self, t, global_model, shard=None):
         """model.py:222-330: the stream moved to a new timestamp.  Sample num_k subjects (objects) from the global
         model's distribution, score every (relation, entity) continuation for them, keep the num_k most probable
-        triples, turn them into the predicted graph of `latest_time`, and roll the per-entity histories."""
+        triples, turn them into the predicted graph of `latest_time`, and roll the per-entity histories.
+
+        Both directions are sampled first, subject then object as the reference draws them: the global model reads
+        graph_dict, which changes only after both directions, and the candidate scoring draws no random numbers, so the RNG
+        stream and the global model's calls are the reference's.  Then both directions' candidates are scored together
+        (_pick_candidates, sharded over ``shard`` when given) and the caches are updated in the reference's order."""
         K, R = self.num_k, self.num_rels
-        last = {}
+        draws = []
         for subject in (True, False):
-            cache = self.s_his_cache if subject else self.o_his_cache
-            cache_t = self.s_his_cache_t if subject else self.o_his_cache_t
             if subject:
                 _, _, prob = global_model.predict(self.latest_time, self.graph_dict, subject=True)
             else:
                 _, logits, _ = global_model.predict(t, self.graph_dict, subject=False)
                 prob = torch.softmax(logits.view(-1), dim=0)                               # model.py:262
             picks = torch.distributions.categorical.Categorical(prob).sample(torch.Size([K]))
-            # NOTE: the reference de-duplicates with a set of 0-dim tensors (model.py:228-234), which never matches
-            # (tensors hash by identity), so repeated samples are scored again and kept as separate entries.
-            lists, inds = self._pick_candidates(picks, prob, subject)                     # [K picks, K] in picks order
+            draws.append((picks, prob, subject))
+        if shard is not None:
+            sums = [int((p.cpu().long() * torch.arange(1, len(p) + 1)).sum()) for p, _, _ in draws]
+            if not shard.same_everywhere(sums):
+                raise RuntimeError('evaluate_stream_batched: the ranks of process_group sampled different roll-over picks; '
+                                   'they need the same torch seeds and a deterministic global model')
+        last = {}
+        # NOTE: the reference de-duplicates with a set of 0-dim tensors (model.py:228-234), which never matches (tensors
+        # hash by identity), so repeated samples are scored again and kept as separate entries.
+        for (picks, _, subject), (lists, inds) in zip(draws, self._pick_candidates(draws, shard)):   # [K picks, K] each
+            cache = self.s_his_cache if subject else self.o_his_cache
+            cache_t = self.s_his_cache_t if subject else self.o_his_cache_t
             ents = picks.tolist()
             _, cand = torch.topk(lists.view(-1), K, sorted=False)
             for c in cand.tolist():
@@ -543,7 +593,7 @@ class RENetInference:
 
     # ---- batched evaluation -------------------------------------------------------------------------------------------
     def evaluate_stream_batched(self, test_data, s_history, o_history, global_model, total_data=None, raw=False,
-                                time_aware=False):
+                                time_aware=False, process_group=None):
         """evaluate_stream, one timestamp at a time: same arguments, same result dict, same state afterwards (histories,
         caches, graph_dict, global_emb, latest_time, torch's RNG stream).  All triples of a timestamp are scored against the
         same state -- predict changes it only at the first triple of a new timestamp, through the roll-over -- so for each
@@ -556,9 +606,23 @@ class RENetInference:
 
         ``time_aware=True``: the call takes two lists per row, the static filter and the time-aware one (a TimeFilterIndex
         built once from the quadruples ``total_data``), and the result gets result['protocols'] as
-        evaluate_stream(time_aware=True) returns it."""
-        self._trim_test_histories()
+        evaluate_stream(time_aware=True) returns it.
+
+        ``process_group`` (a torch.distributed group, one process per GPU over NCCL, or gloo for a model on the host): every
+        rank of the group calls with the same arguments, model state and torch seeds, and the work is sharded over the ranks
+        in whole units of the one-process schedule -- the roll-over's candidate chunks (_pick_candidates), the query
+        encoding chunks (_encode_queries) and contiguous row slices of each rank call (_score_run) -- each unit getting the
+        operands it gets in one process.  Every rank then returns the result and ends in the state one process does, bit
+        for bit; the host steps of the roll-over run on every rank.  None, or a group of one, runs unsharded.  Ranks called
+        with different test data, latest_time, num_k or flags raise ValueError; ranks that sample different roll-over picks
+        raise RuntimeError.  A caller outside the group raises ValueError.  A member of the group that never calls is not
+        detected: the callers wait for it in the first all-gather, until the process group's own timeout (a collective
+        cannot tell a late rank from an absent one)."""
+        shard = self._eval_shard(process_group)
         test_data = torch.as_tensor(test_data)
+        if shard is not None:
+            self._check_ranks_agree(shard, test_data, len(s_history[0]), total_data, raw, time_aware)
+        self._trim_test_histories()
         fidx = tfidx = None
         if time_aware:
             tfidx = TimeFilterIndex(_quadruples(total_data))
@@ -580,10 +644,10 @@ class RENetInference:
                 t = test_data[i0][3].cpu()
                 rebind = None
                 if self.latest_time != t:                                   # predict's roll-over (model.py:222-330)
-                    last_s, last_o = self._roll_over(t, global_model)
+                    last_s, last_o = self._roll_over(t, global_model, shard)
                     if self.reference_rebinding:
                         rebind = (last_s, last_o)
-                r, loss = self._score_run(quads[i0:i1], s_empty[i0:i1], o_empty[i0:i1], rebind, fidx, tfidx)
+                r, loss = self._score_run(quads[i0:i1], s_empty[i0:i1], o_empty[i0:i1], rebind, fidx, tfidx, shard)
                 if time_aware:
                     for k in PROTOCOLS:
                         protocols[k].append(r[k])
@@ -596,12 +660,42 @@ class RENetInference:
             out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
         return out
 
-    def _score_run(self, quads, s_empty, o_empty, rebind, fidx, tfidx=None):
+    def _eval_shard(self, process_group):
+        """The parallel.Shard evaluate_stream_batched runs on, or None to run unsharded."""
+        if process_group is None:
+            return None
+        import torch.distributed as dist
+        from .parallel import Shard
+        if not (dist.is_available() and dist.is_initialized()):
+            raise ValueError('evaluate_stream_batched: process_group given, but torch.distributed is not initialised')
+        if dist.get_rank(process_group) < 0:
+            raise ValueError('evaluate_stream_batched: this process is not a member of process_group')
+        if dist.get_world_size(process_group) == 1:
+            return None
+        if dist.get_backend(process_group) == 'nccl' and not self.ent_embeds.is_cuda:
+            raise ValueError('evaluate_stream_batched: an NCCL process_group needs the model on a GPU; a model on the host '
+                             'takes a gloo group')
+        return Shard(process_group, self.ent_embeds.device)
+
+    def _check_ranks_agree(self, shard, test_data, n_hist, total_data, raw, time_aware):
+        """ValueError on every rank unless every rank of ``shard`` was called with the same test data (length and a hash of
+        the quadruples), latest_time, num_k and flags: one small all-gather, before any work."""
+        import hashlib
+        q = np.ascontiguousarray(test_data.cpu().numpy().astype(np.int64))
+        digest = int.from_bytes(hashlib.blake2b(q.tobytes(), digest_size=7).digest(), 'little')
+        fp = [len(q), digest, int(self.latest_time), int(self.num_k), n_hist, int(total_data is None), int(bool(raw)),
+              int(bool(time_aware)), int(bool(self.reference_rebinding))]
+        if not shard.same_everywhere(fp):
+            raise ValueError('evaluate_stream_batched: the ranks of process_group were called with different test data, '
+                             'latest_time, num_k or flags')
+
+    def _score_run(self, quads, s_empty, o_empty, rebind, fidx, tfidx=None, shard=None):
         """Scores the triples of one timestamp against the current state: (ranks float64 [2n] as [sub, ob] per triple,
         loss float32 [n] = predict's two cross-entropies per triple).  rebind = (s, o) of the roll-over that the run's first
         triple is scored with (model.py:279,290) or None; its rank labels and filter keys stay its own.  With a
         TimeFilterIndex ``tfidx`` (and ``fidx``) the ranks are a dict of the three PROTOCOLS, the time-aware keys taking the
-        run's timestamp."""
+        run's timestamp.  With a ``shard`` the encoding and the rank call are sharded over its ranks."""
+        from .decoder import ranks_from_counts
         R, h = self.num_rels, self.h_dim
         dev = self.ent_embeds.device
         n = len(quads)
@@ -611,8 +705,8 @@ class RENetInference:
             si[0], oi[0] = rebind
         has_s = ~s_empty & np.asarray([len(self.s_hist_test[e]) != 0 for e in si], dtype=bool)
         has_o = ~o_empty & np.asarray([len(self.o_hist_test[e]) != 0 for e in oi], dtype=bool)
-        s_h = self._encode_queries(si, r, has_s, True)
-        o_h = self._encode_queries(oi, r, has_o, False)
+        s_h = self._encode_queries(si, r, has_s, True, shard)
+        o_h = self._encode_queries(oi, r, has_o, False, shard)
         to_dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(dev)    # noqa: E731
         si_d, oi_d, r_d = to_dev(si), to_dev(oi), to_dev(r)
         x = torch.cat((torch.cat((self.ent_embeds[si_d], s_h, self.rel_embeds[:R][r_d]), dim=1),
@@ -624,16 +718,22 @@ class RENetInference:
             x = torch.cat((x, x[[0, n]]), dim=0)
             rank_lab = np.concatenate((rank_lab, [oi[0], si[0]]))
             loss_row[0], loss_row[n] = 2 * n, 2 * n + 1
+        # Each row's loss and counts depend on that row alone (the rank passes have no split-K and no kernel choice by row
+        # count), so a shard ranks a contiguous slice of the rows, with the exclusion lists of its rows only.
+        m = len(rank_lab)
+        lo, hi = (0, m) if shard is None else shard.slice(m)
         excludes = []                                            # the static filter, then the time-aware one
         if fidx is not None:
-            m = len(rank_lab)
-            fix = np.concatenate((s, o, [s[0], o[0]]))[:m]
-            rr = np.concatenate((r, r, [r[0], r[0]]))[:m]
-            direction = np.concatenate((np.zeros(n, bool), np.ones(n, bool), [False, True]))[:m]
+            fix = np.concatenate((s, o, [s[0], o[0]]))[:m][lo:hi]
+            rr = np.concatenate((r, r, [r[0], r[0]]))[:m][lo:hi]
+            direction = np.concatenate((np.zeros(n, bool), np.ones(n, bool), [False, True]))[:m][lo:hi]
             excludes.append(_exclusion_lists(fidx, direction, fix, rr))
             if tfidx is not None:
-                excludes.append(_exclusion_lists(tfidx, direction, fix, rr, np.full(m, quads[0, 3])))
-        loss_rows, rks = self._rank_rows(x, rank_lab, excludes)
+                excludes.append(_exclusion_lists(tfidx, direction, fix, rr, np.full(hi - lo, quads[0, 3])))
+        loss_rows, counts = self._rank_rows(x[lo:hi], rank_lab[lo:hi], excludes)
+        if shard is not None:
+            loss_rows, counts = shard.allgather_slices(loss_rows, m), shard.allgather_slices(counts, m)
+        rks = [ranks_from_counts(counts[:, 2 * j], counts[:, 2 * j + 1]) for j in range(len(excludes) + 1)]
         pair = lambda rk: np.stack((rk[n:2 * n], rk[:n]), axis=1).reshape(-1)    # noqa: E731
         if tfidx is None:
             ranks = pair(rks[-1].cpu().numpy())                  # filtered with a filter index, else raw
@@ -643,27 +743,31 @@ class RENetInference:
         return ranks, lr[loss_row[:n]] + lr[loss_row[n:]]
 
     def _rank_rows(self, x, label, excludes):
-        """(loss_rows, [raw ranks, then the filtered ranks against each of the 0-2 exclusion lists ``excludes``]) of the
-        rows of x against ``linear``: one renet_decoder_rank_multi call on the GPU; on the host, row by row through
-        ``linear`` as predict computes them, counted with torch once per list."""
-        from .decoder import decoder_rank_counts_multi, ranks_from_counts
+        """(loss_rows [M], counts [M, 2 + 2L]) of the rows of x against ``linear``: the raw (greater, equal) pair, then the
+        filtered pair against each of the L = 0-2 exclusion lists ``excludes``.  One renet_decoder_rank_multi call on the
+        GPU; on the host, row by row through ``linear`` as predict computes them, counted with torch once per list."""
+        from .decoder import decoder_rank_counts_multi
         dev = x.device
         lab = torch.from_numpy(np.ascontiguousarray(label, dtype=np.int64)).to(dev)
+        if len(lab) == 0:
+            # a shard without rows (fewer rows than ranks): nothing to launch, and the empty results keep the dtypes of
+            # the other ranks' shares, which the all-gather after this call needs
+            return (torch.zeros(0, device=dev),
+                    torch.zeros(0, 2 + 2 * len(excludes), dtype=torch.int32 if x.is_cuda else torch.long, device=dev))
         if x.is_cuda:
             ex = [tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev) for a in e) for e in excludes]
-            loss_rows, c = decoder_rank_counts_multi(x, self.linear.weight, self.linear.bias, lab, ex)
-        else:
-            z = torch.stack([self.linear(row) for row in x])
-            loss_rows = torch.stack([self.criterion(z[m].view(1, -1), lab[m].view(1)) for m in range(len(lab))])
-            cs = [rank_counts_torch(z, lab, e) for e in excludes]
-            c = torch.cat([rank_counts_torch(z, lab)[:, :2]] + [ci[:, 2:] for ci in cs], dim=1)
-        return loss_rows, [ranks_from_counts(c[:, 2 * j], c[:, 2 * j + 1]) for j in range(len(excludes) + 1)]
+            return decoder_rank_counts_multi(x, self.linear.weight, self.linear.bias, lab, ex)
+        z = torch.stack([self.linear(row) for row in x])
+        loss_rows = torch.stack([self.criterion(z[m].view(1, -1), lab[m].view(1)) for m in range(len(lab))])
+        cs = [rank_counts_torch(z, lab, e) for e in excludes]
+        return loss_rows, torch.cat([rank_counts_torch(z, lab)[:, :2]] + [ci[:, 2:] for ci in cs], dim=1)
 
-    def _encode_queries(self, ents, rels, has, subject):
+    def _encode_queries(self, ents, rels, has, subject, shard=None):
         """s_h [n, h] of the queries (ents[i], rels[i]) against the current test-time histories; rows where ``has`` is
         False stay zero (predict's empty-history rule).  Equal queries are encoded once.  On the GPU the distinct queries go
         through the device batcher in chunks, one isolation group per entity, so that each equals _encode_one's encoding
-        of it alone; on the host, through _encode_one."""
+        of it alone; on the host, through _encode_one, one query per chunk.  With a ``shard`` chunk j runs on rank
+        j mod world and every rank all-gathers the encodings."""
         h, R = self.h_dim, self.num_rels
         dev = self.ent_embeds.device
         out = torch.zeros(len(ents), h, device=dev)
@@ -674,17 +778,15 @@ class RENetInference:
         q_e, q_r = keys // R, keys % R
         hist = self.s_hist_test if subject else self.o_hist_test
         hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
-        enc = torch.empty(len(keys), h, device=dev)
         if not self.ent_embeds.is_cuda:
-            for j, (e, rr) in enumerate(zip(q_e.tolist(), q_r.tolist())):
-                enc[j] = self._encode_one(e, rr, hist[e], hist_t[e], subject)
+            chunks = [(j, j + 1) for j in range(len(keys))]
         else:
             rel_embeds, reverse = self._direction(subject)
             sizes = {}
             for t in {int(t) for e in np.unique(q_e) for t in hist_t[e]}:
                 g = self.graph_dict[t]
                 sizes[t] = g.number_of_nodes() + g.number_of_edges()
-            j0 = 0
+            chunks, j0 = [], 0
             while j0 < len(keys):
                 # a chunk: whole entities (keys are sorted by entity), within both budgets
                 cost, j1 = 0, j0
@@ -696,18 +798,28 @@ class RENetInference:
                             break
                         cost += c
                     j1 += 1
-                ue, pos = np.unique(q_e[j0:j1], return_inverse=True)
-                view, gs = self._grouped_view(ue, pos, subject)
-                s_dev = torch.from_numpy(q_e[j0:j1]).to(dev)
-                r_dev = torch.from_numpy(q_r[j0:j1]).to(dev)
-                sh, _, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, self.global_emb,
-                                                   reverse, self.encoder, self.encoder_r)
-                # the encoder returns the sequences length-sorted: row k is sample sample_order[k] of the view
-                idx = hb.sample_order(dev)
-                part = torch.empty_like(sh)
-                part[idx] = sh
-                enc[j0:j1] = part
+                chunks.append((j0, j1))
                 j0 = j1
+        parts = []
+        for j0, j1 in (chunks[c] for c in (range(len(chunks)) if shard is None else shard.units(len(chunks)))):
+            if not self.ent_embeds.is_cuda:
+                e, rr = int(q_e[j0]), int(q_r[j0])
+                parts.append(self._encode_one(e, rr, hist[e], hist_t[e], subject).view(1, h).to(out.dtype))
+                continue
+            ue, pos = np.unique(q_e[j0:j1], return_inverse=True)
+            view, gs = self._grouped_view(ue, pos, subject)
+            s_dev = torch.from_numpy(q_e[j0:j1]).to(dev)
+            r_dev = torch.from_numpy(q_r[j0:j1]).to(dev)
+            sh, _, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, self.global_emb,
+                                               reverse, self.encoder, self.encoder_r)
+            # the encoder returns the sequences length-sorted: row k is sample sample_order[k] of the view
+            idx = hb.sample_order(dev)
+            part = torch.empty_like(sh)
+            part[idx] = sh
+            parts.append(part)
+        if shard is not None:
+            parts = shard.gather_units(parts, [j1 - j0 for j0, j1 in chunks], out[:0])
+        enc = torch.cat(parts)
         out[torch.from_numpy(sel).to(dev)] = enc[torch.from_numpy(inverse.reshape(-1)).to(dev)]
         return out
 

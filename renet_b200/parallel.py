@@ -37,6 +37,67 @@ def shard_batch(batch, s_hist, o_hist, rank, world):
     return batch[lo:hi], cut(s_hist), cut(o_hist), (hi - lo)
 
 
+def round_robin(n_units, rank, world):
+    """The units of rank when n_units are handed out round-robin -- unit c to rank c mod world -- in unit order."""
+    return range(rank, n_units, world)
+
+
+class Shard:
+    """One process's place in an evaluation sharded over ``group`` (RENet.evaluate_stream_batched(process_group=...)):
+    its rank and the group's size, and the exchanges the sharded units need.  Exchanges run on ``device`` over NCCL and on
+    the host over any other backend; their results come back on the device of what was sent."""
+
+    def __init__(self, group, device):
+        self.group = group
+        self.rank, self.world = dist.get_rank(group), dist.get_world_size(group)
+        self.xdev = torch.device(device) if dist.get_backend(group) == 'nccl' else torch.device('cpu')
+
+    def units(self, n_units):
+        return round_robin(n_units, self.rank, self.world)
+
+    def slice(self, n):
+        return shard_slice(n, self.rank, self.world)
+
+    def allgather(self, local, counts):
+        """Every rank's block of rows, in rank order: ``local`` [counts[rank], ...] is this rank's, ``counts`` every rank's
+        row count (known on every rank).  The blocks travel padded to the largest one."""
+        cap = max(counts)
+        if cap == 0:
+            return [local[:0]] * self.world
+        buf = torch.zeros((cap,) + tuple(local.shape[1:]), dtype=local.dtype, device=self.xdev)
+        buf[:len(local)] = local
+        out = [torch.empty_like(buf) for _ in range(self.world)]
+        dist.all_gather(out, buf, group=self.group)
+        return [o[:c].to(local.device) for o, c in zip(out, counts)]
+
+    def allgather_slices(self, local, n):
+        """The whole of n rows on every rank, from each rank's contiguous slice(n) of them, ``local`` being this rank's."""
+        counts = [hi - lo for lo, hi in (shard_slice(n, r, self.world) for r in range(self.world))]
+        return torch.cat(self.allgather(local, counts))
+
+    def gather_units(self, blocks, sizes, empty):
+        """Every unit's block, in unit order, on every rank.  ``sizes[c]`` is unit c's row count; ``blocks`` are the blocks of
+        this rank's units (units(len(sizes)), in order); ``empty`` is a zero-row tensor of the blocks' trailing shape, dtype
+        and device."""
+        n = len(sizes)
+        counts = [sum(sizes[c] for c in round_robin(n, r, self.world)) for r in range(self.world)]
+        got = self.allgather(torch.cat([empty] + list(blocks)), counts)
+        out = [None] * n
+        for r in range(self.world):
+            off = 0
+            for c in round_robin(n, r, self.world):
+                out[c] = got[r][off:off + sizes[c]]
+                off += sizes[c]
+        return out
+
+    def same_everywhere(self, values):
+        """True when the int64 vector ``values`` is the same on every rank (one small all-gather; the answer is the same on
+        every rank)."""
+        v = torch.as_tensor(values, dtype=torch.long).view(1, -1)
+        got = self.allgather(v, [1] * self.world)
+        return all(torch.equal(g, got[0]) for g in got)
+
+
 def _world(group=None):
     if dist.is_available() and dist.is_initialized():
         return dist.get_world_size(group)
