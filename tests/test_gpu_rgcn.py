@@ -186,11 +186,17 @@ def test_full_size_properties(G):
 @pytest.mark.parametrize('N,E,heavy,empty_frac', [(5000, 40000, 6000, 0.25), (120, 20000, 0, 0.0), (40000, 17000, 0, 0.7),
                                                   (700000, 17000, 0, 0.9)])
 def test_batch_scale_kernel_edge_cases_fwd_bwd_vs_oracle(G, N, E, heavy, empty_frac):
-    """The persistent batch-scale kernel (rgcn_stream.cuh; taken for E >= 16384) on graphs that stress its partition and
-    hand-over logic: destinations without in-edges (also leading / trailing ones), a destination heavier than a whole
-    CTA's share (its edges span all warps of one CTA: a chain of heads), far fewer destinations than warps, far more
-    destinations than edges, and more destinations per CTA than the shared-memory row_ptr slice holds.  Forward and
-    backward (dH through the same kernel on the reversed graph) against the CPU oracle; bitwise reproducible."""
+    """Whole-layer forward and backward against the CPU oracle on graphs with destinations without in-edges (also leading /
+    trailing ones), a destination heavier than a whole CTA's share, far fewer destinations than warps and far more
+    destinations than edges; the forward is bitwise reproducible.  With today's selection rule (gather_use_stream: E >= 16384
+    and 2048 <= N <= 40960 for plain input rows, 16384 <= N for every backward) the four cases run:
+      (5000, 40000)    forward on the persistent stream kernel (rgcn_stream.cuh), the 6 000-edge destination's chain of heads
+                       included; dH on the tile kernel;
+      (120, 20000)     tile kernels, forward and dH: 8 tiles of ~ 2 500 edges each;
+      (40000, 17000)   stream kernel, forward and dH: about 300 destinations per CTA;
+      (700000, 17000)  tile kernels, forward and dH: 43 750 tiles, most of them without an edge.
+    The stream kernel's remaining paths (row_ptr read from global memory, every instantiation, the selection boundaries)
+    are pinned per row, with the serving kernel asserted, in tests/rgcn_contract_check.py."""
     rng = np.random.RandomState(N + E)
     R2 = 480
     dst = rng.randint(0, N, E)
