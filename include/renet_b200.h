@@ -9,7 +9,8 @@
  *
  * Conventions (all entry points):
  *   - plain pointers + sizes only; every pointer is a DEVICE pointer unless named host_*;
- *   - the caller owns every buffer; nothing is allocated, freed or retained by the library;
+ *   - the caller owns every buffer it passes; the few blocks the library allocates for itself (the GEMM engine's
+ *     per-stream blocks and packed-weight cache, deterministic mode's partial sums) are listed in INTEGRATION.md;
  *   - work is enqueued on `stream` (a cudaStream_t passed as void*; NULL = legacy default stream);
  *     no hidden synchronisation, safe to capture in a CUDA graph, re-entrant, stateless;
  *   - fp32 features/weights, int32 indices (the reference uses int64; convert at the boundary);
@@ -50,9 +51,9 @@ int renet_get_gemm_engine(void);
  * scatter-add, GRU weight, bias and input gradients, with or without input dropout) sums each output element in an order
  * fixed by its inputs and shapes, so repeated calls on identical inputs give bitwise identical results.  It costs extra
  * passes over per-chunk partial sums and a stream-ordered scratch buffer per (device, stream), allocated with
- * cudaMallocAsync on first use and grown on demand (the one exception to "nothing is allocated by the library").  When
- * off, the reductions add with float atomics and the last bits of a gradient may vary from run to run.  The Python
- * binding follows torch.use_deterministic_algorithms.  renet_set_deterministic returns the previous value. */
+ * cudaMallocAsync on first use and grown on demand.  When off, the reductions add with float atomics and the last bits
+ * of a gradient may vary from run to run.  The Python binding follows torch.use_deterministic_algorithms.
+ * renet_set_deterministic returns the previous value. */
 int renet_set_deterministic(int on);
 int renet_get_deterministic(void);
 /* Packed-weight cache of the wgmma GEMM engine.   The engine consumes weights (self-loop matrices, GRU W_ih / W_hh)
@@ -62,12 +63,6 @@ int renet_get_deterministic(void);
  * them.  generation < 0 (default) disables the cache: weights are packed on every call.  The Python host derives the
  * generation from the parameters' identities and in-place version counters. */
 int renet_set_weight_generation(int64_t generation);
-/* Optional caller-owned DEVICE scratch buffer (128-byte aligned) the tensor-core GEMM engine uses for the packed
- * (hi/lo split, K-major, 128-byte-swizzled) copy of the B operand, so that GEMM CTAs can fetch it with TMA bulk
- * copies.  Needs ceil(N/200)*ceil(K/32)*53248 bytes per GEMM (W_loop: 373 KB; GRU input projection: 2.2 MB); without
- * it (or if it is too small) the engine stages B itself.  The buffer is shared by all GEMMs: issue them on ONE
- * stream.  Pass NULL/0 to unregister.  The library never frees it. */
-int renet_set_scratch(void* device_ptr, int64_t bytes);
 
 /* ------------------------------------------------------------------------------------------------
  * Graph preprocessing.  Replaces what DGL does inside g.update_all (RGCN.py:91) to find the
@@ -148,14 +143,14 @@ int renet_debug_gemm_timing(void* buffer);
  * own; never used in production code.
  *   form RENET_GEMM_FORM_NN:        C (+)= A[a_index] @ B (+bias)   A rows through a_index (or NULL); row-major operands
  *                                   with lda / ldb / ldc; kernel 0 dispatches exactly as the self-loop, GRU and RGCN products
- *                                   do (engine, scratch buffer, shape and alignment decide).
+ *                                   do (engine, shape and alignment decide).
  *   form RENET_GEMM_FORM_PREPACKED: for b < batch: B + b*batch_b (row-major [K,N], ldb) is packed into `workspace`, then
  *                                   C + b*batch_c (+)= (A + b*batch_a)[a_index] @ B_b (+ bias + b*N), all entries in one
  *                                   tensor-core launch: the form of the GRU's projections and recurrent products.
  *   form RENET_GEMM_FORM_TN:        C (+)= A[a_index]^T @ B   A [K, lda] (M columns used), B [K, ldb]; no bias; without
  *                                   accumulate C is zeroed first (weight gradients).
  * kernel: 0, or a renet_gemm_kernel to force.  A forced kernel must be able to serve the form and its preconditions must hold
- * (for example RESIDENT needs K <= 224, LEGACY K % 40 == 0, FFMA_TILED 16-byte aligned operands); otherwise the call returns
+ * (for example RESIDENT needs K <= 224, FFMA_TILED 16-byte aligned operands); otherwise the call returns
  * RENET_ERR_INVALID_ARG before anything is launched.  The packed kernels (PREPACKED form, or STREAMING / RESIDENT / DEDUP
  * forced in the NN form) pack B into `workspace`: batch * ceil(N/200) * ceil(K/32) * 53248 bytes, 128-byte aligned.
  * Returns the renet_gemm_kernel that computed C (0 when M == 0), or a negative renet_status. */
@@ -163,7 +158,6 @@ typedef enum { RENET_GEMM_FORM_NN = 0, RENET_GEMM_FORM_PREPACKED = 1, RENET_GEMM
 typedef enum {
   RENET_GEMM_FFMA_TILED = 1,   /* fp32 FFMA, register-tiled (tn form: split-K)                                       */
   RENET_GEMM_FFMA_NAIVE = 2,   /* fp32 FFMA, one thread per output (unaligned operands, N or K not multiples of 4)   */
-  RENET_GEMM_LEGACY = 3,       /* wgmma 3xTF32 staging B itself: no scratch buffer; K % 40 == 0                       */
   RENET_GEMM_STREAMING = 4,    /* wgmma 3xTF32, packed B streamed per 128 x 104 unit, persistent, warp-specialised  */
   RENET_GEMM_RESIDENT = 5,     /* wgmma 3xTF32, packed B panel resident in shared memory (K <= 224)                  */
   RENET_GEMM_DEDUP = 6         /* RESIDENT over the distinct rows of a_index, copied out to every row               */

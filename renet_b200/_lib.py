@@ -23,7 +23,6 @@ SIGNATURES = {
     'renet_set_deterministic': (ctypes.c_int, [ctypes.c_int]),
     'renet_get_deterministic': (ctypes.c_int, []),
     'renet_set_weight_generation': (ctypes.c_int, [_i64]),
-    'renet_set_scratch': (ctypes.c_int, [_vp, _i64]),
     'renet_csr_workspace_bytes': (_i64, [_i64, _i64]),
     'renet_build_csr': (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     'renet_rgcn_block_fwd': (ctypes.c_int, [_vp] * 9 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),
@@ -127,9 +126,6 @@ def stream():
     Every kernel call asks for its stream here, so this is also where the library's deterministic mode follows
     torch.use_deterministic_algorithms(): the flag is read on every call and passed on when it has changed."""
     dev = torch._C._cuda_getDevice()
-    if dev not in _scratch_ready:
-        ensure_scratch(dev)
-        _scratch_ready.add(dev)
     det = torch.are_deterministic_algorithms_enabled()
     if det != _deterministic[0]:
         lib().renet_set_deterministic(int(det))
@@ -137,7 +133,6 @@ def stream():
     return ctypes.c_void_p(torch._C._cuda_getCurrentRawStream(dev))
 
 
-_scratch_ready = set()
 _deterministic = [False]       # the value last passed to renet_set_deterministic (the library starts at 0)
 
 
@@ -153,20 +148,6 @@ def require_cuda(*tensors):
         if t is not None and not t.is_cuda:
             raise RuntimeError('renet_b200: the hot path runs on CUDA only (got a %s tensor); '
                                'there is no CPU fallback' % t.device)
-
-
-_scratch = {}
-
-
-def ensure_scratch(device, nbytes=16 << 20):
-    """Register a per-process device scratch buffer for the tensor-core GEMM engine (packed B operand)."""
-    key = str(device)
-    if key not in _scratch:
-        buf = torch.empty(nbytes, dtype=torch.uint8, device=torch.device('cuda', device) if isinstance(device, int) else device)
-        check(lib().renet_set_scratch(ctypes.c_void_p(buf.data_ptr()), nbytes), 'renet_set_scratch')
-        _scratch.clear()              # one registered buffer at a time (single device per process)
-        _scratch[key] = buf
-    return _scratch[key]
 
 
 def launch_count():

@@ -65,7 +65,6 @@ int launch_pack_inputs(const float* H2, const int32_t* readout, const int32_t* r
 
 int gemm_mode();
 int set_gemm_mode(int m);
-void set_scratch(void* p, int64_t bytes);
 
 namespace {
 
@@ -134,11 +133,6 @@ int renet_get_gemm_engine(void) { return gemm_mode(); }
 int renet_set_deterministic(int on) { return set_deterministic(on); }
 int renet_get_deterministic(void) { return deterministic() ? 1 : 0; }
 int renet_set_weight_generation(int64_t generation) { renet::set_weight_generation(generation); return RENET_OK; }
-int renet_set_scratch(void* device_ptr, int64_t bytes) {
-  RENET_CHECK_ARG(bytes >= 0 && (device_ptr != nullptr || bytes == 0), "renet_set_scratch: bad arguments");
-  set_scratch(device_ptr, bytes);
-  return RENET_OK;
-}
 
 int64_t renet_csr_workspace_bytes(int64_t N, int64_t E) {
   size_t cub_bytes = 0;

@@ -69,8 +69,18 @@ __device__ __forceinline__ void red_add_f4(float* p, float4 v) {
 // only on the inputs and shapes -- no float atomics, no order set by CTA scheduling (DESIGN §4)
 bool deterministic();
 int set_deterministic(int on);
-// Stream-ordered scratch of the deterministic reductions: one buffer per (device, stream), grown on demand with
-// cudaMallocAsync.  *out holds at least `bytes` until the next det_scratch call on the same stream.
+// Stream-ordered device blocks the library keeps for itself: one per (device, stream, kind), allocated with cudaMallocAsync
+// on first use and grown on demand in 8 MB steps, the old block freed behind the work already queued on that stream.  The
+// work of one stream is ordered, so a block is only ever used by its own stream's calls.  *out holds at least `bytes` for
+// work enqueued on `stream` until the next call of the same kind on that stream.
+enum StreamBlockKind { kBlockPackedB, kBlockDedupKeys, kBlockDedupRows, kBlockDeterministic, kNumBlockKinds };
+struct StreamBlock {
+  void* p;
+  int64_t bytes;   // the block's size: at least the bytes asked for
+  int64_t uses;    // earlier calls that returned this block: 0 = allocated by this call (contents undefined)
+};
+int stream_block(StreamBlockKind kind, int64_t bytes, cudaStream_t stream, StreamBlock* out);
+// The block of the deterministic reductions' partial sums and sort keys
 int det_scratch(int64_t bytes, cudaStream_t stream, void** out);
 // out[r * ldo + c] (+)= sum over s = 0, 1, ..., n_parts - 1 of parts[s * stride + r * cols + c]   (r < rows, c < cols)
 int launch_sum_partials(const float* parts, int n_parts, int64_t stride, int64_t rows, int cols, float* out, int64_t ldo,

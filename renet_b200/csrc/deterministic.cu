@@ -2,8 +2,8 @@
 //
 // With the mode on, no gradient of the training step is summed by float atomics: every producer writes partial sums to a
 // buffer indexed by something the inputs and shapes fix (a K chunk, a row chunk, an edge run), and a second pass adds
-// them in index order.  The buffers live in one stream-ordered scratch allocation per (device, stream), so no entry
-// point's signature or workspace size depends on the mode.
+// them in index order.  The buffers live in one stream-ordered block per (device, stream), so no entry point's signature
+// or workspace size depends on the mode.  That per-(device, stream) allocator (stream_block) serves the GEMM engine too.
 #include <cub/device/device_radix_sort.cuh>
 
 #include <atomic>
@@ -20,15 +20,15 @@ int set_deterministic(int on) { return g_deterministic.exchange(on ? 1 : 0); }
 
 namespace {
 
-struct DetScratch {
+struct StreamBlocks {
   int device;
   cudaStream_t stream;
-  void* p;
-  int64_t bytes;
+  StreamBlock kind[kNumBlockKinds];
 };
-std::mutex g_det_mu;
-std::vector<DetScratch> g_det;
-constexpr int kDetMaxStreams = 8;
+std::mutex g_blocks_mu;
+std::vector<StreamBlocks> g_blocks;
+constexpr int kMaxStreams = 8;
+constexpr int64_t kBlockStep = int64_t(8) << 20;
 
 inline int64_t align256(int64_t x) { return (x + 255) & ~int64_t(255); }
 
@@ -82,31 +82,41 @@ __global__ void scatter_add_rows_sorted_kernel(const float* __restrict__ src, in
 
 }  // namespace
 
-int det_scratch(int64_t bytes, cudaStream_t stream, void** out) {
-  std::lock_guard<std::mutex> lk(g_det_mu);
+int stream_block(StreamBlockKind kind, int64_t bytes, cudaStream_t stream, StreamBlock* out) {
+  std::lock_guard<std::mutex> lk(g_blocks_mu);
   int dev = 0;
   RENET_CHECK_CUDA(cudaGetDevice(&dev));
-  DetScratch* s = nullptr;
-  for (auto& e : g_det)
+  StreamBlocks* s = nullptr;
+  for (auto& e : g_blocks)
     if (e.device == dev && e.stream == stream) s = &e;
   if (s == nullptr) {
-    if ((int)g_det.size() >= kDetMaxStreams) {     // bounded: drop the oldest (its stream may be gone: free synchronously)
+    if ((int)g_blocks.size() >= kMaxStreams) {     // bounded: drop the oldest (its stream may be gone: free synchronously)
       RENET_CHECK_CUDA(cudaDeviceSynchronize());
-      RENET_CHECK_CUDA(cudaFree(g_det.front().p));
-      g_det.erase(g_det.begin());
+      for (const StreamBlock& b : g_blocks.front().kind)
+        if (b.p) RENET_CHECK_CUDA(cudaFree(b.p));
+      g_blocks.erase(g_blocks.begin());
     }
-    g_det.push_back(DetScratch{dev, stream, nullptr, 0});
-    s = &g_det.back();
+    g_blocks.push_back(StreamBlocks{dev, stream, {}});
+    s = &g_blocks.back();
   }
-  if (bytes > s->bytes) {
-    const int64_t grown = (bytes + (int64_t(8) << 20) - 1) / (int64_t(8) << 20) * (int64_t(8) << 20);   // 8 MB steps
-    if (s->p) RENET_CHECK_CUDA(cudaFreeAsync(s->p, stream));
-    s->p = nullptr;
-    s->bytes = 0;
-    RENET_CHECK_CUDA(cudaMallocAsync(&s->p, (size_t)grown, stream));
-    s->bytes = grown;
+  StreamBlock& b = s->kind[kind];
+  if (bytes > b.bytes) {
+    const int64_t grown = (bytes + kBlockStep - 1) / kBlockStep * kBlockStep;
+    if (b.p) RENET_CHECK_CUDA(cudaFreeAsync(b.p, stream));
+    b = StreamBlock{};
+    RENET_CHECK_CUDA(cudaMallocAsync(&b.p, (size_t)grown, stream));
+    b.bytes = grown;
   }
-  *out = s->p;
+  *out = b;
+  ++b.uses;
+  return RENET_OK;
+}
+
+int det_scratch(int64_t bytes, cudaStream_t stream, void** out) {
+  StreamBlock b;
+  const int rc = stream_block(kBlockDeterministic, bytes, stream, &b);
+  if (rc) return rc;
+  *out = b.p;
   return RENET_OK;
 }
 

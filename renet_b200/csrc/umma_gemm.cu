@@ -2,22 +2,20 @@
 //
 // RE-Net's dense work on the hot path -- the self-loop H @ W_loop (RGCN.py:35) and the GRU input /
 // recurrent projections (model.py:86,94) -- must match a CPU fp32 oracle to 1e-4, which single-pass
-// TF32 (10-bit mantissa, ~3e-4 on K=200) does not.  This kernel issues wgmma .tf32 with the
+// TF32 (10-bit mantissa, ~3e-4 on K=200) does not.  The kernels issue wgmma .tf32 with the
 // 3xTF32 split:  a = a_hi + a_lo,  b = b_hi + b_lo  (hi = top 19 bits, lo = a - a_hi exactly),
 //     D += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo        (fp32 accumulation in registers)
 // which recovers ~fp32 accuracy (dropped term a_lo*b_lo ~ 2^-22 relative) at 1/3 of TF32 peak -- still
 // several times the FFMA roofline.
 //
-// Structure (one CTA per 128-row tile of A x one <=200-column tile of B, 256 threads = two warpgroups):
-//   * operands are staged by the threads themselves (not TMA): A rows may be gathered through an index
-//     (fused embedding lookup / read-out), B is row-major [K,N] and has to be transposed to K-major,
-//     and both need the hi/lo split, so a register pass is required anyway;
-//   * smem holds two stages of {A_hi, A_lo [128 x 40], B_hi, B_lo [208 x 40]} in the canonical
-//     no-swizzle K-major layout (8-row x 16-byte core matrices; LBO = one 4-column slab, SBO = 128 B);
-//   * warpgroup g issues 15 wgmma (5 k-steps x 3 split products, M=64 rows [64g, 64g+64), N=208, K=8) per stage;
-//     the staging of chunk c+1 overlaps the MMAs of chunk c (at most one wgmma group in flight);
-//   * accumulator: 104 fp32 registers per thread; the epilogue goes through shared memory (thread = row) and
-//     writes C with bias / accumulate applied.
+// Structure: B is packed once per product by umma_pack_b_kernel into the exact shared-memory image the kernels read (hi
+// and lo planes, K-major, 128-byte swizzle), into an image of the packed-weight cache or into a block of the calling
+// stream (stream_block, common.cuh).  A is split into hi / lo as it is staged; its rows may be gathered through an index
+// (fused embedding lookup / read-out).  Two kernels consume the packed image:
+//   * umma_gemm_packed_kernel ("streaming"): persistent and warp-specialised, B streamed per 128 x 104 work unit with TMA
+//     bulk copies; any K, split-K and the fused epilogues;
+//   * umma_gemm_resident_kernel: the whole B panel (K <= 224) resident in shared memory, A fed to wgmma from registers;
+//     umma_gemm_dedup runs it over the distinct rows of an index and copies the rows out.
 #include "common.cuh"
 #include <mutex>
 #include <vector>
@@ -30,164 +28,12 @@ namespace {
 constexpr int UM = 128;          // rows per CTA tile
 constexpr int UN = 200;          // logical columns per CTA tile
 constexpr int UNP = 208;         // padded to a multiple of 16 for the MMA N
-constexpr int UKC = 40;          // K per stage (5 MMA k-steps of 8)
-constexpr int USLABS = UKC / 4;  // 16-byte (4 x fp32) column slabs per stage
-constexpr int UTHREADS = 256;
-constexpr int A_SLAB_BYTES = UM * 16;    // 2048
-constexpr int B_SLAB_BYTES = UNP * 16;   // 3328
-constexpr int A_BYTES = USLABS * A_SLAB_BYTES;   // 20480
-constexpr int B_BYTES = USLABS * B_SLAB_BYTES;   // 33280
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;   // 107520
-constexpr int NUM_STAGES = 2;
-constexpr int SMEM_BYTES = NUM_STAGES * STAGE_BYTES;
-constexpr int CLD = UNP + 4;     // row stride (floats) of the accumulator tile in shared memory: conflict-free float4 rows
-static_assert(UM * CLD * 4 <= SMEM_BYTES, "accumulator tile reuses the operand stages");
-
-template <bool INDEXED>
-__global__ void __launch_bounds__(UTHREADS, 1)
-umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_index, int64_t lda,
-                    const float* __restrict__ B, int64_t ldb, float* __restrict__ C, int64_t ldc,
-                    const float* __restrict__ bias, int64_t M, int N, int K, int accumulate) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
-  const int64_t row0 = (int64_t)blockIdx.x * UM;
-  const int n0 = blockIdx.y * UN;
-  const int tile_n = min(UN, N - n0);
-  const uint32_t smem_base = smem_u32(smem);
-
-  // zero the 8 padding rows (n = 200..207) of every B slab once; they are never written again
-  for (int i = tid; i < NUM_STAGES * 2 * USLABS * (UNP - UN); i += UTHREADS) {
-    const int r = i % (UNP - UN), sl = (i / (UNP - UN)) % USLABS, which = (i / ((UNP - UN) * USLABS)) % 2,
-              st = i / ((UNP - UN) * USLABS * 2);
-    float4* p = reinterpret_cast<float4*>(smem + st * STAGE_BYTES + 2 * A_BYTES + which * B_BYTES + sl * B_SLAB_BYTES +
-                                          (UN + r) * 16);
-    *p = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-
-  // per-thread A source rows: task = slab * 128 + row  (5 tasks per thread per chunk)
-  const float* a_rows[5];
-#pragma unroll
-  for (int t = 0; t < 5; ++t) {
-    const int task = tid + t * UTHREADS;
-    const int r = task % UM;
-    const int64_t gr = row0 + r;
-    a_rows[t] = nullptr;
-    if (gr < M) {
-      const int64_t rr = INDEXED ? (int64_t)__ldg(a_index + gr) : gr;
-      a_rows[t] = A + rr * lda;
-    }
-  }
-
-  float acc[UNP / 2];
-#pragma unroll
-  for (int i = 0; i < UNP / 2; ++i) acc[i] = 0.f;
-  const int nchunks = K / UKC;
-  for (int c = 0; c < nchunks; ++c) {
-    const int st = c % NUM_STAGES;                       // its MMAs of chunk c-2 are complete (barrier below)
-    uint8_t* sA_hi = smem + st * STAGE_BYTES;
-    uint8_t* sA_lo = sA_hi + A_BYTES;
-    uint8_t* sB_hi = sA_lo + A_BYTES;
-    uint8_t* sB_lo = sB_hi + B_BYTES;
-    const int k0 = c * UKC;
-    // ---- A: 128 rows x 10 slabs; thread -> (slab, row): conflict-free 16-byte smem stores ----------
-#pragma unroll
-    for (int t = 0; t < 5; ++t) {
-      const int task = tid + t * UTHREADS;
-      const int sl = task / UM, r = task % UM;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (a_rows[t] != nullptr) v = ldg_f4(a_rows[t] + k0 + 4 * sl);
-      float4 hi, lo;
-      split4(v, hi, lo);
-      *reinterpret_cast<float4*>(sA_hi + sl * A_SLAB_BYTES + r * 16) = hi;
-      *reinterpret_cast<float4*>(sA_lo + sl * A_SLAB_BYTES + r * 16) = lo;
-    }
-    // ---- B: [40 k] x [200 n] row-major -> K-major: 4x4 register transposes -----------------------------
-    for (int task = tid; task < USLABS * (UN / 4); task += UTHREADS) {
-      const int sl = task / (UN / 4), j = task % (UN / 4);
-      float4 m[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        m[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (4 * j < tile_n) m[i] = ldg_f4(B + (int64_t)(k0 + 4 * sl + i) * ldb + n0 + 4 * j);
-      }
-      const float4 t0 = make_float4(m[0].x, m[1].x, m[2].x, m[3].x);
-      const float4 t1 = make_float4(m[0].y, m[1].y, m[2].y, m[3].y);
-      const float4 t2 = make_float4(m[0].z, m[1].z, m[2].z, m[3].z);
-      const float4 t3 = make_float4(m[0].w, m[1].w, m[2].w, m[3].w);
-      const float4 tr[4] = {t0, t1, t2, t3};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float4 hi, lo;
-        split4(tr[q], hi, lo);
-        *reinterpret_cast<float4*>(sB_hi + sl * B_SLAB_BYTES + (4 * j + q) * 16) = hi;
-        *reinterpret_cast<float4*>(sB_lo + sl * B_SLAB_BYTES + (4 * j + q) * 16) = lo;
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
-    __syncthreads();
-    {
-      const uint32_t a_hi = smem_base + st * STAGE_BYTES + wg * 64 * 16, a_lo = a_hi + A_BYTES;   // this warpgroup's 64 rows
-      const uint32_t b_hi = smem_base + st * STAGE_BYTES + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
-      wgmma_fence();
-      acc_fence(acc);
-#pragma unroll
-      for (int ks = 0; ks < UKC / 8; ++ks) {
-        const uint32_t ao = ks * 2 * A_SLAB_BYTES, bo = ks * 2 * B_SLAB_BYTES;
-        const uint64_t dAh = make_desc(a_hi + ao, A_SLAB_BYTES, 128), dAl = make_desc(a_lo + ao, A_SLAB_BYTES, 128);
-        const uint64_t dBh = make_desc(b_hi + bo, B_SLAB_BYTES, 128), dBl = make_desc(b_lo + bo, B_SLAB_BYTES, 128);
-        wgmma_tf32_n208(acc, dAh, dBh, (c | ks) != 0);
-        wgmma_tf32_n208(acc, dAl, dBh, 1);
-        wgmma_tf32_n208(acc, dAh, dBl, 1);
-      }
-      wgmma_commit();
-    }
-    wgmma_wait<1>();             // this warpgroup's MMAs of chunk c-1 are complete
-    acc_fence(acc);
-    __syncthreads();             // ... and the other warpgroup's: stage (c+1) % 2 may be overwritten
-  }
-  wgmma_wait<0>();
-  acc_fence(acc);
-  __syncthreads();               // every MMA has read its operands: the stages hold the accumulator tile now
-
-  // ---- epilogue: registers -> shared tile -> global (thread = row; warps 0-3 cols [0,104), warps 4-7 [104,208)) ---
-  float* sC = reinterpret_cast<float*>(smem);
-  acc_store(acc, sC + wg * 64 * CLD, CLD, tid & 127);
-  __syncthreads();
-  {
-    const int q = warp & 3, half = warp >> 2;
-    const int r = q * 32 + lane;
-    const int64_t gr = row0 + r;
-#pragma unroll 1
-    for (int cc = half * 104; cc < half * 104 + 104; cc += 8) {
-      if (gr < M && cc < tile_n) {
-        const float4 a0 = *reinterpret_cast<const float4*>(sC + r * CLD + cc);
-        const float4 a1 = *reinterpret_cast<const float4*>(sC + r * CLD + cc + 4);
-        float o[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-        float* cp = C + gr * ldc + n0 + cc;
-        if (bias != nullptr) {
-          const float4 b0 = ldg_f4(bias + n0 + cc), b1 = ldg_f4(bias + n0 + cc + 4);
-          o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w;
-          o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
-        }
-        if (accumulate) {
-          const float4 c0 = *reinterpret_cast<const float4*>(cp), c1 = *reinterpret_cast<const float4*>(cp + 4);
-          o[0] += c0.x; o[1] += c0.y; o[2] += c0.z; o[3] += c0.w;
-          o[4] += c1.x; o[5] += c1.y; o[6] += c1.z; o[7] += c1.w;
-        }
-        st_f4(cp, make_float4(o[0], o[1], o[2], o[3]));
-        st_f4(cp + 4, make_float4(o[4], o[5], o[6], o[7]));
-      }
-    }
-  }
-}
-
 
 // ======================================================================================================
-// v2: pre-packed B + TMA bulk copies + 128-byte swizzle, persistent and warp-specialised
+// Streaming kernel: pre-packed B + TMA bulk copies + 128-byte swizzle, persistent and warp-specialised
 //
-// Profiling v1 showed the tile time dominated by operand staging, not by the MMAs: every CTA re-transposed and
-// re-split the same B (W_loop / GRU weights), and the no-swizzle layout forced row-strided A loads (16 useful
-// bytes per 128-byte line).  v2:
+// Operand staging, not the MMAs, dominates a tile's time when every CTA re-transposes and re-splits the same B (W_loop /
+// GRU weights) and a no-swizzle layout forces row-strided A loads (16 useful bytes per 128-byte line).  So:
 //   * B is packed ONCE per GEMM by umma_pack_b_kernel into the exact shared-memory image (hi and lo planes,
 //     K-major, SWIZZLE_128B, one 53 KB block per (column tile, 32-wide K chunk)); rows 0-103 and 104-207 of each
 //     plane are contiguous 13 KB halves (13 whole swizzle atoms), and the GEMM fetches the half it needs with two
@@ -198,8 +44,7 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
 //
 // Work unit = 128 rows x one 104-column half of a 200-column tile (x one batch entry / K-split).  The grid has at most
 // one CTA per SM and CTA b walks the units [b*U/G, (b+1)*U/G), so no SM gets more than one unit above the average:
-// 34.5 k rows x 200 columns are 540 units, 4.09 per SM, at most 5 (half the work of one of the old 128 x 208 tiles
-// each; the old one-tile-per-CTA grid ran 3 waves for 2.05 waves of work).
+// 34.5 k rows x 200 columns are 540 units, 4.09 per SM, at most 5.
 //
 // 384 threads.  Warpgroup 0 is the producer: per chunk it loads A (rows gathered through a_index), splits it into
 // hi/lo, stores it swizzled and issues the B copies.  Warpgroups 1 and 2 are the consumers: each owns 64 rows of the
@@ -207,7 +52,7 @@ umma_gemm_nn_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_i
 // {A hi, A lo [128 x 32], B hi, B lo [104 x 32]} with a full and an empty mbarrier per stage replaces block-wide
 // barriers; the producer runs up to a ring ahead across unit boundaries, so the next unit's operands land while the
 // consumers finish and store the current one, and the consumers keep one wgmma group in flight across chunks.
-// Each output element sees the k-steps in order and per k-step the products hi*hi, lo*hi, hi*lo, as in v1.
+// Each output element sees the k-steps in order and per k-step the products hi*hi, lo*hi, hi*lo.
 // ======================================================================================================
 constexpr int P_BK = 32;
 constexpr int P_A_BYTES = UM * 128;                  // 16384: one plane of 128 rows x 32 K
@@ -856,11 +701,6 @@ dedup_expand_kernel(const float* __restrict__ P, const int32_t* __restrict__ slo
 
 }  // namespace
 
-// Returns 1 if the shape was taken by the tensor-core path (launch enqueued), 0 if the caller should
-// fall back to the FFMA kernel, negative on error.
-static uint8_t* g_scratch = nullptr;
-static int64_t g_scratch_bytes = 0;
-void set_scratch(void* p, int64_t bytes) { g_scratch = (uint8_t*)p; g_scratch_bytes = p ? bytes : 0; }
 static long long* g_gemm_dbg = nullptr;
 void set_gemm_debug_buffer(long long* p) { g_gemm_dbg = p; }
 
@@ -1000,124 +840,32 @@ static int launch_streaming(const float* A, const int32_t* a_index, int64_t lda,
   return RENET_OK;
 }
 
-// The first tensor-core kernel (umma_gemm_nn_kernel): stages B itself, so it needs no scratch buffer, but K % 40 == 0.
-static bool legacy_ok(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias,
-                      int N, int K) {
-  const bool aligned = ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C) |
-                         reinterpret_cast<uintptr_t>(bias)) & 15) == 0;
-  return (K % UKC == 0) && K >= UKC && (N % 8 == 0) && (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) && aligned;
-}
-
-static int launch_legacy(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
-                         int64_t ldc, const float* bias, int64_t M, int N, int K, bool accumulate, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e1 = cudaFuncSetAttribute(umma_gemm_nn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    cudaError_t e2 = cudaFuncSetAttribute(umma_gemm_nn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e1 != cudaSuccess || e2 != cudaSuccess) {
-      set_error("cudaFuncSetAttribute(umma_gemm_nn_kernel) failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
-      return RENET_ERR_CUDA;
-    }
-    attr_set = true;
-  }
-  dim3 grid((unsigned)((M + UM - 1) / UM), (unsigned)((N + UN - 1) / UN));
-  if (a_index)
-    umma_gemm_nn_kernel<true><<<grid, UTHREADS, SMEM_BYTES, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
-  else
-    umma_gemm_nn_kernel<false><<<grid, UTHREADS, SMEM_BYTES, stream>>>(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("launch of umma_gemm_nn_kernel failed: %s", cudaGetErrorString(e));
-    return RENET_ERR_CUDA;
-  }
-  count_launch();
-  note_gemm_kernel(RENET_GEMM_LEGACY);
-  return RENET_OK;
-}
-
-// ---- workspace of the deduplicated product (umma_gemm_dedup) ----------------------------------------------------------
-// One per (device, stream): renet_encode_fwd runs GEMMs on a side stream concurrently with the caller's, and each stream's
-// calls are ordered among themselves, so a workspace is only ever used by the work of its own stream.  It grows on demand
-// with stream-ordered allocations: the old block is freed behind the work already queued on that stream.  The table is
-// zeroed once when allocated (epoch 0 = empty) and never again.
-namespace {
-struct DedupWs {
-  int device;
-  cudaStream_t stream;
-  float* P;                        // [rows, N] compact distinct-row products
-  int64_t p_floats;
-  uint8_t* ix;                     // table [slots] u64 | slot_row [slots] | uniq [rows] | link [rows] | count
-  int64_t rows, slots;
-  uint32_t epoch;
-};
-std::mutex g_dedup_mu;
-std::vector<DedupWs> g_dedup;
-constexpr int kDedupMaxStreams = 8;
-}  // namespace
-
-static int dedup_workspace(int64_t M, int N, cudaStream_t stream, DedupWs* out) {
-  std::lock_guard<std::mutex> lk(g_dedup_mu);
-  int dev = 0;
-  RENET_CHECK_CUDA(cudaGetDevice(&dev));
-  DedupWs* w = nullptr;
-  for (auto& e : g_dedup)
-    if (e.device == dev && e.stream == stream) w = &e;
-  if (w == nullptr) {
-    if ((int)g_dedup.size() >= kDedupMaxStreams) {   // bounded: drop the oldest (its stream may be gone: free synchronously)
-      RENET_CHECK_CUDA(cudaDeviceSynchronize());
-      RENET_CHECK_CUDA(cudaFree(g_dedup.front().P));
-      RENET_CHECK_CUDA(cudaFree(g_dedup.front().ix));
-      g_dedup.erase(g_dedup.begin());
-    }
-    g_dedup.push_back(DedupWs{dev, stream, nullptr, 0, nullptr, 0, 0, 0});
-    w = &g_dedup.back();
-  }
-  const int64_t rows = (M + 16383) / 16384 * 16384;        // grow in steps: batches vary by a few thousand rows
-  if (M * N > w->p_floats) {
-    if (w->P) RENET_CHECK_CUDA(cudaFreeAsync(w->P, stream));
-    w->P = nullptr;
-    w->p_floats = 0;
-    RENET_CHECK_CUDA(cudaMallocAsync((void**)&w->P, (size_t)(rows * N) * sizeof(float), stream));
-    w->p_floats = rows * N;
-  }
-  if (M > w->rows) {
-    if (w->ix) RENET_CHECK_CUDA(cudaFreeAsync(w->ix, stream));
-    w->ix = nullptr;
-    w->rows = w->slots = 0;
-    int64_t s = 1;
-    while (s < 2 * rows) s <<= 1;
-    const size_t bytes = (size_t)s * 12 + (size_t)rows * 8 + 16;
-    RENET_CHECK_CUDA(cudaMallocAsync((void**)&w->ix, bytes, stream));
-    RENET_CHECK_CUDA(cudaMemsetAsync(w->ix, 0, bytes, stream));   // empty table, count = 0
-    w->rows = rows;
-    w->slots = s;
-  }
-  if (++w->epoch == 0) {                                    // wrapped: keys of epoch 0 would read as this call's
-    RENET_CHECK_CUDA(cudaMemsetAsync(w->ix, 0, (size_t)w->slots * 8, stream));
-    w->epoch = 1;
-  }
-  *out = *w;
-  return RENET_OK;
-}
-
-// C[n] = A[a_index[n]] @ Bp (+bias) for n < M through the distinct rows of a_index (see the kernels above)
+// C[n] = A[a_index[n]] @ Bp (+bias) for n < M through the distinct rows of a_index (see the kernels above).  The workspace
+// is two blocks of the calling stream: the keys block holds the count and the hash table and is written by nothing but
+// these kernels, so it is zeroed only when it is new (epoch 0 = empty slot) or every epoch has been used; the rows block
+// holds P, slot_row, uniq and link, each written by a call before that call reads it.
 static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, const void* Bp, float* C, int64_t ldc,
                            const float* bias, int64_t M, int N, int K, cudaStream_t stream) {
-  DedupWs w;
-  int rc = dedup_workspace(M, N, stream, &w);
-  if (rc) return rc;
   int bits = 1;
-  while ((int64_t(1) << bits) < 2 * M) ++bits;              // the table of this call: 2^bits >= 2M of the w.slots
-  unsigned long long* table = reinterpret_cast<unsigned long long*>(w.ix);
-  int32_t* slot_row = reinterpret_cast<int32_t*>(w.ix + w.slots * 8);
-  int32_t* uniq = slot_row + w.slots;
-  int32_t* link = uniq + w.rows;
-  int32_t* count = link + w.rows;
-  dedup_insert_kernel<<<(unsigned)((M + 255) / 256), 256, 0, stream>>>(a_index, M, table, bits, w.epoch, slot_row, uniq, link,
+  while ((int64_t(1) << bits) < 2 * M) ++bits;              // the table of this call: 2^bits >= 2M slots
+  const int64_t slots = int64_t(1) << bits;
+  StreamBlock keys, rows;
+  int rc = stream_block(kBlockDedupKeys, 256 + slots * 8, stream, &keys);
+  if (!rc) rc = stream_block(kBlockDedupRows, (M * N + slots + 2 * M) * 4, stream, &rows);
+  if (rc) return rc;
+  const uint32_t epoch = (uint32_t)(keys.uses % 0xFFFFFFFFu) + 1;   // 1, 2, ..., 2^32 - 1, 1, ...
+  if (epoch == 1) RENET_CHECK_CUDA(cudaMemsetAsync(keys.p, 0, (size_t)keys.bytes, stream));
+  int32_t* count = static_cast<int32_t*>(keys.p);
+  unsigned long long* table = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(keys.p) + 256);
+  float* P = static_cast<float*>(rows.p);
+  int32_t* slot_row = reinterpret_cast<int32_t*>(P + M * N);
+  int32_t* uniq = slot_row + slots;
+  int32_t* link = uniq + M;
+  dedup_insert_kernel<<<(unsigned)((M + 255) / 256), 256, 0, stream>>>(a_index, M, table, bits, epoch, slot_row, uniq, link,
                                                                        count);
   RENET_CHECK_LAUNCH("dedup_insert_kernel");
-  if ((rc = launch_resident(A, uniq, lda, Bp, w.P, N, bias, M, count, N, K, false, 1, 0, 0, 0, stream))) return rc;
-  dedup_expand_kernel<<<(unsigned)((M + 7) / 8), 256, 0, stream>>>(w.P, slot_row, link, C, ldc, M, N, count);
+  if ((rc = launch_resident(A, uniq, lda, Bp, P, N, bias, M, count, N, K, false, 1, 0, 0, 0, stream))) return rc;
+  dedup_expand_kernel<<<(unsigned)((M + 7) / 8), 256, 0, stream>>>(P, slot_row, link, C, ldc, M, N, count);
   RENET_CHECK_LAUNCH("dedup_expand_kernel");
   note_gemm_kernel(RENET_GEMM_DEDUP);
   return RENET_OK;
@@ -1153,29 +901,31 @@ int umma_gemm_prepacked(const float* A, const int32_t* a_index, int64_t lda, con
   return r < 0 ? r : RENET_OK;
 }
 
+// Returns 1 if the shape was taken by the tensor-core path (launch enqueued), 0 if the caller should fall back to the FFMA
+// kernel, negative on error.
 int umma_gemm_nn_try(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
                      int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
                      cudaStream_t stream) {
   const bool aligned = ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C) |
                          reinterpret_cast<uintptr_t>(bias)) & 15) == 0;
-  // ---- packed path: needs the registered scratch buffer for the packed copy of B ---------------------------------
-  if (aligned && umma_shape_ok(N, K) && (lda % 4 == 0) && (ldc % 4 == 0) && M >= 64 && g_scratch != nullptr &&
-      umma_packed_bytes(N, K) <= g_scratch_bytes && (reinterpret_cast<uintptr_t>(g_scratch) & 127) == 0) {
-    bool hit = false;
-    const void* keys[4] = {B, reinterpret_cast<const void*>((intptr_t)ldb), reinterpret_cast<const void*>((intptr_t)N),
-                           reinterpret_cast<const void*>((intptr_t)K)};
-    void* cached = packed_cache_lookup(keys, 4, umma_packed_bytes(N, K), &hit);
-    void* Bp = cached ? cached : g_scratch;
-    int rc = hit ? 0 : umma_pack_b(B, ldb, 1, N, K, Bp, 0, stream);
-    if (rc) return rc;
-    if (a_index != nullptr && !accumulate && M >= kDedupMinRows && resident_ok(N, K, 1))
-      rc = umma_gemm_dedup(A, a_index, lda, Bp, C, ldc, bias, M, N, K, stream);
-    else
-      rc = umma_gemm_prepacked(A, a_index, lda, Bp, C, ldc, bias, M, N, K, accumulate, 1, 0, 0, 0, stream);
-    return rc ? rc : 1;
+  if (!aligned || !umma_shape_ok(N, K) || lda % 4 != 0 || ldc % 4 != 0 || M < 64) return 0;
+  // B's packed image: the cached one of this weight, or (cache off) a fresh one in the calling stream's block
+  const int64_t pb = umma_packed_bytes(N, K);
+  bool hit = false;
+  const void* keys[4] = {B, reinterpret_cast<const void*>((intptr_t)ldb), reinterpret_cast<const void*>((intptr_t)N),
+                         reinterpret_cast<const void*>((intptr_t)K)};
+  void* Bp = packed_cache_lookup(keys, 4, pb, &hit);
+  int rc = 0;
+  if (Bp == nullptr) {
+    StreamBlock blk;
+    if ((rc = stream_block(kBlockPackedB, pb, stream, &blk))) return rc;
+    Bp = blk.p;
   }
-  if (M < 64 || !legacy_ok(A, lda, B, ldb, C, ldc, bias, N, K)) return 0;
-  const int rc = launch_legacy(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
+  if (!hit && (rc = umma_pack_b(B, ldb, 1, N, K, Bp, 0, stream))) return rc;
+  if (a_index != nullptr && !accumulate && M >= kDedupMinRows && resident_ok(N, K, 1))
+    rc = umma_gemm_dedup(A, a_index, lda, Bp, C, ldc, bias, M, N, K, stream);
+  else
+    rc = umma_gemm_prepacked(A, a_index, lda, Bp, C, ldc, bias, M, N, K, accumulate, 1, 0, 0, 0, stream);
   return rc ? rc : 1;
 }
 
@@ -1185,7 +935,8 @@ int debug_gemm(int form, int kernel, const float* A, const int32_t* a_index, int
                int64_t ldc, const float* bias, int64_t M, int N, int64_t K, bool accumulate, int batch, int64_t batch_a,
                int64_t batch_b, int64_t batch_c, void* ws, int64_t ws_bytes, cudaStream_t stream) {
   RENET_CHECK_ARG(form >= RENET_GEMM_FORM_NN && form <= RENET_GEMM_FORM_TN, "renet_debug_gemm: unknown form %d", form);
-  RENET_CHECK_ARG(kernel >= 0 && kernel <= RENET_GEMM_DEDUP, "renet_debug_gemm: unknown kernel %d", kernel);
+  RENET_CHECK_ARG((kernel >= 0 && kernel <= RENET_GEMM_FFMA_NAIVE) || (kernel >= RENET_GEMM_STREAMING && kernel <= RENET_GEMM_DEDUP),
+                  "renet_debug_gemm: unknown kernel %d", kernel);
   RENET_CHECK_ARG(M >= 0 && N > 0 && K > 0 && K < (int64_t(1) << 31) && lda > 0 && ldb > 0 && ldc > 0 && batch >= 1 &&
                       (batch == 1 || form == RENET_GEMM_FORM_PREPACKED),
                   "renet_debug_gemm: bad shape");
@@ -1199,16 +950,13 @@ int debug_gemm(int form, int kernel, const float* A, const int32_t* a_index, int
     if (M == 0) return RENET_OK;
     return sgemm_tn(A, a_index, lda, B, ldb, C, ldc, (int)M, N, K, accumulate, stream, kernel == RENET_GEMM_FFMA_NAIVE);
   }
-  if (form == RENET_GEMM_FORM_NN && (kernel == 0 || ffma || kernel == RENET_GEMM_LEGACY)) {
+  if (form == RENET_GEMM_FORM_NN && (kernel == 0 || ffma)) {
     RENET_CHECK_ARG(kernel != RENET_GEMM_FFMA_TILED || sgemm_nn_tiled_ok(A, lda, B, ldb, C, ldc, bias, N, (int)K),
                     "renet_debug_gemm: the tiled FFMA kernel needs 16-byte aligned operands and N, K, ld* multiples of 4");
-    RENET_CHECK_ARG(kernel != RENET_GEMM_LEGACY || legacy_ok(A, lda, B, ldb, C, ldc, bias, N, (int)K),
-                    "renet_debug_gemm: the legacy kernel needs K %% 40 == 0, N %% 8 == 0, ld* %% 4 == 0, 16-byte aligned operands");
     if (M == 0) return RENET_OK;
     if (kernel == 0) return sgemm_nn(A, a_index, lda, B, ldb, C, ldc, bias, M, N, (int)K, accumulate, stream);
-    if (ffma) return sgemm_nn_ffma(A, a_index, lda, B, ldb, C, ldc, bias, M, N, (int)K, accumulate,
-                                   kernel == RENET_GEMM_FFMA_NAIVE, stream);
-    return launch_legacy(A, a_index, lda, B, ldb, C, ldc, bias, M, N, (int)K, accumulate, stream);
+    return sgemm_nn_ffma(A, a_index, lda, B, ldb, C, ldc, bias, M, N, (int)K, accumulate, kernel == RENET_GEMM_FFMA_NAIVE,
+                         stream);
   }
   // the packed kernels: B (batch of them) packed into the caller's workspace
   RENET_CHECK_ARG(kernel == 0 || kernel == RENET_GEMM_STREAMING || kernel == RENET_GEMM_RESIDENT ||

@@ -22,8 +22,9 @@ The shapes are those of the callers:
     down to 1;
   * the weight gradients (tn form): dW_loop over ~34 k indexed nodes, the GRU dW_hh reduction over (L - 1) * Q rows into the
     right half of dWhh, and the written (not accumulated) input-projection gradients;
-  * the FFMA engine (renet_set_gemm_engine(0)), the legacy tensor-core kernel (no or too small scratch buffer), the FFMA
-    fall-backs (N % 8 != 0, fewer than 64 rows, a pointer 4 bytes off 16-byte alignment)."""
+  * the FFMA engine (renet_set_gemm_engine(0)), the FFMA fall-backs (N % 8 != 0, fewer than 64 rows, a pointer 4 bytes
+    off 16-byte alignment);
+  * two products with different B enqueued at once on two streams, each packing its B into its own stream's block."""
 import collections
 import ctypes
 import os
@@ -37,21 +38,14 @@ from renet_b200 import _lib  # noqa: E402
 L = _lib.lib()
 dev = 'cuda:0'
 PAD = 16            # sentinel rows past M
-FFMA_TILED, FFMA_NAIVE, LEGACY, STREAMING, RESIDENT, DEDUP = 1, 2, 3, 4, 5, 6
-NAMES = {FFMA_TILED: 'ffma-tiled', FFMA_NAIVE: 'ffma-naive', LEGACY: 'legacy', STREAMING: 'streaming', RESIDENT: 'resident',
-         DEDUP: 'dedup'}
+FFMA_TILED, FFMA_NAIVE, STREAMING, RESIDENT, DEDUP = 1, 2, 4, 5, 6
+NAMES = {FFMA_TILED: 'ffma-tiled', FFMA_NAIVE: 'ffma-naive', STREAMING: 'streaming', RESIDENT: 'resident', DEDUP: 'dedup'}
 FORMS = {'nn': 0, 'prepacked': 1, 'tn': 2}
-TOL = {FFMA_TILED: 1e-5, FFMA_NAIVE: 1e-5, LEGACY: 2e-5, STREAMING: 2e-5, RESIDENT: 2e-5, DEDUP: 2e-5}
+TOL = {FFMA_TILED: 1e-5, FFMA_NAIVE: 1e-5, STREAMING: 2e-5, RESIDENT: 2e-5, DEDUP: 2e-5}
 ENT_ROWS = 23033    # ICEWS18 entities: the table the indexed products gather from
 
-stream = _lib.stream()                  # registers the default scratch buffer
-SCRATCH = _lib.ensure_scratch(dev)
+stream = _lib.stream()
 L.renet_set_weight_generation(-1)       # no packed-weight cache: every product packs its B
-
-
-def set_scratch(mode):
-    nbytes = {'yes': SCRATCH.numel(), 'small': 4096, 'no': 0}[mode]
-    _lib.check(L.renet_set_scratch(_lib.ptr(SCRATCH) if nbytes else None, nbytes), 'renet_set_scratch')
 
 
 def addr(t, off=0):
@@ -68,7 +62,7 @@ worst = collections.defaultdict(float)
 n_cases = 0
 
 
-def case(name, expect, M, N, K, form='nn', kernel=0, engine=1, scratch='yes', indexed=False, bias=False, acc=False, batch=1,
+def case(name, expect, M, N, K, form='nn', kernel=0, engine=1, indexed=False, bias=False, acc=False, batch=1,
          lda=None, batch_a=None, a_off=0, ldb=None, b_off=0, ldc=None, batch_c=None, n0=0, same_as=()):
     """One product.  A, B and C are flat buffers; entry b of A / C starts batch_a / batch_c elements after entry 0 (the GRU's
     column-interleaved encoders), C's window starts at column n0 of ldc; a_off shifts A off its allocation (a_off = 1: 4
@@ -130,13 +124,11 @@ def case(name, expect, M, N, K, form='nn', kernel=0, engine=1, scratch='yes', in
     def run_at(kern):
         Cx = C0.clone()
         L.renet_set_gemm_engine(engine)
-        set_scratch(scratch)
         try:
             got = L.renet_debug_gemm(FORMS[form], kern, addr(A, a_off), _lib.ptr(idx), lda, addr(B, b_off), ldb, addr(Cx, n0),
                                      ldc, _lib.ptr(bvec), M, N, K, int(acc), batch, batch_a, batch_b, batch_c, _lib.ptr(ws),
                                      ws_bytes, stream)
         finally:
-            set_scratch('yes')
             L.renet_set_gemm_engine(1)
         if got < 0:
             _lib.check(got, 'renet_debug_gemm(%s)' % name)
@@ -179,9 +171,9 @@ for M in (16384, 64 * 264 - 1, 64 * 264, 64 * 264 + 1, 34483, 34500):
 case('selfloop deduplicated, bias, column window', DEDUP, 16384, 200, 200, indexed=True, bias=True, ldc=1200, n0=600,
      same_as=(RESIDENT,))
 case('selfloop engine 0', FFMA_TILED, 34500, 200, 200, indexed=True, engine=0)
-case('selfloop no scratch', LEGACY, 5000, 200, 200, scratch='no')
-case('selfloop no scratch, indexed', LEGACY, 34483, 200, 200, indexed=True, scratch='no')
-case('selfloop scratch too small', LEGACY, 8449, 200, 200, indexed=True, scratch='small')
+case('selfloop 5000 rows', RESIDENT, 5000, 200, 200)
+case('selfloop indexed, 34483 rows', DEDUP, 34483, 200, 200, indexed=True, same_as=(RESIDENT,))
+case('selfloop indexed, 8449 rows', RESIDENT, 8449, 200, 200, indexed=True)
 
 # ---- K: partly filled last k-step (4, 12, 28), the resident maximum (224), the first streaming K (228), the GRU's 3h / 4h
 for K in (4, 12, 28, 200, 224):
@@ -191,14 +183,14 @@ for K in (228, 600, 800):
     case('K axis', STREAMING, 1153, 200, K)
     case('K axis, engine 0', FFMA_TILED, 1153, 200, K, engine=0)
 case('K axis, indexed, accumulate', STREAMING, 129, 200, 228, indexed=True, acc=True)
-case('K = 40, no scratch', LEGACY, 128, 104, 40, scratch='no')
+case('K = 40, N = 104', RESIDENT, 128, 104, 40, same_as=(STREAMING,))
 
 # ---- N: one 8-column group, 104-column halves and their neighbours, the GRU's 3h / 6h, a non-multiple of 8
 for N in (8, 96, 104, 112, 200, 208, 600, 1200):
     case('N axis', RESIDENT, 1153, N, 200, same_as=(STREAMING,))
     case('N axis, K = 228', STREAMING, 1153, N, 228)
 for N in (104, 112, 208, 600):
-    case('N axis, no scratch', LEGACY, 1153, N, 200, scratch='no', acc=True)
+    case('N axis, accumulate', RESIDENT, 1153, N, 200, acc=True, same_as=(STREAMING,))
 case('N = 196 (N % 8 != 0)', FFMA_TILED, 1153, 196, 200)
 case('N = 196, engine 0', FFMA_TILED, 1153, 196, 200, engine=0)
 case('N = 196, accumulate, bias, window', FFMA_TILED, 129, 196, 200, acc=True, bias=True, ldc=208, n0=4)
@@ -255,7 +247,7 @@ case('batch 2, bias, gaps', RESIDENT, 1153, 200, 200, form='prepacked', batch=2,
 case('batch 2, bias, gaps, K = 228', STREAMING, 1153, 200, 228, form='prepacked', batch=2, bias=True, acc=True, batch_c=208,
      n0=4, ldc=420, indexed=True)
 
-# ---- lda > K, A 4 bytes off 16-byte alignment (FFMA naive), forced FFMA / legacy under engine 1
+# ---- lda > K, A 4 bytes off 16-byte alignment (FFMA naive), forced FFMA under engine 1
 case('lda > K', RESIDENT, 1153, 200, 200, lda=212, indexed=True, same_as=(STREAMING,))
 case('lda > K, engine 0', FFMA_TILED, 1153, 200, 200, lda=212, indexed=True, engine=0)
 case('unaligned A', FFMA_NAIVE, 1153, 200, 200, a_off=1)
@@ -263,8 +255,8 @@ case('unaligned A, engine 0, bias, accumulate', FFMA_NAIVE, 129, 600, 200, a_off
      n0=600)
 case('forced FFMA naive', FFMA_NAIVE, 129, 208, 228, kernel=FFMA_NAIVE, indexed=True, acc=True)
 case('forced FFMA tiled', FFMA_TILED, 1153, 1200, 200, kernel=FFMA_TILED, bias=True)
-case('forced legacy', LEGACY, 1153, 1200, 200, kernel=LEGACY, indexed=True, bias=True)
-case('legacy, bias, window', LEGACY, 1153, 600, 800, scratch='no', bias=True, ldc=1200, n0=600)
+case('N = 6h, indexed, bias', RESIDENT, 1153, 1200, 200, indexed=True, bias=True)
+case('K = 4h, bias, window', STREAMING, 1153, 600, 800, bias=True, ldc=1200, n0=600)
 
 # ---- tn form (FFMA split-K): dW_loop, the GRU dW_hh reduction, the written input-projection gradients
 case('tn dW_loop: indexed, accumulate', FFMA_TILED, 200, 200, 34500, form='tn', indexed=True, acc=True)
@@ -275,6 +267,44 @@ case('tn GRU dW_hh: right half, accumulate', FFMA_TILED, 200, 600, 15 * 3000, fo
 case('tn GRU dB_row: written, window', FFMA_TILED, 200, 600, 1153, form='tn', indexed=True, ldc=1208, n0=4)
 case('tn unaligned', FFMA_NAIVE, 200, 600, 1153, form='tn', acc=True, a_off=1)
 case('tn forced naive', FFMA_NAIVE, 100, 300, 2000, form='tn', kernel=FFMA_NAIVE, indexed=True)
+
+
+def two_streams():
+    """Two self-loop products with different B enqueued back to back on two non-blocking streams (torch's pool streams),
+    with no synchronisation between them: each packs its B while the other's kernels may still read theirs.  Each must
+    match fp64 and leave its sentinel rows untouched."""
+    global n_cases
+    torch.manual_seed(n_cases)
+    n_cases += 1
+    M, N, K = 34500, 200, 200
+    runs = []
+    for indexed, kern in ((True, DEDUP), (False, RESIDENT)):
+        A = torch.randn(ENT_ROWS if indexed else M, K, device=dev) * 0.3
+        B = torch.randn(K, N, device=dev) * 0.1
+        idx = torch.randint(0, A.shape[0], (M,), device=dev, dtype=torch.int32) if indexed else None
+        C0 = torch.full((M + PAD, N), float('nan'), device=dev)
+        runs.append((kern, A, B, idx, C0, C0.clone(), torch.cuda.Stream(device=dev)))
+    torch.cuda.synchronize()
+    got = [L.renet_debug_gemm(FORMS['nn'], 0, _lib.ptr(A), _lib.ptr(idx), K, _lib.ptr(B), N, _lib.ptr(C), N, None, M, N, K,
+                              0, 1, 0, 0, 0, None, 0, ctypes.c_void_p(s.cuda_stream))
+           for kern, A, B, idx, C0, C, s in runs]
+    torch.cuda.synchronize()
+    for g, (kern, A, B, idx, C0, C, s) in zip(got, runs):
+        if g < 0:
+            _lib.check(g, 'renet_debug_gemm(two streams)')
+        assert g == kern, 'two streams: served by %s, expected %s' % (NAMES.get(g, g), NAMES[kern])
+        ref = (A[idx.long()] if idx is not None else A).double() @ B.double()
+        assert not torch.isnan(C[:M]).any(), 'two streams (%s): outputs left unwritten' % NAMES[kern]
+        err = ((C[:M].double() - ref).abs().max() / ref.abs().max()).item()
+        assert torch.equal(C[M:].view(torch.int32), C0[M:].view(torch.int32)), 'two streams (%s): sentinels changed' % (
+            NAMES[kern])
+        assert err < TOL[kern], 'two streams (%s): error %.3e > %.0e' % (NAMES[kern], err, TOL[kern])
+        print('%-44s %-10s M=%-6d N=%-5d K=%-5d err %.2e' % ('two streams', NAMES[kern], M, N, K, err), flush=True)
+        count[kern] += 1
+        worst[kern] = max(worst[kern], err)
+
+
+two_streams()
 
 print('cases per kernel: ' + ', '.join('%s %d' % (NAMES[k], count[k]) for k in sorted(count)))
 print('forms: ' + ', '.join('%s/%s %d' % (f, NAMES[k], n) for (f, k), n in sorted(forms_seen.items())))

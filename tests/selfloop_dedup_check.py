@@ -23,7 +23,6 @@ PAD = 64          # rows past M that must stay untouched
 K = N = 200
 
 torch.manual_seed(0)
-_lib.ensure_scratch(dev)
 L.renet_set_gemm_engine(1)
 L.renet_set_weight_generation(-1)       # no packed-weight cache: every call packs B (one launch)
 B = torch.randn(K, N, device=dev) * 0.1

@@ -63,7 +63,7 @@ def test_argument_validation_needs_no_gpu(so_path):
             (dict(form=0, kernel=5, K=228), b'resident kernel needs K <= 224'),    # RESIDENT past its panel size
             (dict(form=1, kernel=6, idx=fake[3]), b'cannot serve'),              # DEDUP outside the nn form
             (dict(form=0, kernel=6, idx=fake[3], acc=1), b'no accumulate'),       # DEDUP accumulating
-            (dict(form=0, kernel=3, K=228), b'legacy kernel needs K % 40'),       # LEGACY with K % 40 != 0
+            (dict(form=0, kernel=3), b'unknown kernel'),                         # 3: the retired kernel id
             (dict(form=0, kernel=1, A=ctypes.c_void_p(4100)), b'tiled FFMA'),     # FFMA_TILED on an unaligned operand
             (dict(form=2, kernel=5), b'FFMA kernels only'),                       # the tn form on a tensor-core kernel
             (dict(form=0, kernel=4, A=ctypes.c_void_p(4100)), b'16-byte aligned'),  # STREAMING on an unaligned operand

@@ -18,7 +18,6 @@ indexed = (sys.argv[2] if len(sys.argv) > 2 else 'indexed') == 'indexed'
 N = K = 200
 dev = torch.device('cuda:0')
 L, P = _lib.lib(), _lib.ptr
-_lib.ensure_scratch(dev)
 L.renet_set_gemm_engine(1)
 torch.manual_seed(0)
 rows = 23033 if indexed else M
