@@ -329,7 +329,8 @@ int renet_gru_dense_bwd(const float* X4, int32_t k4, const float* X3, int32_t k3
 
 /* Per-graph pooling over a batched graph: out[g] = max (mode 1) or mean (mode 0) of H[seg_ptr[g] .. seg_ptr[g+1]) -- dgl.max_nodes /
  * dgl.mean_nodes of the reference's global aggregator (Aggregator.py:58-61).  argmax [G,d] (mode 1) keeps the winning row for
- * backward; renet_segment_pool_bwd writes dH [N,d] (zeros elsewhere). */
+ * backward; renet_segment_pool_bwd writes dH [N,d] (zeros elsewhere).  The max starts from -inf and the first maximum wins,
+ * so a segment whose values are all -inf gives -inf with argmax at its first row, as torch.max does; an empty segment gives 0. */
 int renet_segment_pool_fwd(const float* H, const int32_t* seg_ptr, int64_t G, int32_t d, int32_t mode, float* out,
                            int32_t* argmax, void* stream);
 int renet_segment_pool_bwd(const float* dout, const int32_t* seg_ptr, const int32_t* argmax, int64_t G, int64_t N,
@@ -597,7 +598,8 @@ int renet_decoder_rank_multi(const float* X, const float* W, const float* bias, 
  * engine keeps all parameters / gradients as views into one flat buffer each (the gradient buffer is what NCCL
  * all-reduces), so the step is two HBM-bound launches.
  *   renet_grad_sumsq : out[0] (=|+=) sum(grad[i]^2), fixed-order reduction (reproducible, no float atomics);
- *                      workspace: renet_grad_sumsq_workspace_bytes() bytes.
+ *                      workspace: renet_grad_sumsq_workspace_bytes() bytes.  n == 0 launches only the final kernel
+ *                      (out = 0, or unchanged with accumulate) and never touches grad or the workspace, which may be NULL.
  *   renet_adam_step  : g = grad*grad_scale*clip (+ weight_decay*param);  clip = min(1, max_norm/(sqrt(sumsq[0])*grad_scale
  *                      + 1e-6)) when sumsq != NULL and max_norm > 0, else 1;  m,v moments; bias correction with `step`
  *                      (counts from 1); param updated in place.  Matches torch.optim.Adam (amsgrad=False).

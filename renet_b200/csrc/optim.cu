@@ -107,10 +107,13 @@ int renet_grad_sumsq(const float* grad, int64_t n, float* out, int32_t accumulat
   RENET_CHECK_ARG(n == 0 || (grad != nullptr && workspace != nullptr && workspace_bytes >= renet_grad_sumsq_workspace_bytes()),
                   "renet_grad_sumsq: null pointer / workspace too small");
   RENET_CHECK_ARG((reinterpret_cast<uintptr_t>(grad) & 15) == 0, "renet_grad_sumsq: grad must be 16-byte aligned");
+  // n == 0 may come with a NULL workspace: no partial block runs, and the final kernel (nblk = 0) writes 0 or keeps out
   int64_t want = (n / 4 + kRedThreads - 1) / kRedThreads;
-  const int nblk = (int)(want < 1 ? 1 : (want > kRedBlocks ? kRedBlocks : want));
-  grad_sumsq_partial_kernel<<<nblk, kRedThreads, 0, (cudaStream_t)stream>>>(grad, n, (float*)workspace);
-  RENET_CHECK_LAUNCH("grad_sumsq_partial_kernel");
+  const int nblk = n == 0 ? 0 : (int)(want < 1 ? 1 : (want > kRedBlocks ? kRedBlocks : want));
+  if (nblk > 0) {
+    grad_sumsq_partial_kernel<<<nblk, kRedThreads, 0, (cudaStream_t)stream>>>(grad, n, (float*)workspace);
+    RENET_CHECK_LAUNCH("grad_sumsq_partial_kernel");
+  }
   grad_sumsq_final_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>((const float*)workspace, nblk, out, accumulate);
   RENET_CHECK_LAUNCH("grad_sumsq_final_kernel");
   return RENET_OK;

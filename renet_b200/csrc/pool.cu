@@ -1,6 +1,8 @@
 // Per-graph pooling of node features over a batched graph: dgl.max_nodes / dgl.mean_nodes of the reference's global
 // aggregator (Aggregator.py:58-61, 101-104) -- one row per batched graph (timestamp) out of all its nodes' layer-2 features.
 // HBM-bound: every node row is read once (forward) / written once (backward).
+#include <math.h>
+
 #include "common.cuh"
 
 namespace renet {
@@ -14,7 +16,7 @@ segment_pool_fwd_kernel(const float* __restrict__ H, const int32_t* __restrict__
   const int g = blockIdx.x, c = blockIdx.y * 128 + threadIdx.x;
   if (c >= d) return;
   const int r0 = __ldg(seg_ptr + g), r1 = __ldg(seg_ptr + g + 1);
-  float best = MAX ? -3.402823466e38f : 0.f;
+  float best = MAX ? -INFINITY : 0.f;      // an all -inf segment gives -inf (arg = its first row), as torch.max does
   int arg = r0;
   for (int r = r0; r < r1; ++r) {
     const float v = __ldg(H + (int64_t)r * d + c);
