@@ -561,6 +561,25 @@ int renet_decoder_group_topk(const float* X, const float* W, const float* bias, 
                              int32_t N, int32_t K, int32_t k, int32_t order, int32_t capacity, float* values, int32_t* indices,
                              int32_t* needed, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Per-row top-k with exclusion lists: the forecast of M queries (RENet.forecast).  z = X @ W^T + bias, p[m, n] =
+ * exp(z[m, n] - logsumexp_n z[m, n]) over all N columns.  Row m's exclusion list is excl_col[excl_begin[m] ..
+ * excl_end[m]) (int32, ascending; rows may share a range; excl_col == NULL: no lists, and excl_begin / excl_end are not
+ * read).  values[m, :k] = the k largest p[m, n] over the columns n not in the list, in RENET_TOPK_ORDER_VALUE order (p
+ * descending, ties to the lower column), indices[m, :k] = those columns.  The excluded columns stay in the softmax's
+ * normaliser, so a value is the model's own probability of its answer.  A row with fewer than k admissible columns gets
+ * index -1 and value 0 in its last slots.  The steps of renet_decoder_group_topk with R = 1 and weight 1; the per-row
+ * threshold is taken at rank k + (excl_end[m] - excl_begin[m]) of the partial maxima, so that at least k admissible
+ * columns pass it.  The capacity protocol (*needed) is renet_decoder_group_topk's; a row's candidates include its
+ * excluded columns, so the first capacity should allow for the list lengths.  No float atomics; the output is bitwise
+ * reproducible, and each row depends on that row alone.  K % 4 == 0, 1 <= k <= min(N, RENET_TOPK_MAX_K), capacity >= k;
+ * X [M,K], W [N,K] row-major, 16-byte aligned; bias [N] may be NULL; values fp32 [M,k], indices int32 [M,k].  Rejected
+ * before any launch: a bad shape or k, a null excl_begin or excl_end with a non-null excl_col, null pointers, a workspace
+ * too small. */
+int64_t renet_decoder_topk_workspace_bytes(int64_t M, int32_t N, int32_t K, int32_t capacity);
+int renet_decoder_topk(const float* X, const float* W, const float* bias, const int32_t* excl_col, const int32_t* excl_begin,
+                       const int32_t* excl_end, int64_t M, int32_t N, int32_t K, int32_t k, int32_t capacity, float* values,
+                       int32_t* indices, int32_t* needed, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Rank of a label among a decoder's logits: the test-time scoring of reference model.py:365-419 (evaluate /
  * evaluate_filter) for M rows at once.  z = X @ W^T + bias; row m has the label l = label[m] in [0, N).

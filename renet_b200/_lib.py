@@ -79,6 +79,8 @@ SIGNATURES = {
     'renet_decoder_group_topk_workspace_bytes': (_i64, [_i64, _i32, _i32, _i32, _i32]),
     'renet_decoder_group_topk': (ctypes.c_int, [_vp] * 4 + [_i64, _i32, _i32, _i32, _i32, _i32, _i32] + [_vp] * 4 +
                                  [_i64, _vp]),
+    'renet_decoder_topk_workspace_bytes': (_i64, [_i64, _i32, _i32, _i32]),
+    'renet_decoder_topk': (ctypes.c_int, [_vp] * 6 + [_i64, _i32, _i32, _i32, _i32] + [_vp] * 4 + [_i64, _vp]),
     'renet_decoder_rank_workspace_bytes': (_i64, [_i64, _i32, _i32]),
     'renet_decoder_rank': (ctypes.c_int, [_vp] * 9 + [_i64, _i32, _i32, _vp, _i64, _vp]),
     'renet_decoder_rank_multi': (ctypes.c_int, [_vp] * 4 + [_i32] + [_vp] * 5 + [_i64, _i32, _i32, _vp, _i64, _vp]),

@@ -31,6 +31,11 @@
 //      the lower index, and bitonic-sorts the k winners into the output order in shared memory.
 // Every step is either a fixed-order computation or an integer count, so the output is bitwise reproducible.
 //
+// Per-row top-k with exclusion lists (renet_decoder_topk; the forecast of RENet.forecast): the same four steps with R = 1
+// and row weight 1, through the EXCL instantiations of the tau and final kernels.  Step 2 takes the (k + L_m)-th partial
+// maximum of row m, L_m the length of its exclusion list, so that at least k admissible columns pass; step 4 drops the
+// listed columns before the select.  The softmax stays over all N columns.
+//
 // Rank counts (test-time scoring, reference model.py:365-419): per row, the label's rank among the row's logits, raw and
 // filtered against each of 0-2 exclusion lists (the static and the time-aware filter of evaluate_stream(time_aware=True)),
 // by the tie rule #greater + (#equal - 1) / 2 + 1, without writing the [M, N] logits.  One rank pass (rank_counts below):
@@ -207,22 +212,35 @@ __device__ KeyT block_kth_largest(int64_t n, int64_t k, F key, int* hist) {
 
 // tau[g] = the k-th largest of w_m * exp(pmax[i, m] - lse_m) over the rows m of group g and the partials i (0 when the
 // group has fewer than k partials).  One block per group.
+// EXCL (renet_decoder_topk): R = 1, every row weight is 1 (the kernel writes it to ones_out[g] for the EPI 5 pass), and
+// row g has the exclusion list [excl_begin[g], excl_end[g]) (no lists when excl_begin is null).  The rank taken is k + L_g,
+// L_g the list's length: each partial max is a real logit of its (row, half tile) unit and each excluded column lies in one
+// unit, so at most L_g of the k + L_g largest partial maxima are excluded columns, and at least k admissible columns have
+// p >= tau.
+template <bool EXCL>
 __global__ void __launch_bounds__(256) topk_tau_kernel(const float* __restrict__ pmax, const float* __restrict__ lse,
                                                        const float* __restrict__ row_w, int n_part, int R, int64_t M, int k,
-                                                       float* __restrict__ tau) {
+                                                       float* __restrict__ tau, const int32_t* __restrict__ excl_begin = nullptr,
+                                                       const int32_t* __restrict__ excl_end = nullptr,
+                                                       float* __restrict__ ones_out = nullptr) {
   __shared__ int hist[256];
   const int64_t g = blockIdx.x;
   const int64_t n = (int64_t)R * n_part;
-  if (n < k) {
+  int64_t rank = k;
+  if constexpr (EXCL) {
+    if (threadIdx.x == 0) ones_out[g] = 1.f;
+    if (excl_begin != nullptr) rank += max(0, __ldg(excl_end + g) - __ldg(excl_begin + g));
+  }
+  if (n < rank) {
     if (threadIdx.x == 0) tau[g] = 0.f;
     return;
   }
   const int64_t m0 = g * R;
   auto key = [&](int64_t i) -> uint32_t {
     const int64_t part = i / R, m = m0 + (i - part * R);
-    return prob_bits(topk_prob(__ldg(pmax + part * M + m), __ldg(lse + m), __ldg(row_w + m)));
+    return prob_bits(topk_prob(__ldg(pmax + part * M + m), __ldg(lse + m), EXCL ? 1.f : __ldg(row_w + m)));
   };
-  const uint32_t t = block_kth_largest<uint32_t>(n, k, key, hist);
+  const uint32_t t = block_kth_largest<uint32_t>(n, rank, key, hist);
   if (threadIdx.x == 0) tau[g] = __uint_as_float(t);
 }
 
@@ -230,11 +248,18 @@ constexpr int kTopkFinalThreads = 512;
 
 // One block per group: the k best candidates by (p descending, index ascending), written in the caller's order.
 // sort_n = the power of two >= k the shared-memory sort runs over.
+// EXCL (renet_decoder_topk): R = 1, and the candidates in row g's exclusion list excl_col[excl_begin[g] .. excl_end[g])
+// (ascending; no lists when excl_col is null) are dropped before the select.  When fewer than k candidates remain, the
+// slots past them get index -1 and value 0.
+template <bool EXCL>
 __global__ void __launch_bounds__(kTopkFinalThreads) topk_final_kernel(const float* __restrict__ cand_val,
                                                                        const int32_t* __restrict__ cand_idx,
                                                                        const int32_t* __restrict__ count, int cap, int k,
                                                                        int order, int sort_n, float* __restrict__ values,
-                                                                       int32_t* __restrict__ indices, int32_t* __restrict__ needed) {
+                                                                       int32_t* __restrict__ indices, int32_t* __restrict__ needed,
+                                                                       const int32_t* __restrict__ excl_col = nullptr,
+                                                                       const int32_t* __restrict__ excl_begin = nullptr,
+                                                                       const int32_t* __restrict__ excl_end = nullptr) {
   extern __shared__ unsigned long long s_keys[];      // [sort_n]
   __shared__ int hist[256];
   __shared__ int s_fill;
@@ -246,11 +271,43 @@ __global__ void __launch_bounds__(kTopkFinalThreads) topk_final_kernel(const flo
   }
   const float* cv = cand_val + g * cap;
   const int32_t* ci = cand_idx + g * cap;
-  // larger key = better: p descending, then index ascending; keys are distinct because indices are
+  int xb = 0, xe = 0;
+  if constexpr (EXCL) {
+    if (excl_col != nullptr) {
+      xb = __ldg(excl_begin + g);
+      xe = __ldg(excl_end + g);
+    }
+  }
+  auto excluded = [&](int32_t c) -> bool {            // binary search of the row's ascending list
+    int lo = xb, hi = xe;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (__ldg(excl_col + mid) < c) lo = mid + 1; else hi = mid;
+    }
+    return lo < xe && __ldg(excl_col + lo) == c;
+  };
+  // larger key = better: p descending, then index ascending; keys are distinct because indices are.  EXCL: an excluded
+  // candidate has key 0, below every real key (whose low word ~index is >= 2^31)
   auto key = [&](int64_t i) -> unsigned long long {
+    if constexpr (EXCL) {
+      if (xb < xe && excluded(ci[i])) return 0ull;
+    }
     return ((unsigned long long)prob_bits(cv[i]) << 32) | (uint32_t)~(uint32_t)ci[i];
   };
-  const unsigned long long kth = block_kth_largest<unsigned long long>(n, k, key, hist);
+  int kk = k;                                          // the winners: min(k, admissible candidates)
+  if constexpr (EXCL) {
+    if (threadIdx.x == 0) s_fill = 0;
+    __syncthreads();
+    int adm = 0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) adm += key(i) != 0ull;
+    if (adm) atomicAdd(&s_fill, adm);
+    __syncthreads();
+    kk = min(k, s_fill);
+    __syncthreads();
+  }
+  unsigned long long kth;
+  if constexpr (EXCL) kth = kk > 0 ? block_kth_largest<unsigned long long>(n, kk, key, hist) : ~0ull;   // ~0: no real key
+  else kth = block_kth_largest<unsigned long long>(n, k, key, hist);
   const uint32_t kth_p = (uint32_t)(kth >> 32);
   if (threadIdx.x == 0) s_fill = 0;
   __syncthreads();
@@ -265,7 +322,7 @@ __global__ void __launch_bounds__(kTopkFinalThreads) topk_final_kernel(const flo
                                              : ((unsigned long long)(p == kth_p) << 63) | ((unsigned long long)idx << 32) | p;
     s_keys[atomicAdd(&s_fill, 1)] = sk;
   }
-  for (int i = k + threadIdx.x; i < sort_n; i += blockDim.x) s_keys[i] = ~0ull;
+  for (int i = kk + threadIdx.x; i < sort_n; i += blockDim.x) s_keys[i] = ~0ull;
   __syncthreads();
   for (int size = 2; size <= sort_n; size <<= 1) {
     for (int stride = size >> 1; stride > 0; stride >>= 1) {
@@ -281,6 +338,13 @@ __global__ void __launch_bounds__(kTopkFinalThreads) topk_final_kernel(const flo
     }
   }
   for (int j = threadIdx.x; j < k; j += blockDim.x) {
+    if constexpr (EXCL) {
+      if (j >= kk) {
+        values[g * k + j] = 0.f;
+        indices[g * k + j] = -1;
+        continue;
+      }
+    }
     const unsigned long long sk = s_keys[j];
     uint32_t p, idx;
     if (order == 1) {
@@ -500,7 +564,7 @@ int renet_decoder_group_topk(const float* X, const float* W, const float* bias, 
                   "renet_decoder_group_topk: X and W must be 16-byte aligned");
   static bool attr = false;
   if (!attr) {
-    RENET_CHECK_CUDA(cudaFuncSetAttribute(topk_final_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RENET_TOPK_MAX_K * 8));
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(topk_final_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RENET_TOPK_MAX_K * 8));
     attr = true;
   }
   void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
@@ -519,7 +583,7 @@ int renet_decoder_group_topk(const float* X, const float* W, const float* bias, 
   ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.pmax, w.psum, nullptr, n_part, M, w.lse, nullptr);
   RENET_CHECK_LAUNCH("ce_reduce_kernel");
   // 2. per-group threshold from the partial maxima
-  topk_tau_kernel<<<(unsigned)G, 256, 0, stream>>>(w.pmax, w.lse, row_weight, n_part, R, M, k, w.tau);
+  topk_tau_kernel<false><<<(unsigned)G, 256, 0, stream>>>(w.pmax, w.lse, row_weight, n_part, R, M, k, w.tau);
   RENET_CHECK_LAUNCH("topk_tau_kernel");
   // 3. the candidates at or above it
   EpiArgs sel{};
@@ -530,8 +594,69 @@ int renet_decoder_group_topk(const float* X, const float* W, const float* bias, 
   // 4. the k best of each group's candidates, in the requested order
   int sort_n = 2;
   while (sort_n < k) sort_n <<= 1;
-  topk_final_kernel<<<(unsigned)G, kTopkFinalThreads, (size_t)sort_n * 8, stream>>>(w.cand_val, w.cand_idx, w.count, capacity, k,
-                                                                                     order, sort_n, values, indices, needed);
+  topk_final_kernel<false><<<(unsigned)G, kTopkFinalThreads, (size_t)sort_n * 8, stream>>>(w.cand_val, w.cand_idx, w.count,
+                                                                                            capacity, k, order, sort_n, values,
+                                                                                            indices, needed);
+  RENET_CHECK_LAUNCH("topk_final_kernel");
+  return RENET_OK;
+}
+
+int64_t renet_decoder_topk_workspace_bytes(int64_t M, int32_t N, int32_t K, int32_t capacity) {
+  return carve_topk(nullptr, M, 1, N, K, capacity).total + align256(M * 4) + 256;
+}
+
+int renet_decoder_topk(const float* X, const float* W, const float* bias, const int32_t* excl_col, const int32_t* excl_begin,
+                       const int32_t* excl_end, int64_t M, int32_t N, int32_t K, int32_t k, int32_t capacity, float* values,
+                       int32_t* indices, int32_t* needed, void* workspace, int64_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  RENET_CHECK_ARG(M >= 0 && N > 0 && K > 0 && K % 4 == 0, "renet_decoder_topk: bad shape (K must be a multiple of 4)");
+  RENET_CHECK_ARG(k >= 1 && k <= N, "renet_decoder_topk: k = %d outside [1, N = %d]", k, N);
+  RENET_CHECK_ARG(k <= RENET_TOPK_MAX_K, "renet_decoder_topk: k = %d above RENET_TOPK_MAX_K = %d", k, RENET_TOPK_MAX_K);
+  RENET_CHECK_ARG(capacity >= k, "renet_decoder_topk: capacity %d < k = %d", capacity, k);
+  RENET_CHECK_ARG(excl_col == nullptr || (excl_begin != nullptr && excl_end != nullptr),
+                  "renet_decoder_topk: exclusion lists need excl_begin and excl_end");
+  RENET_CHECK_ARG(needed != nullptr, "renet_decoder_topk: null pointer");
+  if (M == 0) return RENET_OK;
+  RENET_CHECK_ARG(X && W && values && indices && workspace, "renet_decoder_topk: null pointer");
+  RENET_CHECK_ARG(workspace_bytes >= renet_decoder_topk_workspace_bytes(M, N, K, capacity), "renet_decoder_topk: workspace too small");
+  RENET_CHECK_ARG(((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
+                  "renet_decoder_topk: X and W must be 16-byte aligned");
+  static bool attr = false;
+  if (!attr) {
+    RENET_CHECK_CUDA(cudaFuncSetAttribute(topk_final_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RENET_TOPK_MAX_K * 8));
+    attr = true;
+  }
+  void* base = (void*)(((uintptr_t)workspace + 255) & ~uintptr_t(255));
+  TopkWs w = carve_topk(base, M, 1, N, K, capacity);
+  float* ones = (float*)((char*)base + w.total);                 // every row's weight, 1: the EPI 5 pass reads it
+  const int32_t* xb = excl_col != nullptr ? excl_begin : nullptr;
+  const int32_t* xe = excl_col != nullptr ? excl_end : nullptr;
+  const int n_part = 2 * ((N + 199) / 200);
+  RENET_CHECK_CUDA(cudaMemsetAsync(needed, 0, 4, stream));
+  RENET_CHECK_CUDA(cudaMemsetAsync(w.count, 0, (size_t)M * 4, stream));
+  // 1. lse of every row (k_splits = 1: a row's logits and partials do not depend on the other rows)
+  int rc = umma_pack_b(W, 1, K, N, K, w.Wp, 0, stream);          // logical B[k][n] = W[n*K + k]
+  if (rc) return rc;
+  EpiArgs epi{};
+  epi.pmax = w.pmax; epi.psum = w.psum;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 1, epi, 1, 0, stream);
+  if (rc < 0) return rc;
+  ce_reduce_kernel<<<(unsigned)((M + 127) / 128), 128, 0, stream>>>(w.pmax, w.psum, nullptr, n_part, M, w.lse, nullptr);
+  RENET_CHECK_LAUNCH("ce_reduce_kernel");
+  // 2. per-row threshold at rank k + L_m of the partial maxima, and the row weights of 1
+  topk_tau_kernel<true><<<(unsigned)M, 256, 0, stream>>>(w.pmax, w.lse, nullptr, n_part, 1, M, k, w.tau, xb, xe, ones);
+  RENET_CHECK_LAUNCH("topk_tau_kernel");
+  // 3. every p >= tau, excluded columns included
+  EpiArgs sel{};
+  sel.lse = w.lse; sel.row_w = ones; sel.tau = w.tau; sel.sel_count = w.count; sel.sel_val = w.cand_val;
+  sel.sel_idx = w.cand_idx; sel.sel_R = 1; sel.sel_cap = capacity;
+  rc = umma_gemm_prepacked_ex(X, nullptr, K, w.Wp, nullptr, 0, bias, M, N, K, false, 1, 0, 0, 0, 5, sel, 1, 0, stream);
+  if (rc < 0) return rc;
+  // 4. the k best admissible candidates of each row, p descending
+  int sort_n = 2;
+  while (sort_n < k) sort_n <<= 1;
+  topk_final_kernel<true><<<(unsigned)M, kTopkFinalThreads, (size_t)sort_n * 8, stream>>>(
+      w.cand_val, w.cand_idx, w.count, capacity, k, RENET_TOPK_ORDER_VALUE, sort_n, values, indices, needed, excl_col, xb, xe);
   RENET_CHECK_LAUNCH("topk_final_kernel");
   return RENET_OK;
 }

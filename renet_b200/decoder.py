@@ -9,6 +9,8 @@ the forward pass.  ``nn.Linear`` modules stay the parameter holders (state_dict 
 
 ``decoder_group_topk(x, weight, bias, row_weight, R, k)`` is the test-time roll-over's candidate scoring on the same engine
 (renet_decoder_group_topk): per group of R rows, the k largest row_weight * softmax(F.linear(x, weight, bias)) entries.
+``decoder_topk(x, weight, bias, k, exclude)`` is the forecast's scoring (renet_decoder_topk): per row the k largest
+softmax entries outside the row's exclusion list.
 
 ``decoder_rank(x, weight, bias, label, exclude)`` is the test-time scoring on the same engine (renet_decoder_rank): per row
 the cross-entropy loss and the label's raw and filtered ranks by the reference's tie rule (model.py:373-379, 403-418).
@@ -138,6 +140,44 @@ def decoder_group_topk(x, weight, bias, row_weight, R, k, order=ORDER_INDEX, cap
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         _lib.check(L.renet_decoder_group_topk(P(x), P(weight), P(bias), P(row_weight), G, R, N, K, k, order, cap, P(values),
                                               P(indices), P(needed), P(ws), nbytes, _lib.stream()), 'renet_decoder_group_topk')
+        need = int(needed.item())
+        if need == 0:
+            return values, indices.long()
+        cap = need
+
+
+def decoder_topk(x, weight, bias, k, exclude=None, capacity=None):
+    """renet_decoder_topk: for p = softmax(x @ weight^T + bias) over all columns, per row m the k largest p[m, n] over the
+    columns n not in row m's exclusion list, p descending with ties to the lower column.  ``exclude`` = (col, begin, end)
+    as in decoder_rank_counts, or None.  Returns (values float32 [M, k], indices int64 [M, k]); a row with fewer than k
+    admissible columns gets index -1 and value 0 in its last slots.  ``capacity``: the first candidate-buffer size per row
+    (a row that finds more candidates makes the call run once more with the size it reported)."""
+    L, P = _lib.lib(), _lib.ptr
+    _lib.require_cuda(x, weight, bias)
+    x, weight = x.contiguous(), weight.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    M, K = x.shape
+    N = weight.shape[0]
+    col = begin = end = None
+    longest = 0
+    if exclude is not None:
+        col, begin, end = (t.to(torch.int32).contiguous() for t in exclude)
+        _lib.require_cuda(col, begin, end)
+        if begin.numel() != M or end.numel() != M:
+            raise ValueError('decoder_topk: exclusion ranges need one (begin, end) per row')
+        longest = int((end - begin).max()) if M else 0
+    dev = x.device
+    values = torch.empty(M, k, device=dev)
+    indices = torch.empty(M, k, dtype=torch.int32, device=dev)
+    needed = torch.zeros(1, dtype=torch.int32, device=dev)
+    # a row's candidates include its excluded columns: the first buffer allows for the longest list
+    cap = int(capacity) if capacity is not None else group_topk_capacity(k + longest, N)
+    cap = max(cap, k)
+    while True:
+        nbytes = int(L.renet_decoder_topk_workspace_bytes(M, N, K, cap))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _lib.check(L.renet_decoder_topk(P(x), P(weight), P(bias), P(col), P(begin), P(end), M, N, K, k, cap, P(values),
+                                        P(indices), P(needed), P(ws), nbytes, _lib.stream()), 'renet_decoder_topk')
         need = int(needed.item())
         if need == 0:
             return values, indices.long()

@@ -193,6 +193,23 @@ def rank_counts_torch(z, label, exclude=None):
     return out
 
 
+def topk_excluding_torch(z, k, exclude=None):
+    """What renet_decoder_topk returns, on materialised logits z [M, N] with torch: per row the k largest p =
+    softmax(z) over the columns outside row m's list col[begin[m]:end[m]] of ``exclude`` = (col, begin, end), by a stable
+    descending sort (ties to the lower column; torch.topk leaves their order undefined); (values [M, k], indices int64
+    [M, k]), index -1 and value 0 past a row's admissible columns."""
+    p = torch.softmax(z, dim=1)
+    key = p.clone()
+    if exclude is not None:
+        col, begin, end = (torch.as_tensor(a).long().cpu() for a in exclude)
+        for m in range(len(z)):
+            key[m, col[begin[m]:end[m]].to(z.device)] = -1.0         # below every probability
+    order = torch.sort(key, dim=1, descending=True, stable=True).indices[:, :k]
+    keep = torch.gather(key, 1, order) >= 0
+    values = torch.where(keep, torch.gather(p, 1, order), torch.zeros((), dtype=p.dtype, device=p.device))
+    return values, torch.where(keep, order, torch.full((), -1, dtype=torch.long, device=p.device))
+
+
 class RENetInference:
     #: model.py:279,290 re-bind the local names ``s`` / ``o`` inside the roll-over loops, so the FIRST triple scored after
     #: every timestamp change is scored (and its loss taken) with the last subject / object candidate instead of its own
@@ -660,21 +677,22 @@ class RENetInference:
             out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
         return out
 
-    def _eval_shard(self, process_group):
-        """The parallel.Shard evaluate_stream_batched runs on, or None to run unsharded."""
+    def _eval_shard(self, process_group, caller='evaluate_stream_batched'):
+        """The parallel.Shard evaluate_stream_batched (or forecast, named by ``caller`` in errors) runs on, or None to run
+        unsharded."""
         if process_group is None:
             return None
         import torch.distributed as dist
         from .parallel import Shard
         if not (dist.is_available() and dist.is_initialized()):
-            raise ValueError('evaluate_stream_batched: process_group given, but torch.distributed is not initialised')
+            raise ValueError('%s: process_group given, but torch.distributed is not initialised' % caller)
         if dist.get_rank(process_group) < 0:
-            raise ValueError('evaluate_stream_batched: this process is not a member of process_group')
+            raise ValueError('%s: this process is not a member of process_group' % caller)
         if dist.get_world_size(process_group) == 1:
             return None
         if dist.get_backend(process_group) == 'nccl' and not self.ent_embeds.is_cuda:
-            raise ValueError('evaluate_stream_batched: an NCCL process_group needs the model on a GPU; a model on the host '
-                             'takes a gloo group')
+            raise ValueError('%s: an NCCL process_group needs the model on a GPU; a model on the host takes a gloo group'
+                             % caller)
         return Shard(process_group, self.ent_embeds.device)
 
     def _check_ranks_agree(self, shard, test_data, n_hist, total_data, raw, time_aware):
@@ -822,4 +840,122 @@ class RENetInference:
         enc = torch.cat(parts)
         out[torch.from_numpy(sel).to(dev)] = enc[torch.from_numpy(inverse.reshape(-1)).to(dev)]
         return out
+
+    # ---- forecasting ------------------------------------------------------------------------------------------------
+    def forecast(self, queries, global_model, k=10, subject=True, known=None, time_aware=False, process_group=None):
+        """The model's k most likely answers of each query, over its own test-time state as predict keeps it.
+
+        ``queries``: int64 [n, 3] rows (entity, relation, timestamp), timestamps non-decreasing and not before
+        ``latest_time``.  ``subject=True`` asks for the objects of (e, r, ?, t): the rows [ent_e | s_h(e, r) | rel_r]
+        predict builds for its object scores; ``False`` for the subjects of (?, r, e, t), from the object-side history and
+        the inverse relation embeddings.  Returns (values float32 [n, k], entity ids int64 [n, k]) on the model's device,
+        values p = softmax over all entities, descending, ties to the lower id.
+
+        For each run of equal timestamps the stream rolls over as evaluate_stream_batched rolls it (the same _roll_over: the
+        same histories, caches, graph_dict, global_emb, latest_time and torch RNG stream afterwards), then the run's
+        queries are encoded in one batched pass and scored by one renet_decoder_topk call.  Each query is scored as itself
+        (``reference_rebinding`` is an evaluation quirk and does not apply).  A query's history is empty, and its s_h zero,
+        when its entity's test-time history is: unlike predict, a forecast has no ground-truth history of the caller's to
+        consult.
+
+        ``known``: triples (or quadruples) whose answers are left out of the lists -- every answer known for (e, r), or with
+        ``time_aware=True`` (quadruples) only those known at the query's own timestamp.  The excluded answers stay in the
+        softmax's normaliser, so a value is the model's probability of its answer; a query with fewer than k admissible
+        answers gets id -1 and value 0 in its last slots.
+
+        ``process_group``: sharded as evaluate_stream_batched shards -- roll-over and encoding chunks round-robin,
+        contiguous row slices of each top-k call, each rank building its own rows' lists -- and every rank returns the
+        one-process result bit for bit (a row's top-k depends on that row alone).  Ranks called with different arguments
+        raise ValueError.
+
+        A model on the host takes the same control flow with _encode_one per query, materialised logits and a stable
+        sort (topk_excluding_torch)."""
+        from .decoder import TOPK_MAX_K
+        q = torch.as_tensor(queries)
+        if q.dim() != 2 or q.shape[1] != 3 or q.dtype.is_floating_point:
+            raise ValueError('forecast: queries must be integer rows (entity, relation, timestamp), got %s %s'
+                             % (tuple(q.shape), q.dtype))
+        q = q.cpu().long()
+        qn = q.numpy()
+        n = len(qn)
+        if not 1 <= k <= min(self.in_dim, TOPK_MAX_K):
+            raise ValueError('forecast: k = %d outside [1, %d]' % (k, min(self.in_dim, TOPK_MAX_K)))
+        if n and (qn[:, 0].min() < 0 or qn[:, 0].max() >= self.in_dim):
+            raise ValueError('forecast: entity ids outside [0, %d)' % self.in_dim)
+        if n and (qn[:, 1].min() < 0 or qn[:, 1].max() >= self.num_rels):
+            raise ValueError('forecast: relation ids outside [0, %d)' % self.num_rels)
+        if n and (np.any(np.diff(qn[:, 2]) < 0) or qn[0, 2] < int(self.latest_time)):
+            raise ValueError('forecast: timestamps must be non-decreasing and not before latest_time = %d'
+                             % int(self.latest_time))
+        if time_aware and known is None:
+            raise ValueError('forecast: time_aware needs known quadruples (s, r, o, t)')
+        shard = self._eval_shard(process_group, 'forecast')
+        if shard is not None:
+            import hashlib
+            digest = int.from_bytes(hashlib.blake2b(np.ascontiguousarray(qn).tobytes(), digest_size=7).digest(), 'little')
+            fp = [n, digest, int(self.latest_time), int(self.num_k), int(k), int(bool(subject)), int(bool(time_aware)),
+                  -1 if known is None else len(known)]
+            if not shard.same_everywhere(fp):
+                raise ValueError('forecast: the ranks of process_group were called with different queries, latest_time, '
+                                 'num_k, k or flags')
+        self._trim_test_histories()
+        index = None
+        if known is not None:
+            index = TimeFilterIndex(_quadruples(known)) if time_aware else FilterIndex(known)
+        dev = self.ent_embeds.device
+        direction = 'objects' if subject else 'subjects'
+        col = None
+        if index is not None:
+            col = index.col(direction)
+            if self.ent_embeds.is_cuda:
+                col = torch.from_numpy(col).to(dev)                  # once per call; each run sends its ranges
+        rel_embeds, _ = self._direction(subject)
+        hist = self.s_hist_test if subject else self.o_hist_test
+        values = torch.empty(n, k, device=dev)
+        ids = torch.empty(n, k, dtype=torch.long, device=dev)
+        with torch.no_grad():
+            i0 = 0
+            while i0 < n:
+                i1 = i0 + 1
+                while i1 < n and qn[i1, 2] == qn[i0, 2]:
+                    i1 += 1
+                t = q[i0, 2]
+                if self.latest_time != t:
+                    self._roll_over(t, global_model, shard)
+                e, r = qn[i0:i1, 0], qn[i0:i1, 1]
+                has = np.asarray([len(hist[x]) != 0 for x in e], dtype=bool)
+                s_h = self._encode_queries(e, r, has, subject, shard)
+                x = torch.cat((self.ent_embeds[torch.from_numpy(e).to(dev)], s_h, rel_embeds[torch.from_numpy(r).to(dev)]),
+                              dim=1)
+                # a row's top-k depends on that row alone (no split-K, no kernel choice by row count, per-row steps after
+                # the GEMM), so a shard scores a contiguous slice of the rows with the lists of its rows only
+                m = i1 - i0
+                lo, hi = (0, m) if shard is None else shard.slice(m)
+                exclude = None
+                if index is not None:
+                    key = (e[lo:hi], r[lo:hi]) + ((np.full(hi - lo, int(t)),) if time_aware else ())
+                    exclude = (col,) + index.ranges(direction, *key)
+                v, c = self._topk_rows(x[lo:hi], k, exclude)
+                if shard is not None:
+                    v, c = shard.allgather_slices(v, m), shard.allgather_slices(c, m)
+                values[i0:i1], ids[i0:i1] = v, c
+                i0 = i1
+        return values, ids
+
+    def _topk_rows(self, x, k, exclude):
+        """(values [M, k], ids int64 [M, k]) of the rows of x against ``linear`` with the exclusion lists ``exclude`` =
+        (col, begin, end) or None: one renet_decoder_topk call on the GPU; on the host, row by row through ``linear`` as
+        predict computes them, then topk_excluding_torch."""
+        from .decoder import decoder_topk
+        dev = x.device
+        if len(x) == 0:                  # a shard without rows: the empty results keep the dtypes the all-gather needs
+            return torch.zeros(0, k, device=dev), torch.zeros(0, k, dtype=torch.long, device=dev)
+        if x.is_cuda:
+            ex = None
+            if exclude is not None:
+                ex = (exclude[0],) + tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev)
+                                           for a in exclude[1:])
+            return decoder_topk(x, self.linear.weight, self.linear.bias, k, ex)
+        z = torch.stack([self.linear(row) for row in x])
+        return topk_excluding_torch(z, k, exclude)
 
