@@ -225,9 +225,9 @@ def rgcn_block_layer(H, W, Wloop, src, dst, etype, norm, relu, num_bases):
         w = W[etype].view(-1, nb, si, so)                      # RGCN.py:81-85
         x = H[src].view(-1, nb, si)                            # RGCN.py:86
         msg = torch.einsum('ebi,ebij->ebj', x, w).reshape(-1, dout)   # RGCN.py:87
-        agg = torch.zeros(N, dout, dtype=H.dtype).index_add(0, dst, msg)  # fn.sum, RGCN.py:91
+        agg = torch.zeros(N, dout, dtype=H.dtype, device=H.device).index_add(0, dst, msg)  # fn.sum, RGCN.py:91
     else:
-        agg = H if din == dout else torch.zeros(N, dout, dtype=H.dtype)  # DGL 0.4: reduce skipped
+        agg = H if din == dout else torch.zeros(N, dout, dtype=H.dtype, device=H.device)  # DGL 0.4: reduce skipped
     out = agg * norm.view(-1, 1)                               # RGCN.py:93-94
     if Wloop is not None:
         out = out + H @ Wloop                                  # RGCN.py:35,45-46
@@ -361,8 +361,8 @@ def renet_forward(params, triplets, hist, hist_t, graph_dict, global_emb, subjec
     s_q = gru_final_hidden_batched(X3, bh.seq_len, P['encoder_r.weight_ih_l0'], P['encoder_r.weight_hh_l0'],
                                    P['encoder_r.bias_ih_l0'], P['encoder_r.bias_hh_l0'])
     B, h = len(s), ent.shape[1]
-    s_h_pad = torch.cat((s_h, torch.zeros(B - len(s_h), h)), dim=0)     # model.py:88
-    s_q_pad = torch.cat((s_q, torch.zeros(B - len(s_q), h)), dim=0)     # model.py:96
+    s_h_pad = torch.cat((s_h, s_h.new_zeros(B - len(s_h), h)), dim=0)   # model.py:88
+    s_q_pad = torch.cat((s_q, s_q.new_zeros(B - len(s_q), h)), dim=0)   # model.py:96
     ob_pred = torch.cat((ent[s_tem], s_h_pad, rel[r_tem]), dim=1) @ P['linear.weight'].t() + P['linear.bias']
     loss_sub = torch.nn.functional.cross_entropy(ob_pred, o_tem)         # model.py:89-91
     ob_pred_r = torch.cat((ent[s_tem], s_q_pad), dim=1) @ P['linear_r.weight'].t() + P['linear_r.bias']

@@ -53,6 +53,18 @@ class _PackInputsFn(torch.autograd.Function):
         return dH2, dent, drel, dglob, None, None, None, None
 
 
+def _require_edges(hb):
+    """Reject a batch whose history graph has no edge at all.  Histories drawn from the graph dict never give one (each
+    history entry is an event of the subject in that timestamp's graph); with no edge DGL would pass h through both layers
+    unchanged, which the fused encoder does not implement.  Waits for the device batcher's edge count only when the host
+    could not show an edge (BatchedHistoryGraph.has_edge)."""
+    g = hb.graph
+    if not g.has_edge and g.E == 0:
+        raise ValueError('RGCNAggregator: the batch\'s history graph has no edge -- the histories do not match graph_dict '
+                         '(each history entry must be an event of its subject in that timestamp\'s graph)')
+    return hb
+
+
 class RGCNAggregator(nn.Module):
     def __init__(self, h_dim, dropout, num_nodes, num_rels, num_bases, model, seq_len=10):
         super(RGCNAggregator, self).__init__()
@@ -70,6 +82,9 @@ class RGCNAggregator(nn.Module):
 
     # ---------------------------------------------------------------------------------------------
     def _batch(self, s_hist, s, graph_dict, device, sort):
+        return _require_edges(self._assemble(s_hist, s, graph_dict, device, sort))
+
+    def _assemble(self, s_hist, s, graph_dict, device, sort):
         from .hoststore import GraphStore, HistoryView, assemble_view, view_from_lists
         from .utils import HistoryBatch
         if isinstance(s_hist, HistoryBatch):         # already assembled and uploaded (hoststore.prefetch)

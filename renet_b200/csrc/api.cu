@@ -2,7 +2,9 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include <atomic>
+#include <mutex>
 #include <string.h>
+#include <vector>
 
 #include "common.cuh"
 
@@ -119,6 +121,69 @@ __global__ void prepare_sequences_kernel(const int64_t* __restrict__ triplets, i
   }
   if (i < S) row_graph[i] = comp_graph[row_comp[i]];
 }
+
+// renet_encode_fwd's fork / join: one side stream per device, one event pair per (device, caller stream), so that calls on
+// several devices, or from several host threads on their own streams, never record or wait on another call's event.  The
+// pair table is bounded like stream_block's; an entry is only dropped while no call holds it (busy == 0), and dropping it
+// needs no synchronisation (cudaEventDestroy releases a pending event once it completes).
+struct EncodeFork {
+  int device;
+  cudaStream_t caller;
+  cudaEvent_t fork, join;
+  int busy;
+};
+std::mutex g_fork_mu;
+std::vector<cudaStream_t> g_side;       // indexed by device
+std::vector<EncodeFork> g_forks;
+constexpr int kMaxForks = 8;
+
+int fork_acquire(cudaStream_t caller, cudaStream_t* side, cudaEvent_t* fork, cudaEvent_t* join) {
+  std::lock_guard<std::mutex> lk(g_fork_mu);
+  int dev = 0;
+  RENET_CHECK_CUDA(cudaGetDevice(&dev));
+  if ((int)g_side.size() <= dev) g_side.resize(dev + 1, nullptr);
+  if (g_side[dev] == nullptr) RENET_CHECK_CUDA(cudaStreamCreateWithFlags(&g_side[dev], cudaStreamNonBlocking));
+  EncodeFork* f = nullptr;
+  for (auto& e : g_forks)
+    if (e.device == dev && e.caller == caller) f = &e;
+  if (f == nullptr) {
+    if ((int)g_forks.size() >= kMaxForks) {
+      for (size_t i = 0; i < g_forks.size(); ++i)
+        if (g_forks[i].busy == 0) {            // the oldest idle entry
+          cudaEventDestroy(g_forks[i].fork);
+          cudaEventDestroy(g_forks[i].join);
+          g_forks.erase(g_forks.begin() + i);
+          break;
+        }
+    }
+    EncodeFork e{dev, caller, nullptr, nullptr, 0};
+    RENET_CHECK_CUDA(cudaEventCreateWithFlags(&e.fork, cudaEventDisableTiming));
+    RENET_CHECK_CUDA(cudaEventCreateWithFlags(&e.join, cudaEventDisableTiming));
+    g_forks.push_back(e);
+    f = &g_forks.back();
+  }
+  ++f->busy;
+  *side = g_side[dev];
+  *fork = f->fork;
+  *join = f->join;
+  return RENET_OK;
+}
+
+void fork_release(cudaStream_t caller) {
+  std::lock_guard<std::mutex> lk(g_fork_mu);
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return;
+  for (auto& e : g_forks)
+    if (e.device == dev && e.caller == caller && e.busy > 0) --e.busy;
+}
+
+struct ForkLease {
+  cudaStream_t caller;
+  bool held = false;
+  ~ForkLease() {
+    if (held) fork_release(caller);
+  }
+};
 }  // namespace
 }  // namespace renet
 
@@ -464,23 +529,25 @@ int renet_encode_fwd(const float* ent, const int32_t* node_ent, const int32_t* r
                      int32_t n_hot, void* workspace, int64_t workspace_bytes, void* stream) {
   RENET_CHECK_ARG(n_hot >= 0 && (n_hot == 0 || hot_rel != nullptr), "renet_encode_fwd: bad hot-relation list");
   if (n_hot == 0) hot_rel = nullptr;
+  // a history graph without edges would pass h through both layers (DGL); layer 2 runs on the read-out sub-graph, where
+  // that pass-through is not implemented, so such a batch is refused (RGCNAggregator rejects it before it gets here)
+  RENET_CHECK_ARG(N == 0 || E > 0, "renet_encode_fwd: the history graph has no edges");
   // The part of the GRU that does not depend on the RGCN output -- weight packing, bias rows, the per-sequence and
   // per-timestamp input projections: four small launches, latency-bound, a handful of CTAs -- runs on a side stream
-  // underneath the two RGCN layers (fork / join by events; the side stream and its events are created on first use and
-  // live for the process: one device, one caller stream at a time, as everywhere in this library).
-  static cudaStream_t side = nullptr;
-  static cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  // underneath the two RGCN layers (fork / join by events: the side stream is the device's, the event pair the caller
+  // stream's, both created on first use, fork_acquire).
+  cudaStream_t side = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  ForkLease lease{(cudaStream_t)stream};
   const bool gru_args_ok = S > 0 && Q > 0 && readout && row_glob && glob && rel && seq_s && seq_r && seq_len && seq_start &&
                            host_batch_sizes && w_ih4 && w_hh4 && b_ih4 && b_hh4 && w_ih3 && w_hh3 && b_ih3 && b_hh3 && hn4 && hn3 &&
                            workspace && workspace_bytes >= renet_gru_workspace_bytes(S, Q, T, h) &&
                            (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && max_len >= 0 && T >= 0;
   bool forked = false;
   if (gru_args_ok) {
-    if (side == nullptr) {
-      RENET_CHECK_CUDA(cudaStreamCreateWithFlags(&side, cudaStreamNonBlocking));
-      RENET_CHECK_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
-      RENET_CHECK_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-    }
+    const int rc0 = fork_acquire((cudaStream_t)stream, &side, &ev_fork, &ev_join);
+    if (rc0) return rc0;
+    lease.held = true;
     RENET_CHECK_CUDA(cudaEventRecord(ev_fork, (cudaStream_t)stream));
     RENET_CHECK_CUDA(cudaStreamWaitEvent(side, ev_fork, 0));
     int rc1 = launch_gru_fwd(nullptr, readout, row_glob, glob, ent, rel, seq_s, seq_r, seq_len, seq_start, host_batch_sizes, max_len,
@@ -512,7 +579,7 @@ int renet_encode_fwd(const float* ent, const int32_t* node_ent, const int32_t* r
         rc = sgemm_nn(H1, sub_uniq, h, Wloop2, h, H2, h, nullptr, S, h, h, false, (cudaStream_t)stream);
         if (rc) return rc;
       }
-      rc = launch_rgcn_gather(H1, nullptr, W2, sub_row_ptr, sub_col_src, sub_col_type, sub_norm, H2, S, E > 0 ? E : 1, h, h,
+      rc = launch_rgcn_gather(H1, nullptr, W2, sub_row_ptr, sub_col_src, sub_col_type, sub_norm, H2, S, E, h, h,
                               num_bases, 0, Wloop2 != nullptr, (cudaStream_t)stream, R2, hot_rel, n_hot);
       if (rc) return rc;
     }

@@ -167,6 +167,7 @@ class BatchedHistoryGraph:
     _E = None
     _E_pending = None       # PendingCount of the asynchronous read-back (device-assembled batches)
     E_cap = None            # capacity of the col_* arrays (>= E); launch argument while E is still in flight
+    has_edge = False        # E >= 1 is known on the host without waiting for E (hoststore._first_entry_has_edge)
 
     @property
     def E(self):

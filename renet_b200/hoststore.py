@@ -404,6 +404,24 @@ def _fill(hb, view, r, d, h, csr, device):
     return g
 
 
+def _first_entry_has_edge(view):
+    """True when the batch's first history entry shows, on the host, that the batched graph has an edge: its subject has an
+    in-edge from one of that entry's neighbours in the entry's graph.  Histories drawn from the graph dict always show one
+    (every neighbour is the other end of an event with the subject), so the edge count, which the device batcher produces
+    asynchronously, need not be waited for."""
+    hs, gs = view.store, view.store.gs
+    so = hs.samp_off
+    nz = np.flatnonzero(so[view.sample_idx + 1] > so[view.sample_idx])
+    if len(nz) == 0:
+        return False
+    e = hs.samp_entry[so[view.sample_idx[nz[0]]]]
+    gi, s = int(hs.ent_graph[e]), int(hs.ent_srow[e])
+    lo, hi = int(gs.edge_off[gi]), int(gs.edge_off[gi + 1])
+    dst = gs.dst[lo:hi]                                   # a graph's edges are sorted by destination
+    a, b = np.searchsorted(dst, s), np.searchsorted(dst, s, 'right')
+    return bool(np.isin(gs.src[lo + a:lo + b], hs.nbr_row[hs.ent_off[e]:hs.ent_off[e + 1]]).any())
+
+
 def _upload_plan(hb, view, buf, r, device):
     """Device part of the device batcher (caller's thread / current stream): one pinned H2D copy of the plan, then
     renet_induce_edges builds the CSR on the GPU from the resident graph store; the edge count comes back
@@ -441,6 +459,7 @@ def _upload_plan(hb, view, buf, r, device):
         _lib.check(rc, 'renet_induce_edges')
     g = _fill(hb, view, r, d, h, parts, device)
     g.E_cap = E_cand
+    g.has_edge = _first_entry_has_edge(view)
     g._keep = (blob, dev)
     with torch.cuda.stream(ls):
         rev = getattr(view.store, 'reverse', None)

@@ -359,3 +359,31 @@ def test_graph_store_rejects_negative_edge_types():
     for ts, to in (([-1], [1]), ([0], [-1])):
         with pytest.raises(ValueError):
             hoststore.GraphStore({0: HistoryGraph([3, 5], [0], [1], ts, to)})
+
+
+def test_first_history_entry_shows_an_edge():
+    """hoststore._first_entry_has_edge: True on histories drawn from the graph dict (the device batcher then never waits for
+    its edge count to reject an edge-free batch), False when the first entry's neighbours are not the subject's neighbours
+    in that timestamp's graph, and False for a batch of empty histories."""
+    from renet_b200 import hoststore
+    quads, num_e, num_r = synthetic.make_quads('icews18', seed=5, num_timestamps=12)
+    S, ST, O, OT = synthetic.build_history(quads)
+    gs = hoststore.GraphStore(synthetic.build_graph_dict(quads, num_r))
+    rng = np.random.RandomState(2)
+    late = np.arange(len(quads) // 2, len(quads))
+    for col, (hist, hist_t) in ((0, (S, ST)), (2, (O, OT))):
+        store = hoststore.HistoryStore(hist, hist_t, quads[:, col], gs)
+        lens = np.diff(store.samp_off)
+        for _ in range(20):
+            sel = rng.choice(late, 64)
+            assert hoststore._first_entry_has_edge(store.select(sel)) == bool(lens[sel].any())
+        assert not hoststore._first_entry_has_edge(store.select(np.flatnonzero(lens == 0)[:5]))
+    # a history whose neighbour shares the subject's timestamp graph but no edge with it
+    t = int(quads[0, 3])
+    g = gs[t]
+    ents = np.asarray(g.node_id if hasattr(g, 'node_id') else g.id)
+    s = int(quads[0, 0])
+    linked = set(quads[(quads[:, 3] == t) & (quads[:, 0] == s), 2]) | set(quads[(quads[:, 3] == t) & (quads[:, 2] == s), 0])
+    other = next(int(e) for e in ents if int(e) != s and int(e) not in linked)
+    bogus = hoststore.HistoryStore([[np.asarray([[0, other]], dtype=np.int64)]], [[t]], [s], gs, dedupe=False)
+    assert not hoststore._first_entry_has_edge(bogus.select([0]))
