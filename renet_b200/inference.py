@@ -30,6 +30,34 @@ ROLLOVER_SEQ_BUDGET = 16384
 EVAL_PLAN_BUDGET = 1 << 28
 
 
+#: rows evaluate_observed ranks per renet_decoder_rank_multi call (two per triple): 16 384 rows of [ent | h | rel] at
+#: h = 200 are 39 MB, and the call's per-row lists stay a few MB
+OBSERVED_RANK_ROWS = 16384
+
+
+def _isolated_view(hist, hist_t, subjects, samples, groups, graph_dict):
+    """A HistoryView over a store of the histories hist / hist_t (one entry each, all non-empty, of subjects[i]) that
+    selects ``samples`` (positions in hist), sample j in isolation group groups[j], over a GraphStore of the timestamps
+    those histories reference.  Returns (view, graph store)."""
+    from .hoststore import GraphStore, HistoryStore
+    times = sorted({int(t) for ht in hist_t for t in ht})
+    gs = GraphStore({t: graph_dict[t] for t in times})
+    store = HistoryStore(list(hist), list(hist_t), np.asarray(subjects, dtype=np.int64), gs, dedupe=False)
+    return store.select(np.asarray(samples, dtype=np.int64), groups=groups), gs
+
+
+def _chunk_view(hist, hist_t, q_h, q_e, graph_dict):
+    """The grouped view of one chunk of queries: query k has history hist[q_h[k]] / hist_t[q_h[k]] of entity q_e[k].  One
+    store entry per distinct history, one isolation group per entity, so the batched graph's components are the distinct
+    (entity, timestamp) pairs of the chunk.  Returns (view, graph store)."""
+    uh, pos = np.unique(q_h, return_inverse=True)
+    ue = np.zeros(len(uh), dtype=np.int64)
+    ue[pos] = q_e
+    group = np.unique(ue, return_inverse=True)[1].reshape(-1)
+    return _isolated_view([hist[x] for x in uh], [hist_t[x] for x in uh], ue, pos.reshape(-1), group[pos.reshape(-1)],
+                          graph_dict)
+
+
 def rank_with_ties(scores, label):
     """model.py:373-379: rank = #(strictly greater) + (#equal - 1)/2 + 1."""
     ref = scores[label]
@@ -267,15 +295,17 @@ class RENetInference:
         R = self.num_rels
         return (self.rel_embeds[:R], False) if subject else (self.rel_embeds[R:], True)
 
-    def _encode_one(self, entity, r, history, history_t, subject):
+    def _encode_one(self, entity, r, history, history_t, subject, graph_dict=None, global_emb=None):
         """Final hidden state of `encoder` for ONE (entity, relation) history (aggregator.predict + encoder,
-        model.py:333-351)."""
+        model.py:333-351), over the model's graph_dict / global_emb unless others are given."""
         rel_embeds, reverse = self._direction(subject)
         dev = self.ent_embeds.device
         e = torch.as_tensor(entity, device=dev).view(1)
         rr = torch.as_tensor(r, device=dev).view(1)
-        s_h, _, _ = self.aggregator.encode(([history], [history_t]), e, rr, self.ent_embeds, rel_embeds, self.graph_dict,
-                                           self.global_emb, reverse, self.encoder, self.encoder_r)
+        s_h, _, _ = self.aggregator.encode(([history], [history_t]), e, rr, self.ent_embeds, rel_embeds,
+                                           self.graph_dict if graph_dict is None else graph_dict,
+                                           self.global_emb if global_emb is None else global_emb, reverse, self.encoder,
+                                           self.encoder_r)
         return s_h.view(-1)
 
     def pred_r_rank2(self, s, r, subject=True):
@@ -306,14 +336,11 @@ class RENetInference:
         """A HistoryView over the current test-time histories of ``entities`` (all non-empty): one store entry per entity,
         the view's samples = ``samples`` (positions in ``entities``), each sample isolated in the group of its entity, over
         a GraphStore of the timestamps those histories reference.  Returns (view, graph store)."""
-        from .hoststore import GraphStore, HistoryStore
         hist = self.s_hist_test if subject else self.o_hist_test
         hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
-        times = sorted({int(t) for e in entities for t in hist_t[e]})
-        gs = GraphStore({t: self.graph_dict[t] for t in times})
-        store = HistoryStore([hist[e] for e in entities], [hist_t[e] for e in entities], entities, gs, dedupe=False)
         samples = np.asarray(samples, dtype=np.int64)
-        return store.select(samples, groups=samples), gs
+        return _isolated_view([hist[e] for e in entities], [hist_t[e] for e in entities], entities, samples, samples,
+                              self.graph_dict)
 
     def pred_r_topk(self, entities, weights, k, subject=True, capacity=None):
         """pred_r_rank2 followed by torch.topk for many entities at once (model.py:168-213, 236-240).  For entity
@@ -677,6 +704,122 @@ class RENetInference:
             out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
         return out
 
+    def evaluate_observed(self, test_data, s_history, o_history, graph_dict, global_emb, total_data=None, raw=False,
+                          time_aware=False):
+        """Evaluation over observed history ("RE-Net w. GT"): every test triple (s, r, o, t) is encoded from its own
+        ground-truth histories ``s_history`` / ``o_history`` = (lists, timestamp lists) per triple, as evaluate_stream takes
+        them, over the true graphs ``graph_dict`` (e.g. synthetic.build_graph_dict of every known quadruple, a GraphStore,
+        or the reference's dict) and the global embeddings ``global_emb`` of the timestamps those histories reference.
+        Returns evaluate_stream_batched's result dict (``protocols`` with ``time_aware``, the top-level keys following
+        ``raw``).
+
+        Per triple: s_h = encoder(aggregator.predict(s's history, s, r)) (model.py:336-339 with the triple's own history in
+        place of the test-time state), o_h the same on the object side (model.py:346-351), zero rows for empty histories;
+        scores linear([ent | h | rel]) in both directions, ranked with the reference's tie rule raw, filtered
+        (FilterIndex(total_data)) and time-aware filtered (TimeFilterIndex, keyed at the triple's own t); loss = predict's
+        two cross-entropies.  Nothing rolls over and nothing is sampled: the test-time state (histories, caches,
+        graph_dict, global_emb, latest_time) and torch's RNG are left as they are, so the call can run between
+        evaluate_stream calls or inside a training loop.  The model scores in eval mode (no dropout) and its mode is
+        restored.
+
+        No timestamp depends on another, so the whole split is batched: each direction's distinct (entity, relation,
+        history) queries are encoded once, in chunks through the device batcher with one isolation group per entity, whose
+        components are the distinct (entity, history timestamp) pairs; then the rows are ranked OBSERVED_RANK_ROWS at a
+        time by renet_decoder_rank_multi.  This needs the entries of one (entity, timestamp, direction) to be equal in every
+        history that holds them, as histories built from one graph dict are; unequal ones raise ValueError, as do histories
+        whose length differs from the test data's, ids out of range, history timestamps missing from graph_dict or
+        global_emb, and ``time_aware`` without quadruples -- all before any work.  A model on the host takes the same flow
+        through _encode_one and materialised logits."""
+        test_data = torch.as_tensor(test_data)
+        if test_data.dim() != 2 or test_data.shape[1] < 4:
+            raise ValueError('evaluate_observed: test_data must be quadruples (s, r, o, t)')
+        quads = test_data.cpu().numpy().astype(np.int64)
+        n = len(quads)
+        if time_aware:
+            _quadruples(total_data)
+        if (not raw or time_aware) and total_data is None:
+            raise ValueError('filtered evaluation needs total_data (all known triples)')
+        for name, hist in (('s_history', s_history), ('o_history', o_history)):
+            if len(hist) != 2 or len(hist[0]) != n or len(hist[1]) != n:
+                raise ValueError('evaluate_observed: %s must be (lists, timestamp lists) of %d test triples' % (name, n))
+        if n and (min(quads[:, 0].min(), quads[:, 2].min()) < 0 or max(quads[:, 0].max(), quads[:, 2].max()) >= self.in_dim):
+            raise ValueError('evaluate_observed: entity ids outside [0, %d)' % self.in_dim)
+        if n and (quads[:, 1].min() < 0 or quads[:, 1].max() >= self.num_rels):
+            raise ValueError('evaluate_observed: relation ids outside [0, %d)' % self.num_rels)
+        s_obs, has_s = self._observed_histories(quads[:, 0], s_history, 's_history', graph_dict, global_emb)
+        o_obs, has_o = self._observed_histories(quads[:, 2], o_history, 'o_history', graph_dict, global_emb)
+        tfidx = TimeFilterIndex(_quadruples(total_data)) if time_aware else None
+        fidx = FilterIndex(total_data) if not raw or time_aware else None
+        protocols = {k: [] for k in PROTOCOLS}
+        ranks, total_loss = [], 0.0
+        modes = [(mod, mod.training) for mod in self.modules()]
+        self.eval()
+        try:
+            with torch.no_grad():
+                graphs = (graph_dict, global_emb)
+                s_h = self._encode_queries(quads[:, 0], quads[:, 1], has_s, True, history=s_obs, graphs=graphs)
+                o_h = self._encode_queries(quads[:, 2], quads[:, 1], has_o, False, history=o_obs, graphs=graphs)
+                per = max(1, OBSERVED_RANK_ROWS // 2)
+                for i0 in range(0, n, per):
+                    i1 = min(i0 + per, n)
+                    q = quads[i0:i1]
+                    r, loss = self._rank_triples(q, q[:, 0], q[:, 2], s_h[i0:i1], o_h[i0:i1], fidx, tfidx)
+                    if time_aware:
+                        for k in PROTOCOLS:
+                            protocols[k].append(r[k])
+                        r = r['raw' if raw else 'filtered']
+                    ranks.append(r)
+                    total_loss += float(np.sum(loss.astype(np.float64)))
+        finally:
+            for mod, mode in modes:
+                mod.training = mode
+        out = stream_metrics(ranks, total_loss)
+        if time_aware:
+            out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
+        return out
+
+    def _observed_histories(self, ents, history, name, graph_dict, global_emb):
+        """evaluate_observed's histories of one direction, checked: ((hist, hist_t, hid, ent_of), has) -- the distinct
+        histories (lists, timestamp lists), each triple's history id (-1 when empty), the entity of each history, and which
+        triples have one.  A history is identified by its entity and timestamps, since the entries of one (entity, timestamp)
+        must be equal wherever they appear (ValueError otherwise); ids ascend with the entity, as _encode_queries needs.
+        ValueError for entry ids out of range and for timestamps missing from graph_dict or global_emb."""
+        lists, times = history
+        R, E = self.num_rels, self.in_dim
+        seen = {}                                        # (entity, t) -> the first entry seen, as int64 [k, 2]
+        keys = {}                                        # (entity, timestamps) -> first triple holding that history
+        hid = np.full(len(ents), -1, dtype=np.int64)
+        for i, (e, hl, ht) in enumerate(zip(ents.tolist(), lists, times)):
+            if len(hl) != len(ht):
+                raise ValueError('evaluate_observed: %s[%d] has %d entries but %d timestamps' % (name, i, len(hl), len(ht)))
+            if len(hl) == 0:
+                continue
+            ts = tuple(int(t) for t in ht)
+            for a, t in zip(hl, ts):
+                prev = seen.get((e, t))
+                if prev is None:
+                    if t not in graph_dict:
+                        raise ValueError('evaluate_observed: %s[%d] refers to timestamp %d, which graph_dict lacks' % (name, i, t))
+                    if t not in global_emb:
+                        raise ValueError('evaluate_observed: %s[%d] refers to timestamp %d, which global_emb lacks' % (name, i, t))
+                    v = np.asarray(a, dtype=np.int64).reshape(-1, 2)
+                    if len(v) and (v[:, 0].min() < 0 or v[:, 0].max() >= R or v[:, 1].min() < 0 or v[:, 1].max() >= E):
+                        raise ValueError('evaluate_observed: %s[%d] holds ids outside [0, %d) x [0, %d) at timestamp %d'
+                                         % (name, i, R, E, t))
+                    seen[(e, t)] = (a, v)
+                elif prev[0] is not a and not np.array_equal(prev[1], np.asarray(a, dtype=np.int64).reshape(-1, 2)):
+                    raise ValueError('evaluate_observed: %s[%d] holds an entry of entity %d at timestamp %d that differs from '
+                                     'another history\'s entry of the same entity and timestamp' % (name, i, e, t))
+            hid[i] = keys.setdefault((e, ts), i)
+        order = sorted(keys.items())                     # by entity, then timestamps
+        rank = {first: j for j, (_, first) in enumerate(order)}
+        has = hid >= 0
+        hid[has] = [rank[x] for x in hid[has].tolist()]
+        hist = [lists[first] for _, first in order]
+        hist_t = [times[first] for _, first in order]
+        ent_of = np.asarray([e for (e, _), _ in order], dtype=np.int64)
+        return (hist, hist_t, hid, ent_of), has
+
     def _eval_shard(self, process_group, caller='evaluate_stream_batched'):
         """The parallel.Shard evaluate_stream_batched (or forecast, named by ``caller`` in errors) runs on, or None to run
         unsharded."""
@@ -713,10 +856,6 @@ class RENetInference:
         triple is scored with (model.py:279,290) or None; its rank labels and filter keys stay its own.  With a
         TimeFilterIndex ``tfidx`` (and ``fidx``) the ranks are a dict of the three PROTOCOLS, the time-aware keys taking the
         run's timestamp.  With a ``shard`` the encoding and the rank call are sharded over its ranks."""
-        from .decoder import ranks_from_counts
-        R, h = self.num_rels, self.h_dim
-        dev = self.ent_embeds.device
-        n = len(quads)
         s, r, o = quads[:, 0].copy(), quads[:, 1].copy(), quads[:, 2].copy()
         si, oi = s.copy(), o.copy()
         if rebind is not None:
@@ -725,13 +864,27 @@ class RENetInference:
         has_o = ~o_empty & np.asarray([len(self.o_hist_test[e]) != 0 for e in oi], dtype=bool)
         s_h = self._encode_queries(si, r, has_s, True, shard)
         o_h = self._encode_queries(oi, r, has_o, False, shard)
+        return self._rank_triples(quads, si, oi, s_h, o_h, fidx, tfidx, shard)
+
+    def _rank_triples(self, quads, si, oi, s_h, o_h, fidx, tfidx=None, shard=None):
+        """Scores and ranks the triples ``quads`` (s, r, o, t) given their encodings: the object of triple i against
+        [ent[si[i]] | s_h[i] | rel[r]] and its subject against [ent[oi[i]] | o_h[i] | rel_inv[r]].  si / oi equal s / o
+        except at row 0 of a rebound run (_score_run).  Returns (ranks float64 [2n] as [sub, ob] per triple, loss float32 [n]
+        = predict's two cross-entropies per triple); with a TimeFilterIndex ``tfidx`` (and ``fidx``) the ranks are a dict
+        of the three PROTOCOLS, the time-aware key of each row taking its own triple's timestamp.  With a ``shard`` the rank
+        call is sharded over its ranks."""
+        from .decoder import ranks_from_counts
+        R = self.num_rels
+        dev = self.ent_embeds.device
+        n = len(quads)
+        s, r, o, t = (np.ascontiguousarray(quads[:, j]) for j in range(4))
         to_dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(dev)    # noqa: E731
         si_d, oi_d, r_d = to_dev(si), to_dev(oi), to_dev(r)
         x = torch.cat((torch.cat((self.ent_embeds[si_d], s_h, self.rel_embeds[:R][r_d]), dim=1),
                        torch.cat((self.ent_embeds[oi_d], o_h, self.rel_embeds[R:][r_d]), dim=1)), dim=0)
         rank_lab = np.concatenate((o, s))                        # ob rows rank the triple's object, sub rows its subject
         loss_row = np.concatenate((np.arange(n), n + np.arange(n)))
-        if rebind is not None and (si[0] != s[0] or oi[0] != o[0]):
+        if n and (si[0] != s[0] or oi[0] != o[0]):
             # predict's loss for the rebound triple takes the rebound labels: two extra rows carry them
             x = torch.cat((x, x[[0, n]]), dim=0)
             rank_lab = np.concatenate((rank_lab, [oi[0], si[0]]))
@@ -747,7 +900,8 @@ class RENetInference:
             direction = np.concatenate((np.zeros(n, bool), np.ones(n, bool), [False, True]))[:m][lo:hi]
             excludes.append(_exclusion_lists(fidx, direction, fix, rr))
             if tfidx is not None:
-                excludes.append(_exclusion_lists(tfidx, direction, fix, rr, np.full(hi - lo, quads[0, 3])))
+                tt = np.concatenate((t, t, t[:1], t[:1]))[:m][lo:hi]
+                excludes.append(_exclusion_lists(tfidx, direction, fix, rr, tt))
         loss_rows, counts = self._rank_rows(x[lo:hi], rank_lab[lo:hi], excludes)
         if shard is not None:
             loss_rows, counts = shard.allgather_slices(loss_rows, m), shard.allgather_slices(counts, m)
@@ -780,38 +934,50 @@ class RENetInference:
         cs = [rank_counts_torch(z, lab, e) for e in excludes]
         return loss_rows, torch.cat([rank_counts_torch(z, lab)[:, :2]] + [ci[:, 2:] for ci in cs], dim=1)
 
-    def _encode_queries(self, ents, rels, has, subject, shard=None):
-        """s_h [n, h] of the queries (ents[i], rels[i]) against the current test-time histories; rows where ``has`` is
-        False stay zero (predict's empty-history rule).  Equal queries are encoded once.  On the GPU the distinct queries go
-        through the device batcher in chunks, one isolation group per entity, so that each equals _encode_one's encoding
-        of it alone; on the host, through _encode_one, one query per chunk.  With a ``shard`` chunk j runs on rank
-        j mod world and every rank all-gathers the encodings."""
+    def _encode_queries(self, ents, rels, has, subject, shard=None, history=None, graphs=None):
+        """s_h [n, h] of the queries (ents[i], rels[i]); rows where ``has`` is False stay zero (predict's empty-history
+        rule).  Query i's history is the current test-time history of ents[i], or with ``history`` = (hist, hist_t, hid,
+        ent_of) the history hist[hid[i]] / hist_t[hid[i]], whose entity is ent_of[hid[i]] (= ents[i]), over ``graphs`` =
+        (graph_dict, global_emb) instead of the model's.  Equal queries (history, relation) are encoded once.  On the GPU the
+        distinct queries go through the device batcher in chunks, one isolation group per entity, so that each equals
+        _encode_one's encoding of it alone; on the host, through _encode_one, one query per chunk.  With a ``shard`` chunk j
+        runs on rank j mod world and every rank all-gathers the encodings."""
         h, R = self.h_dim, self.num_rels
         dev = self.ent_embeds.device
         out = torch.zeros(len(ents), h, device=dev)
         sel = np.flatnonzero(has)
         if len(sel) == 0:
             return out
-        keys, inverse = np.unique(np.asarray(ents)[sel].astype(np.int64) * R + np.asarray(rels)[sel], return_inverse=True)
-        q_e, q_r = keys // R, keys % R
-        hist = self.s_hist_test if subject else self.o_hist_test
-        hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
+        graph_dict, global_emb = (self.graph_dict, self.global_emb) if graphs is None else graphs
+        if history is None:
+            hist = self.s_hist_test if subject else self.o_hist_test
+            hist_t = self.s_hist_test_t if subject else self.o_hist_test_t
+            hid, ent_of = np.asarray(ents), None
+        else:
+            hist, hist_t, hid, ent_of = history
+        keys, inverse = np.unique(np.asarray(hid)[sel].astype(np.int64) * R + np.asarray(rels)[sel], return_inverse=True)
+        q_h, q_r = keys // R, keys % R                   # history ids ascend with their entity, so keys are sorted by entity
+        q_e = q_h if ent_of is None else np.asarray(ent_of, dtype=np.int64)[q_h]
         if not self.ent_embeds.is_cuda:
             chunks = [(j, j + 1) for j in range(len(keys))]
         else:
             rel_embeds, reverse = self._direction(subject)
+            ent_times = defaultdict(set)                 # the timestamps of every history of each entity
+            for hh, e in zip(*np.unique(np.stack((q_h, q_e), 1), axis=0).T):
+                ent_times[e].update(int(t) for t in hist_t[hh])
             sizes = {}
-            for t in {int(t) for e in np.unique(q_e) for t in hist_t[e]}:
-                g = self.graph_dict[t]
+            for t in set().union(*ent_times.values()):
+                g = graph_dict[t]
                 sizes[t] = g.number_of_nodes() + g.number_of_edges()
             chunks, j0 = [], 0
             while j0 < len(keys):
-                # a chunk: whole entities (keys are sorted by entity), within both budgets
+                # a chunk: whole entities, within both budgets; an entity's components are the distinct timestamps of its
+                # histories
                 cost, j1 = 0, j0
                 while j1 < len(keys) and j1 - j0 < ROLLOVER_SEQ_BUDGET:
                     e = q_e[j1]
                     if j1 == j0 or e != q_e[j1 - 1]:
-                        c = sum(sizes[int(t)] for t in hist_t[e])
+                        c = sum(sizes[t] for t in ent_times[e])
                         if j1 > j0 and cost + c > EVAL_PLAN_BUDGET:
                             break
                         cost += c
@@ -821,14 +987,14 @@ class RENetInference:
         parts = []
         for j0, j1 in (chunks[c] for c in (range(len(chunks)) if shard is None else shard.units(len(chunks)))):
             if not self.ent_embeds.is_cuda:
-                e, rr = int(q_e[j0]), int(q_r[j0])
-                parts.append(self._encode_one(e, rr, hist[e], hist_t[e], subject).view(1, h).to(out.dtype))
+                hh, e, rr = int(q_h[j0]), int(q_e[j0]), int(q_r[j0])
+                parts.append(self._encode_one(e, rr, hist[hh], hist_t[hh], subject, graph_dict, global_emb)
+                             .view(1, h).to(out.dtype))
                 continue
-            ue, pos = np.unique(q_e[j0:j1], return_inverse=True)
-            view, gs = self._grouped_view(ue, pos, subject)
+            view, gs = _chunk_view(hist, hist_t, q_h[j0:j1], q_e[j0:j1], graph_dict)
             s_dev = torch.from_numpy(q_e[j0:j1]).to(dev)
             r_dev = torch.from_numpy(q_r[j0:j1]).to(dev)
-            sh, _, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, self.global_emb,
+            sh, _, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, global_emb,
                                                reverse, self.encoder, self.encoder_r)
             # the encoder returns the sequences length-sorted: row k is sample sample_order[k] of the view
             idx = hb.sample_order(dev)
