@@ -133,13 +133,9 @@ bool gather_use_stream(int64_t E, int64_t N, bool indexed_input) {
 static long long* g_stream_dbg = nullptr;
 void set_stream_debug_buffer(long long* p) { g_stream_dbg = p; }
 
-int stream_cfg_choice() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("RENET_STREAM_CFG");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
+int stream_cfg_choice() {             // read per launch: a test compares hubs on and off in one process
+  const char* e = getenv("RENET_STREAM_CFG");
+  return e ? atoi(e) : 0;
 }
 
 template <bool RELU, bool HAS_LOOP, bool INDEXED, class Cfg>
@@ -174,6 +170,12 @@ static int launch_stream(const float* H, const int32_t* h_index, const float* W,
       default: break;
     }
   }
+  // layer 1 (input rows through an index: a CTA's sources are a few hundred consecutive node ids, half of its edges
+  // come from 64 of them) keeps hub source rows resident; RENET_STREAM_CFG=3 turns them off (A/B measurements, tests:
+  // the results are bitwise the same).  Plain input rows (layer 2's read-out sub-graph) keep 82 relation rows and no hubs:
+  // tools/stream_reuse_model.py counts 27 % fewer L2 bytes per edge there with 49 / 64, which has not been measured
+  if constexpr (INDEXED)
+    if (stream_cfg_choice() != 3) RENET_ST(StHubs);
   RENET_ST(StDefault<false>);
 #undef RENET_ST
 }

@@ -23,6 +23,9 @@
 //     On the H100 the edge loop is bound by what each edge moves from L2 (tools/stream_timeline.py: 74 SM cycles per
 //     edge with cold rows in the ring and 18 resident rows, 61 with 82; the shared-memory work is about 30): so the
 //     ring holds source rows only and the shared memory goes to resident relation rows;
+//   * forward with HUB > 0 (layer 1): part of that memory holds "hub" source rows instead -- the CTA's most frequent
+//     source nodes (star-like timestamp graphs: about half of a CTA's edges come from a few dozen nodes), chosen by a
+//     histogram of its sources in the prologue; an edge from a hub issues no ring copy and reads the resident row;
 //   * the running destination's sum stays in registers (edges are destination-sorted: a segmented reduction); a
 //     destination that starts and ends inside the warp's range goes straight from registers through the fused
 //     norm / self-loop / activation epilogue to global memory; one cut by a warp boundary is handed over through a
@@ -42,31 +45,43 @@ constexpr int kStMaxR2 = 2048;           // relation-id range of the hot-row loo
 constexpr int kStNodeCost = 2;           // a destination (epilogue: self-loop row, norm, 800-byte store) costs about two edges
 constexpr int kStSlot = 800;             // ring slot: one source row (cold relation rows are loaded into registers)
 constexpr int kStHotGroups = 8;          // the resident rows land in 8 groups, one mbarrier each
-// WARPS warps per CTA (>= 16), D edges in flight per warp, HOT relation rows resident per CTA; shared memory map (bytes)
-template <int WARPS, int D, int HOT, bool BWD>
+constexpr int kStHubBins = 2048;         // source-node window of the hub histogram (from the CTA's smallest source node)
+constexpr int kStHubScr = kStMaxR2 + 256 + 16;   // prologue scratch (ints into the ring): hub selection, after cnt + hist
+// WARPS warps per CTA (>= 16), D edges in flight per warp, HOT relation rows and HUB source rows ("hubs": the CTA's most
+// frequent source nodes, forward only) resident per CTA; shared memory map (bytes)
+template <int WARPS, int D, int HOT, bool BWD, int HUB = 0>
 struct StCfg {
-  static constexpr int kWarps = WARPS, kThreads = WARPS * 32, kD = D, kHot = HOT;
+  static constexpr int kWarps = WARPS, kThreads = WARPS * 32, kD = D, kHot = HOT, kHub = HUB;
   static constexpr int kHotPerGroup = (HOT + kStHotGroups - 1) / kStHotGroups;
+  static constexpr int kHubPerGroup = HUB > 0 ? (HUB + kStHotGroups - 1) / kStHotGroups : 1;
   static constexpr int kBlk = (32 / D) * D;                                 // edges per index block (a multiple of D)
-  static constexpr int kOffRing = 0;                                        // [warps][D][800]; prologue scratch: cnt + hist
+  static constexpr int kOffRing = 0;                                        // [warps][D][800]; prologue scratch: cnt + hist (+ hub selection)
   static constexpr int kOffHot = kOffRing + WARPS * D * kStSlot;            // [HOT][1600]
-  static constexpr int kOffHeads = kOffHot + HOT * 1600;                    // [warps][200] floats
+  static constexpr int kOffHub = kOffHot + HOT * 1600;                      // [HUB][800]
+  static constexpr int kOffHeads = kOffHub + HUB * kStSlot;                 // [warps][200] floats
   static constexpr int kOffRp = kOffHeads + WARPS * 800;                    // [kStRpCap] ints
   static constexpr int kOffSlotOf = kOffRp + kStRpCap * 4;                  // [kStMaxR2] uint8: 1 + hot slot, 0 = cold
-  static constexpr int kOffIdx = kOffSlotOf + kStMaxR2;                     // [warps][2][32] int2 {source row, see block_stage}
+  static constexpr int kOffHubOf = kOffSlotOf + kStMaxR2;                   // HUB > 0: [kStHubBins] uint8: 1 + hub slot, 0 = not resident
+  static constexpr int kOffIdx = kOffHubOf + (HUB > 0 ? kStHubBins : 0);    // [warps][2][32] int2 {source row, see block_stage}
   static constexpr int kOffSc = kOffIdx + WARPS * 64 * 8;                   // BWD: [warps][2][32] float edge scales
-  static constexpr int kOffBars = kOffSc + (BWD ? WARPS * 64 * 4 : 0);      // mbarriers: [warps][D] ring slots, [8] hot groups, [warps] heads
-  static constexpr int kOffFlags = kOffBars + (WARPS * D + kStHotGroups + WARPS) * 8;  // [warps] (unused) + partition scratch (16) + range starts [warps + 1]
+  static constexpr int kOffBars = kOffSc + (BWD ? WARPS * 64 * 4 : 0);      // mbarriers: [warps][D] ring slots, [8] hot groups, [warps] heads, HUB > 0: [8] hub groups
+  static constexpr int kOffFlags = kOffBars + (WARPS * D + kStHotGroups + WARPS + (HUB > 0 ? kStHotGroups : 0)) * 8;  // [warps] (unused) + partition scratch (16) + range starts [warps + 1]
   static constexpr int kSmemBytes = kOffFlags + (2 * WARPS + 17) * 4;
   static_assert(WARPS >= 16 && WARPS <= 32, "stream gather: the partition search needs 512 threads");
   static_assert(kBlk == 32, "stream gather: index blocks are 32 edges (D = 2 or 4)");
   static_assert(kSmemBytes <= 227 * 1024, "stream gather: shared memory budget");
   static_assert(WARPS * D * kStSlot >= (kStMaxR2 + 256 + 8) * 4, "stream gather: prologue scratch lives in the ring");
+  static_assert(HUB == 0 || WARPS * D * kStSlot >= (kStHubScr + 64 + kStHubBins + 256) * 4, "stream gather: hub scratch lives in the ring");
   static_assert(HOT <= 254 && (kOffHot + HOT * 1600) / 16 < 65536, "stream gather: hot rows are addressed by 16-bit offsets");
+  static_assert(HUB <= 255 && (kOffHub + HUB * kStSlot) / 16 < 65536, "stream gather: hub rows are addressed by 16-bit offsets");
+  static_assert(!(BWD && HUB), "stream gather: hub source rows are a forward feature");
 };
 // as many resident rows as fit: forward 82 (about three quarters of ICEWS18's edges with the dataset ranking), backward 77
 template <bool BWD>
 using StDefault = StCfg<32, 2, BWD ? 77 : 82, BWD>;
+// forward on layer 1 (input rows through an index): 49 relation rows + 64 hub source rows in about the 82 rows' space
+// (tools/stream_reuse_model.py: about half of a CTA's edges come from its 64 most frequent source nodes)
+using StHubs = StCfg<32, 2, 49, false, 64>;
 
 namespace {
 
@@ -131,6 +146,28 @@ __device__ __forceinline__ uint32_t st_opaque(uint32_t v) {    // keeps a loop-i
 }
 __device__ __forceinline__ void st_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// one warp, over a histogram of counts (256 bins, the last one: 255 and more): the smallest threshold thr >= lo with
+// #(count >= thr) <= k
+__device__ __forceinline__ int st_count_threshold(const int* hist, int k, int lo, int lane) {
+  int s = 0;
+#pragma unroll
+  for (int q = 0; q < 8; ++q) s += hist[lane * 8 + q];
+  int suf = s;                                             // inclusive suffix sum over lanes (lane 31 = highest bins)
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int o = __shfl_down_sync(0xffffffffu, suf, d);
+    if (lane + d < 32) suf += o;
+  }
+  int running = suf - s, thr = 256;                        // inside the lane's 8 bins, from the top: running = #(cnt >= bin)
+#pragma unroll
+  for (int q = 7; q >= 0; --q) {
+    running += hist[lane * 8 + q];
+    if (running <= k && lane * 8 + q >= lo) thr = lane * 8 + q;
+  }
+#pragma unroll
+  for (int d = 16; d >= 1; d >>= 1) thr = min(thr, __shfl_xor_sync(0xffffffffu, thr, d));
+  return thr;
 }
 
 }  // namespace
@@ -209,6 +246,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   }
   const uint32_t hot_bar0 = smem_u32(bars + kStWarps * D);   // [8]: "the resident rows of group g have landed"
   const uint32_t head_bar0 = hot_bar0 + kStHotGroups * 8;    // [warps]: "this warp's head slot is written"
+  const uint32_t hub_bar0 = head_bar0 + kStWarps * 8;        // HUB > 0: [8] "the hub rows of group g have landed"
 
   if (tid < 16) s_part[tid] = 0;
   if (tid < kStWarps) flags[tid] = 0;
@@ -218,11 +256,22 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     mbar_init(head_bar0 + warp * 8, 1);
     if (warp == 0)
       for (int gr = 0; gr < kStHotGroups; ++gr) mbar_init(hot_bar0 + gr * 8, 1);
+    if (Cfg::kHub > 0 && warp == 1)
+      for (int gr = 0; gr < kStHotGroups; ++gr) mbar_init(hub_bar0 + gr * 8, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (!given_hot)
     for (int i = tid; i < kStMaxR2 + 256; i += kStThreads) cnt[i] = 0;
   for (int i = tid; i < kStMaxR2 / 4; i += kStThreads) reinterpret_cast<uint32_t*>(slot_of)[i] = 0u;
+  // hub selection scratch: [0] window start (smallest source node), [1] count threshold, [2] hubs above it, [8..40)
+  // per-warp tie counts, [64..) node counts [kStHubBins] + count histogram [256]
+  constexpr int kHub = Cfg::kHub;
+  int* hub_scr = cnt + kStHubScr;
+  uint8_t* hub_of = st_smem + Cfg::kOffHubOf;
+  if constexpr (kHub > 0) {
+    for (int i = tid; i < 64 + kStHubBins + 256; i += kStThreads) hub_scr[i] = i == 0 ? INT_MAX : 0;
+    for (int i = tid; i < kStHubBins / 4; i += kStThreads) reinterpret_cast<uint32_t*>(hub_of)[i] = 0u;
+  }
   __syncthreads();
   // resident rows (slot sl = lane + 32 k holds relation row_of(k)) -> shared memory, one warp; slot sl lands on the barrier
   // of group sl / kHotPerGroup, so an edge waits only for its own group and the edge loop starts before the table is
@@ -302,7 +351,14 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   auto rp = [&](int v) -> int { return rp_in_smem ? s_rp[v - A] : __ldg(row_ptr + v); };   // row_ptr[v], v in [A, A_next]
   if (rp_in_smem)
     for (int i = tid; i < n_rp; i += kStThreads) s_rp[i] = __ldg(row_ptr + A + i);
+  if constexpr (kHub > 0) {            // hub window start: the smallest source node of the CTA's edges
+    int m = INT_MAX;
+    for (int e = cb + tid; e < ce; e += kStThreads) m = min(m, __ldg(col_a + e));
+    m = __reduce_min_sync(0xffffffffu, m);
+    if (lane == 0 && m != INT_MAX) atomicMin(&hub_scr[0], m);
+  }
   __syncthreads();
+  const int hub_lo = kHub > 0 ? hub_scr[0] : 0;
   // warp ranges: the CTA's work (edges + kStNodeCost per destination) is cut into equal shares at arbitrary EDGE positions.
   // cost(v) = work before destination v; warp j starts inside the last destination whose cost(v) <= j/warps of the total
   const int64_t cta_cost = (int64_t)(ce - cb) + (int64_t)kStNodeCost * (A_next - A);
@@ -336,12 +392,21 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   };
   auto block_gather = [&](int b) {     // phase 2: dependent loads (edge scale, row indirection)
     const int e = e0 + b * kBlk + lane;
-    if ((BWD || INDEXED) && lane < kBlk && e < e1) {
+    bool hub = false;
+    if constexpr (kHub > 0) {          // residency is keyed by the source node, before the row indirection
+      const unsigned w = (unsigned)(ld_s - hub_lo);
+      const int hs = lane < kBlk && e < e1 && w < (unsigned)kStHubBins ? (int)hub_of[w] : 0;
+      hub = hs != 0;                   // staged as 1 << 31 | its group << 16 | its row's byte offset / 16
+      if (hub) ld_s = (int)(0x80000000u | (uint32_t)((hs - 1) / Cfg::kHubPerGroup) << 16 |
+                            (uint32_t)((Cfg::kOffHub + (hs - 1) * kStSlot) >> 4));
+    }
+    if ((BWD || INDEXED) && lane < kBlk && e < e1 && !hub) {
       if (BWD) ld_sc = __ldg(norm + ld_s);
       if (INDEXED) ld_s = __ldg(x_index + ld_s);
     }
   };
-  // phase 3: to shared memory.  Second word: a resident row's byte offset / 16 << 16 | its group, else the relation id
+  // phase 3: to shared memory.  Second word: a resident row's byte offset / 16 << 16 | its group, else the relation id.
+  // First word: the source row (HUB > 0: or a resident source's hub word, see block_gather)
   auto block_stage = [&](int b) {
     const int hs = use_hot ? (int)slot_of[ld_t] : 0;
     const int woff16 = hs ? (Cfg::kOffHot + (hs - 1) * 1600) >> 4 : 0;
@@ -361,24 +426,7 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     }
     __syncthreads();
     if (warp == 0) {
-      // suffix counts over the 256 bins: the smallest threshold thr >= 1 with #(cnt >= thr) <= HOT
-      int s = 0;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) s += hist[lane * 8 + k];
-      int suf = s;                                         // inclusive suffix sum over lanes (lane 31 = highest bins)
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const int o = __shfl_down_sync(0xffffffffu, suf, d);
-        if (lane + d < 32) suf += o;
-      }
-      int running = suf - s, thr = 256;                    // inside the lane's 8 bins, from the top: running = #(cnt >= bin)
-#pragma unroll
-      for (int k = 7; k >= 0; --k) {
-        running += hist[lane * 8 + k];
-        if (running <= Cfg::kHot && lane * 8 + k >= 1) thr = lane * 8 + k;
-      }
-#pragma unroll
-      for (int d = 16; d >= 1; d >>= 1) thr = min(thr, __shfl_xor_sync(0xffffffffu, thr, d));
+      const int thr = st_count_threshold(hist, Cfg::kHot, 1, lane);
       if (lane == 0) s_part[8] = thr;
     }
     __syncthreads();
@@ -403,6 +451,75 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
     }
     if (warp == 1) load_hot(min(s_part[9], Cfg::kHot), [&](int k) { return hist[lane + 32 * k]; });
   }
+  // ---- hub source rows: the CTA's HUB most frequent source nodes among the kStHubBins from its smallest one (a node of at
+  //      least 2 edges; ties at the threshold go to the smaller node ids).  Warp 2 fetches their rows (below) --------------
+  constexpr int kHubIters = kHub > 0 ? (kHub + 31) / 32 : 1;
+  int hub_row[kHubIters];
+  int n_hub = 0;
+  if constexpr (kHub > 0) {
+    int* hcnt = hub_scr + 64;
+    int* hhist = hcnt + kStHubBins;    // count histogram, then the slot -> node list
+    for (int e = cb + tid; e < ce; e += kStThreads) {
+      const unsigned w = (unsigned)(__ldg(col_a + e) - hub_lo);
+      if (w < (unsigned)kStHubBins) atomicAdd(&hcnt[w], 1);
+    }
+    __syncthreads();
+    for (int b = tid; b < kStHubBins; b += kStThreads) {
+      const int c = hcnt[b];
+      if (c >= 2) atomicAdd(&hhist[min(c, 255)], 1);
+    }
+    __syncthreads();
+    if (warp == 0) {
+      const int thr = st_count_threshold(hhist, kHub, 2, lane);
+      if (lane == 0) hub_scr[1] = thr;
+    }
+    __syncthreads();
+    // thread t owns the nodes [t kPer, (t + 1) kPer): thread order is node order, so ranking the ties is a prefix sum
+    constexpr int kPer = (kStHubBins + kStThreads - 1) / kStThreads;
+    const int thr = hub_scr[1];
+    int ties = 0;
+#pragma unroll
+    for (int q = 0; q < kPer; ++q) {
+      const int b = tid * kPer + q;
+      if (b < kStHubBins) {
+        const int c = min(hcnt[b], 255);
+        if (c >= thr) {                // at most HUB nodes
+          const int sl = atomicAdd(&hub_scr[2], 1);
+          hub_of[b] = (uint8_t)(sl + 1);
+          hhist[sl] = b;
+        } else if (c == thr - 1 && c >= 2) {
+          ++ties;
+        }
+      }
+    }
+    int incl = ties;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int o = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += o;
+    }
+    if (lane == 31) hub_scr[8 + warp] = incl;
+    __syncthreads();
+    const int n_above = hub_scr[2];
+    int rank = n_above + __reduce_add_sync(0xffffffffu, lane < warp ? hub_scr[8 + lane] : 0) + incl - ties;
+#pragma unroll
+    for (int q = 0; q < kPer; ++q) {
+      const int b = tid * kPer + q;
+      if (b < kStHubBins && min(hcnt[b], 255) == thr - 1 && thr - 1 >= 2) {
+        if (rank < kHub) { hub_of[b] = (uint8_t)(rank + 1); hhist[rank] = b; }
+        ++rank;
+      }
+    }
+    __syncthreads();                   // hub_of and the slot list are complete
+    if (warp == 2) {
+      n_hub = min(kHub, n_above + __reduce_add_sync(0xffffffffu, lane < kStWarps ? hub_scr[8 + lane] : 0));
+#pragma unroll
+      for (int k = 0; k < kHubIters; ++k) {
+        const int sl = lane + 32 * k;
+        hub_row[k] = sl < n_hub ? (INDEXED ? __ldg(x_index + hub_lo + hhist[sl]) : hub_lo + hhist[sl]) : 0;
+      }
+    }
+  }
   block_gather(0);
   __syncthreads();                     // s_rp, slot_of complete; the ring (= cnt / hist) may be overwritten from here on
   block_stage(0);
@@ -425,9 +542,25 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   // programmatic stream serialisation gets the prologue overlapped with that kernel's tail; in plain stream order (what
   // the library does, see rgcn_fwd.cu) this wait returns immediately.
   asm volatile("griddepcontrol.wait;" ::: "memory");
+  if constexpr (kHub > 0) {
+    if (warp == 2) {                   // the hub rows, on 8 group barriers (every barrier gets its arrival)
+      if (lane < kStHotGroups)
+        st_expect_tx(hub_bar0 + lane * 8,
+                     (uint32_t)min(max(n_hub - lane * Cfg::kHubPerGroup, 0), Cfg::kHubPerGroup) * (uint32_t)kStSlot);
+      __syncwarp();
 #pragma unroll
-  for (int k = 0; k < D; ++k)
-    if (k < n) issue(k, k);
+      for (int k = 0; k < kHubIters; ++k) {
+        const int sl = lane + 32 * k;
+        if (sl < n_hub)
+          st_bulk_g2s(smem_u32(st_smem + Cfg::kOffHub + sl * kStSlot), X + (int64_t)hub_row[k] * 200, kStSlot,
+                      hub_bar0 + (sl / Cfg::kHubPerGroup) * 8);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < D; ++k)
+      if (k < n) issue(k, k);
+  }
 
   // ---- first destination of the range (binary search in the CTA's row_ptr slice while the first copies fly) -----------------
   int va;
@@ -509,61 +642,135 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
   constexpr int kP1 = (kBlk / D / 3) * D, kP2 = (2 * (kBlk / D) / 3) * D;
   int phase_at = kP1, phase = 0, blk = 0;
   if (dbg) stamp(2, clock64());
-  for (int g = 0; g < n; g += D) {     // one pass over the ring: slot numbers are compile-time constants
-    if (g == phase_at) {
-      if (phase == 0) { block_gather(blk + 1); phase_at += kP2 - kP1; phase = 1; }
-      else if (phase == 1) { block_stage(blk + 1); phase_at += kBlk - kP2; phase = 2; }
-      else { ++blk; block_load(blk + 1); phase_at += kP1; phase = 0; }
-    }
-    auto do_slot = [&](auto slot_c) {
-      constexpr int slot = decltype(slot_c)::value;
-      const int i = g + slot;
-      if (i < n) {
-        while (e0 + i >= cur_end) advance();       // warp-uniform: the running destination is complete
-        const uint32_t wsel = st_lds_u32(idx_a + (((uint32_t)i & 63u) << 3) + 4);
-        const uint32_t woff16 = wsel >> 16;
-        const float sc = BWD ? __uint_as_float(st_lds_u32(sc_a + (((uint32_t)i & 63u) << 2))) : 1.f;
-        float2 h[4];
-        float4 w[4];
-        w[3] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (woff16) {                  // resident row: wait for its group once per warp
-          const uint32_t grp = wsel & 0xffffu;
-          if (!((hot_seen >> grp) & 1u)) { mbar_wait(hot_bar0 + grp * 8, 0); hot_seen |= 1u << grp; }
-          const uint32_t wa = smem_l16 + (woff16 << 4);
-          w[0] = st_lds_f4<0>(wa); w[1] = st_lds_f4<512>(wa); w[2] = st_lds_f4<1024>(wa);
-          if (tail4) w[3] = st_lds_f4<1536>(wa);
-        } else {                       // cold row: straight from L2 into registers, in flight while the source row is awaited
-          const float* wr = w_l4 + (int64_t)(int)wsel * 400;
-          w[0] = ldg_f4(wr); w[1] = ldg_f4(wr + 128); w[2] = ldg_f4(wr + 256);
-          if (tail4) w[3] = ldg_f4(wr + 384);
-        }
-        st_wait(bar0 + slot * 8, parity);
-        h[0] = st_lds_f2<slot * kStSlot>(ring_l8);       h[1] = st_lds_f2<slot * kStSlot + 256>(ring_l8);
-        h[2] = st_lds_f2<slot * kStSlot + 512>(ring_l8);
-        h[3] = make_float2(0.f, 0.f);
-        if (tail4) h[3] = st_lds_f2<slot * kStSlot + 768>(ring_l8);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float x = BWD ? h[k].x * sc : h[k].x, y = BWD ? h[k].y * sc : h[k].y;
-          if (!BWD) {                  // out[j] += sum_i in[i] * W[i][j]
-            acc[2 * k] = fmaf(x, w[k].x, fmaf(y, w[k].z, acc[2 * k]));
-            acc[2 * k + 1] = fmaf(x, w[k].y, fmaf(y, w[k].w, acc[2 * k + 1]));
-          } else {                     // din[i] += sum_j W[i][j] * g[j]
-            acc[2 * k] = fmaf(x, w[k].x, fmaf(y, w[k].y, acc[2 * k]));
-            acc[2 * k + 1] = fmaf(x, w[k].z, fmaf(y, w[k].w, acc[2 * k + 1]));
+  if constexpr (kHub == 0) {
+    for (int g = 0; g < n; g += D) {     // one pass over the ring: slot numbers are compile-time constants
+      if (g == phase_at) {
+        if (phase == 0) { block_gather(blk + 1); phase_at += kP2 - kP1; phase = 1; }
+        else if (phase == 1) { block_stage(blk + 1); phase_at += kBlk - kP2; phase = 2; }
+        else { ++blk; block_load(blk + 1); phase_at += kP1; phase = 0; }
+      }
+      auto do_slot = [&](auto slot_c) {
+        constexpr int slot = decltype(slot_c)::value;
+        const int i = g + slot;
+        if (i < n) {
+          while (e0 + i >= cur_end) advance();       // warp-uniform: the running destination is complete
+          const uint32_t wsel = st_lds_u32(idx_a + (((uint32_t)i & 63u) << 3) + 4);
+          const uint32_t woff16 = wsel >> 16;
+          const float sc = BWD ? __uint_as_float(st_lds_u32(sc_a + (((uint32_t)i & 63u) << 2))) : 1.f;
+          float2 h[4];
+          float4 w[4];
+          w[3] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (woff16) {                  // resident row: wait for its group once per warp
+            const uint32_t grp = wsel & 0xffffu;
+            if (!((hot_seen >> grp) & 1u)) { mbar_wait(hot_bar0 + grp * 8, 0); hot_seen |= 1u << grp; }
+            const uint32_t wa = smem_l16 + (woff16 << 4);
+            w[0] = st_lds_f4<0>(wa); w[1] = st_lds_f4<512>(wa); w[2] = st_lds_f4<1024>(wa);
+            if (tail4) w[3] = st_lds_f4<1536>(wa);
+          } else {                       // cold row: straight from L2 into registers, in flight while the source row is awaited
+            const float* wr = w_l4 + (int64_t)(int)wsel * 400;
+            w[0] = ldg_f4(wr); w[1] = ldg_f4(wr + 128); w[2] = ldg_f4(wr + 256);
+            if (tail4) w[3] = ldg_f4(wr + 384);
           }
+          st_wait(bar0 + slot * 8, parity);
+          h[0] = st_lds_f2<slot * kStSlot>(ring_l8);       h[1] = st_lds_f2<slot * kStSlot + 256>(ring_l8);
+          h[2] = st_lds_f2<slot * kStSlot + 512>(ring_l8);
+          h[3] = make_float2(0.f, 0.f);
+          if (tail4) h[3] = st_lds_f2<slot * kStSlot + 768>(ring_l8);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float x = BWD ? h[k].x * sc : h[k].x, y = BWD ? h[k].y * sc : h[k].y;
+            if (!BWD) {                  // out[j] += sum_i in[i] * W[i][j]
+              acc[2 * k] = fmaf(x, w[k].x, fmaf(y, w[k].z, acc[2 * k]));
+              acc[2 * k + 1] = fmaf(x, w[k].y, fmaf(y, w[k].w, acc[2 * k + 1]));
+            } else {                     // din[i] += sum_j W[i][j] * g[j]
+              acc[2 * k] = fmaf(x, w[k].x, fmaf(y, w[k].y, acc[2 * k]));
+              acc[2 * k + 1] = fmaf(x, w[k].z, fmaf(y, w[k].w, acc[2 * k + 1]));
+            }
+          }
+          __syncwarp();                  // every lane has consumed the slot (the FMAs depend on the loads)
+          if (i + D < n) issue(i + D, slot);
         }
-        __syncwarp();                  // every lane has consumed the slot (the FMAs depend on the loads)
-        if (i + D < n) issue(i + D, slot);
+      };
+      do_slot(std::integral_constant<int, 0>{});
+      do_slot(std::integral_constant<int, 1>{});
+      if constexpr (D == 4) {
+        do_slot(std::integral_constant<int, 2>{});
+        do_slot(std::integral_constant<int, 3>{});
+      }
+      parity ^= 1u;
+    }
+  } else {
+    // the ring takes the edges whose source is not resident, in edge order, D copies in flight: `iss` is the next edge to
+    // look at (the staged ones: block blk + 1 from phase 2 on), `fly` the copies issued and not consumed, the oldest of
+    // them in slot `rslot`.  An edge whose source is resident waits once per warp for its hub group (hot_seen bit 8 + g)
+    // and reads the hub row
+    int iss = 0, fly = 0, rslot = 0;
+    auto top_up = [&]() {
+      const int lim = min(n, (blk + (phase == 2 ? 2 : 1)) * kBlk);
+      while (fly < D && iss < lim) {
+        const uint32_t src = st_lds_u32(idx_a + (((uint32_t)iss & 63u) << 3));
+        if (!(src >> 31)) {
+          const int wslot = (rslot + fly) % D;
+          if (st_elect_one()) {
+            const uint32_t bar = bar0 + wslot * 8;
+            st_expect_tx(bar, 800u);
+            st_bulk_g2s(ring + wslot * kStSlot, X + (int64_t)(int)src * 200, 800, bar);
+          }
+          ++fly;
+        }
+        ++iss;
       }
     };
-    do_slot(std::integral_constant<int, 0>{});
-    do_slot(std::integral_constant<int, 1>{});
-    if constexpr (D == 4) {
-      do_slot(std::integral_constant<int, 2>{});
-      do_slot(std::integral_constant<int, 3>{});
+    top_up();
+    const uint32_t smem_l8 = st_opaque(smem_u32(st_smem) + 8 * lane);
+    for (int i = 0; i < n; ++i) {
+      if (i == phase_at) {
+        if (phase == 0) { block_gather(blk + 1); phase_at += kP2 - kP1; phase = 1; }
+        else if (phase == 1) { block_stage(blk + 1); phase_at += kBlk - kP2; phase = 2; top_up(); }
+        else { ++blk; block_load(blk + 1); phase_at += kP1; phase = 0; }
+      }
+      while (e0 + i >= cur_end) advance();         // warp-uniform: the running destination is complete
+      const uint32_t ent = idx_a + (((uint32_t)i & 63u) << 3);
+      const uint32_t src = st_lds_u32(ent), wsel = st_lds_u32(ent + 4);
+      const uint32_t woff16 = wsel >> 16;
+      float2 h[4];
+      float4 w[4];
+      w[3] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (woff16) {                    // resident relation row
+        const uint32_t grp = wsel & 0xffffu;
+        if (!((hot_seen >> grp) & 1u)) { mbar_wait(hot_bar0 + grp * 8, 0); hot_seen |= 1u << grp; }
+        const uint32_t wa = smem_l16 + (woff16 << 4);
+        w[0] = st_lds_f4<0>(wa); w[1] = st_lds_f4<512>(wa); w[2] = st_lds_f4<1024>(wa);
+        if (tail4) w[3] = st_lds_f4<1536>(wa);
+      } else {                         // cold relation row: from L2 into registers
+        const float* wr = w_l4 + (int64_t)(int)wsel * 400;
+        w[0] = ldg_f4(wr); w[1] = ldg_f4(wr + 128); w[2] = ldg_f4(wr + 256);
+        if (tail4) w[3] = ldg_f4(wr + 384);
+      }
+      uint32_t ha;
+      if (src >> 31) {                 // resident source row
+        const uint32_t grp = (src >> 16) & 0x7fffu;
+        if (!((hot_seen >> (8 + grp)) & 1u)) { mbar_wait(hub_bar0 + grp * 8, 0); hot_seen |= 1u << (8 + grp); }
+        ha = smem_l8 + ((src & 0xffffu) << 4);
+      } else {
+        st_wait(bar0 + rslot * 8, parity);
+        ha = ring_l8 + rslot * kStSlot;
+      }
+      h[0] = st_lds_f2<0>(ha); h[1] = st_lds_f2<256>(ha); h[2] = st_lds_f2<512>(ha);
+      h[3] = make_float2(0.f, 0.f);
+      if (tail4) h[3] = st_lds_f2<768>(ha);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {    // out[j] += sum_i in[i] * W[i][j]
+        acc[2 * k] = fmaf(h[k].x, w[k].x, fmaf(h[k].y, w[k].z, acc[2 * k]));
+        acc[2 * k + 1] = fmaf(h[k].x, w[k].y, fmaf(h[k].y, w[k].w, acc[2 * k + 1]));
+      }
+      if (!(src >> 31)) {
+        __syncwarp();                  // every lane has consumed the slot
+        --fly;
+        if (++rslot == D) { rslot = 0; parity ^= 1u; }
+        top_up();
+      }
     }
-    parity ^= 1u;
   }
   if (dbg) stamp(3, clock64());
   // ---- end of the range ------------------------------------------------------------------------------------------------------
