@@ -208,6 +208,11 @@ def batch_graphs(bh, graph_dict):
 # --------------------------------------------------------------------------------------------------
 # RGCN block layer
 # --------------------------------------------------------------------------------------------------
+# rgcn_block_layer gathers W[etype] for at most this many edges at once: a whole-graph batch of 3.5 M edges would need 11 GB
+# in float64
+EDGE_CHUNK = 1 << 18
+
+
 def rgcn_block_layer(H, W, Wloop, src, dst, etype, norm, relu, num_bases):
     """Closed form of RGCNLayer.forward + RGCNBlockLayer (RGCN.py:33-51, 79-94), dropout off:
 
@@ -222,10 +227,13 @@ def rgcn_block_layer(H, W, Wloop, src, dst, etype, norm, relu, num_bases):
     so = W.shape[1] // (nb * si)
     dout = nb * so
     if src.numel() > 0:
-        w = W[etype].view(-1, nb, si, so)                      # RGCN.py:81-85
-        x = H[src].view(-1, nb, si)                            # RGCN.py:86
-        msg = torch.einsum('ebi,ebij->ebj', x, w).reshape(-1, dout)   # RGCN.py:87
-        agg = torch.zeros(N, dout, dtype=H.dtype, device=H.device).index_add(0, dst, msg)  # fn.sum, RGCN.py:91
+        agg = torch.zeros(N, dout, dtype=H.dtype, device=H.device)
+        for a in range(0, src.numel(), EDGE_CHUNK):            # the same adds in the same order, a chunk of edges at a time
+            e = slice(a, a + EDGE_CHUNK)
+            w = W[etype[e]].view(-1, nb, si, so)               # RGCN.py:81-85
+            x = H[src[e]].view(-1, nb, si)                     # RGCN.py:86
+            msg = torch.einsum('ebi,ebij->ebj', x, w).reshape(-1, dout)   # RGCN.py:87
+            agg = agg.index_add(0, dst[e], msg)                # fn.sum, RGCN.py:91
     else:
         agg = H if din == dout else torch.zeros(N, dout, dtype=H.dtype, device=H.device)  # DGL 0.4: reduce skipped
     out = agg * norm.view(-1, 1)                               # RGCN.py:93-94
@@ -390,13 +398,14 @@ def global_windows(t_list, times, seq_len=10):
 def global_pooled(params, window_times, graph_dict, reverse, maxpool, num_bases=100):
     """Aggregator.py:53-62 / 96-105: dgl.batch of WHOLE graphs, two block layers, max / mean over each graph's nodes."""
     P = params
+    dev = P['ent_embeds'].device
     gs = [graph_dict[int(t)] for t in window_times]
     off = np.concatenate(([0], np.cumsum([g.number_of_nodes() for g in gs]))).astype(np.int64)
-    src = torch.as_tensor(np.concatenate([g.src + o for g, o in zip(gs, off[:-1])]))
-    dst = torch.as_tensor(np.concatenate([g.dst + o for g, o in zip(gs, off[:-1])]))
-    et = torch.as_tensor(np.concatenate([g.type_o if reverse else g.type_s for g in gs]))
-    norm = torch.as_tensor(np.concatenate([g.norm for g in gs]))
-    H0 = P['ent_embeds'][torch.as_tensor(np.concatenate([g.id for g in gs]))]
+    src = torch.as_tensor(np.concatenate([g.src + o for g, o in zip(gs, off[:-1])]), device=dev)
+    dst = torch.as_tensor(np.concatenate([g.dst + o for g, o in zip(gs, off[:-1])]), device=dev)
+    et = torch.as_tensor(np.concatenate([g.type_o if reverse else g.type_s for g in gs]), device=dev)
+    norm = torch.as_tensor(np.concatenate([g.norm for g in gs]), device=dev)
+    H0 = P['ent_embeds'][torch.as_tensor(np.concatenate([g.id for g in gs]), device=dev)]
     H1 = rgcn_block_layer(H0, P['aggregator.rgcn1.weight'], P['aggregator.rgcn1.loop_weight'], src, dst, et, norm, True,
                           num_bases)
     H2 = rgcn_block_layer(H1, P['aggregator.rgcn2.weight'], P['aggregator.rgcn2.loop_weight'], src, dst, et, norm, False,
@@ -414,11 +423,13 @@ def soft_cross_entropy(pred, soft_targets):
 
 
 def global_forward(params, t_list, true_prob_s, true_prob_o, graph_dict, subject, maxpool=1, seq_len=10, num_bases=100):
-    """RENet_global.forward (global_model.py:35-55): loss of one direction for a batch of timestamps."""
+    """RENet_global.forward (global_model.py:35-55): loss of one direction for a batch of timestamps.  Runs on the device
+    of ``params``."""
     P = params
+    dev = P['ent_embeds'].device
     reverse = not subject
     lin = 'linear_s' if subject else 'linear_o'
-    true_prob = torch.as_tensor(true_prob_o if subject else true_prob_s)
+    true_prob = torch.as_tensor(true_prob_o if subject else true_prob_s, device=dev)
     t_host = np.asarray(t_list, dtype=np.int64)
     idx = np.argsort(-t_host, kind='stable')                                    # global_model.py:45
     times = list(graph_dict.keys())
@@ -426,13 +437,13 @@ def global_forward(params, t_list, true_prob_s, true_prob_o, graph_dict, subject
     uniq = sorted({int(t) for w in windows for t in w})                          # Aggregator.py:47
     pos = {t: i for i, t in enumerate(uniq)}
     info = global_pooled(P, uniq, graph_dict, reverse, maxpool, num_bases)
-    X = info[torch.as_tensor([pos[int(t)] for w in windows for t in w], dtype=torch.long)]
+    X = info[torch.as_tensor([pos[int(t)] for w in windows for t in w], dtype=torch.long, device=dev)]
     lens = [len(w) for w in windows]
     s_q = gru_final_hidden_batched(X, lens, P['encoder_global.weight_ih_l0'], P['encoder_global.weight_hh_l0'],
                                    P['encoder_global.bias_ih_l0'], P['encoder_global.bias_hh_l0'])
-    s_q = torch.cat((s_q, torch.zeros(len(t_host) - len(s_q), s_q.shape[1])), dim=0)    # global_model.py:51
+    s_q = torch.cat((s_q, s_q.new_zeros(len(t_host) - len(s_q), s_q.shape[1])), dim=0)    # global_model.py:51
     pred = s_q @ P[lin + '.weight'].t() + P[lin + '.bias']
-    return soft_cross_entropy(pred, true_prob[torch.as_tensor(idx)])
+    return soft_cross_entropy(pred, true_prob[torch.as_tensor(idx, device=dev)])
 
 
 def global_predict(params, t, graph_dict, subject=True, maxpool=1, seq_len=10, num_bases=100):
