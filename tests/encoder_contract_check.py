@@ -175,10 +175,21 @@ class Restated:
     pass
 
 
-def restate_dir(P, d, rev, mut=(None, None), samples=None, table=None, mask1=None):
+def _layer(H, W, Wloop, src, dst, et, norm, relu, nb, loop_mask):
+    """restate.rgcn_block_layer, with the self-loop rows scaled by a dropout mask when one is given (RGCN.py:36-37)"""
+    if loop_mask is None:
+        return restate.rgcn_block_layer(H, W, Wloop, src, dst, et, norm, relu, nb)
+    out = restate.rgcn_block_layer(H, W, None, src, dst, et, norm, False, nb) + (H @ Wloop) * loop_mask.double()
+    return torch.relu(out) if relu else out
+
+
+def restate_dir(P, d, rev, mut=(None, None), samples=None, table=None, mask1=None, loop1=None, loop2=None, x4=None, x3=None):
     """s_h, s_q [Q, h] in the restatement's (stable, length-descending) order, plus what the mistakes are picked from.
     mask1 (bool [N, h]): layer 1's ReLU taken as this mask (the kernel's own H1 > 0), so that an element whose
-    pre-activation is within rounding of 0 cannot flip the sign of its derivative between fp32 and fp64"""
+    pre-activation is within rounding of 0 cannot flip the sign of its derivative between fp32 and fp64.
+    Dropout masks (scale factors, None: no dropout): loop1 [N, h] and loop2 [N, h] on the self-loop rows of layers 1 and 2
+    (only layer 2's read-out rows reach the outputs), x4 [S, 4h] and x3 [S, 3h] on the GRU inputs in sequence-major row
+    order"""
     kind, arg = mut
     R, nb = d.R, d.nb
     idx = np.arange(len(d.trip)) if samples is None else np.asarray(samples)
@@ -195,13 +206,13 @@ def restate_dir(P, d, rev, mut=(None, None), samples=None, table=None, mask1=Non
     if kind == 'drop-edge':
         keep[arg] = False
     H0 = P['ent_embeds'][_t(g.id)]
-    H1 = restate.rgcn_block_layer(H0, P['aggregator.rgcn1.weight'], P['aggregator.rgcn1.loop_weight'], _t(g.src[keep]),
-                                  _t(g.dst[keep]), _t(et[keep]), norm, mask1 is None, nb)
+    H1 = _layer(H0, P['aggregator.rgcn1.weight'], P['aggregator.rgcn1.loop_weight'], _t(g.src[keep]), _t(g.dst[keep]),
+                _t(et[keep]), norm, mask1 is None, nb, loop1)
     if mask1 is not None:
         H1 = H1 * mask1.double()
     norm2 = torch.as_tensor(parent_norm(d, bh, g), device=DEV).double() if kind == 'norm-full' else norm
-    H2 = restate.rgcn_block_layer(H1, P['aggregator.rgcn2.weight'], P['aggregator.rgcn2.loop_weight'], _t(g.src), _t(g.dst),
-                                  _t(et), norm2, False, nb)
+    H2 = _layer(H1, P['aggregator.rgcn2.weight'], P['aggregator.rgcn2.loop_weight'], _t(g.src), _t(g.dst), _t(et), norm2,
+                False, nb, loop2)
     seq_len = bh.seq_len.copy()
     starts = np.concatenate(([0], np.cumsum(seq_len)[:-1])).astype(np.int64)
     rows = np.arange(len(g.readout))
@@ -225,6 +236,8 @@ def restate_dir(P, d, rev, mut=(None, None), samples=None, table=None, mask1=Non
     rel = P['rel_embeds'][R:] if rev != (kind == 'rel-half') else P['rel_embeds'][:R]
     table = d.table64() if table is None else table
     X4, X3, _, _ = restate.packed_inputs(H2, _t(readout), seq_len, s_tem, r_tem, P['ent_embeds'], rel, table[_t(gidx)])
+    if x4 is not None:
+        X4, X3 = X4 * x4.double(), X3 * x3.double()
     out = Restated()
     out.s_h = restate.gru_final_hidden_batched(X4, seq_len, P['encoder.weight_ih_l0'], P['encoder.weight_hh_l0'],
                                                P['encoder.bias_ih_l0'], P['encoder.bias_hh_l0'])

@@ -245,11 +245,27 @@ def run_adam(cs, n, step=1, gs=1.0, max_norm=1.0, wd=1e-5, use_sumsq=True, gscal
     for t in tails:
         assert torch.equal(t[n:], torch.full_like(t[n:], SENT_F)), (cs, 'adam wrote past n')
     assert_kernels(cs, call, {'adam_step_kernel'})
-    f32 = lambda x: float(np.float32(x))
-    lr_, b1, b2, eps, wd_, gs_ = f32(lr), f32(0.9), f32(0.999), f32(1e-8), f32(wd), f32(gs)
-    clip = 1.0
-    if use_sumsq and max_norm > 0:
-        clip = min(1.0, f32(max_norm) / (np.sqrt(float(sumsq[0])) * gs_ + 1e-6))
+    clip = clip_coef(float(sumsq[0]), max_norm, gs) if use_sumsq and max_norm > 0 else 1.0
+    (P1, M1, V1), (bp, bm, bv) = adam_ref(p0, g, m0, v0, step, clip, lr, 0.9, 0.999, 1e-8, wd, gs)
+    check_bound('adam m', cs, 'm', m, M1, bm)
+    check_bound('adam v', cs, 'v', v, V1, bv)
+    check_bound('adam p', cs, 'p', p, P1, bp)
+    return clip
+
+
+def f32(x):
+    return float(np.float32(x))
+
+
+def clip_coef(sumsq, max_norm, gs=1.0):
+    """renet_adam_step's clip factor from a sum of squares: clip_grad_norm_'s max_norm / (|g| + 1e-6), capped at 1"""
+    return min(1.0, f32(max_norm) / (np.sqrt(sumsq) * f32(gs) + 1e-6))
+
+
+def adam_ref(p0, g, m0, v0, step, clip, lr, b1, b2, eps, wd, gs=1.0):
+    """one fp64 step of torch.optim.Adam(amsgrad=False) with weight decay on the clipped gradient g * gs * clip, the
+    hyper-parameters rounded to fp32 as the kernel sees them -> ((p, m, v), (their bounds)), as the module docstring derives"""
+    lr_, b1, b2, eps, wd_, gs_ = f32(lr), f32(b1), f32(b2), f32(eps), f32(wd), f32(gs)
     bc1, bc2 = 1.0 - b1 ** step, 1.0 - b2 ** step
     P0, G, M0, V0 = p0.double(), g.double(), m0.double(), v0.double()
     ga = G * gs_ * clip
@@ -262,10 +278,7 @@ def run_adam(cs, n, step=1, gs=1.0, max_norm=1.0, wd=1e-5, use_sumsq=True, gscal
     P1 = P0 - stp
     Tm = b1 * M0.abs() + (1 - b1) * Tg
     Tv = b2 * V0 + (1 - b2) * Tg * Tg
-    check_bound('adam m', cs, 'm', m, M1, C_ADAM * U * Tm)
-    check_bound('adam v', cs, 'v', v, V1, C_ADAM * U * Tv)
-    check_bound('adam p', cs, 'p', p, P1, C_ADAM * U * (P0.abs() + stp.abs() + lr_ / bc1 * Tm / denom))
-    return clip
+    return (P1, M1, V1), (C_ADAM * U * (P0.abs() + stp.abs() + lr_ / bc1 * Tm / denom), C_ADAM * U * Tm, C_ADAM * U * Tv)
 
 
 for _n in (1, 3, 4, 5, 1023):

@@ -50,3 +50,15 @@ def test_mask_layout():
         u = np.float32(r[idx & 3]) * np.float32(2.0 ** -32)
         assert m[i] == (np.float32(2.0) if u >= np.float32(p) else np.float32(0.0))
     assert chk.mask_ref(seed, 0, 64, 0.0).tolist() == [1.0] * 64
+
+
+@pytest.mark.parametrize('seed, off, n, p', [(0x1234_5678_9ABC_DEF1, 0, 4099, 0.5), (0x0DDBA11_5EED, 3, 1001, 0.5),
+                                             (42, (1 << 34) - 6, 37, 0.5), ((1 << 64) - 1, 5, 517, 0.9), (7, 2, 64, 0.0)])
+def test_torch_mask_port(seed, off, n, p):
+    """the training-step suite's torch port of mask_ref (run here on the CPU): the same scale factors, counters whose high
+    word turns non-zero and an all-ones key included"""
+    import torch
+    import step_contract_check as step
+    got = step.mask_torch(seed, off, n, p, device='cpu')
+    assert got.dtype == torch.float32
+    np.testing.assert_array_equal(got.numpy(), chk.mask_ref(seed, off, n, p))
