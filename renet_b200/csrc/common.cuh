@@ -91,10 +91,13 @@ int scatter_add_rows_det(const float* src, int64_t ld, const int32_t* index, con
                          int d, cudaStream_t stream);
 
 // internal (non-exported) launchers shared between translation units -------------------------------
-// C[M,N] (ldc) = A[M,K] (rows optionally through a_index; lda) @ B[K,N] (ldb) [+ bias[N]] [+ C if accumulate]
+// C[M,N] (ldc) = A[M,K] (rows optionally through a_index; lda) @ B[K,N] (ldb) [+ bias[N]] [+ C if accumulate].
+// b_cacheable: B is a weight, so the tensor-core engine may key its packed image on B's address (packed_cache_lookup).
+// Pass false for a B that lives in a per-call workspace: another call of the same weight generation can hold a different
+// matrix at that address, and a cached image would be stale.
 int sgemm_nn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
              int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
-             cudaStream_t stream);
+             cudaStream_t stream, bool b_cacheable = true);
 // The FFMA engine of sgemm_nn: the register-tiled kernel where sgemm_nn_tiled_ok holds (and naive is false), else one thread
 // per output
 bool sgemm_nn_tiled_ok(const float* A, int64_t lda, const float* B, int64_t ldb, const float* C, int64_t ldc,

@@ -446,11 +446,12 @@ int launch_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_g
   concat_bias_kernel<<<(6 * h + 255) / 256, 256, 0, stream>>>(b_hh4, b_hh3, w.bhh, 3 * h);
   RENET_CHECK_LAUNCH("concat_bias_kernel");
 
-  // input projections
-  if ((rc = sgemm_nn(H2, readout, h, w.Brow, 6 * h, w.GI, 6 * h, nullptr, S, 6 * h, h, false, stream))) return rc;
-  if ((rc = sgemm_nn(ent, seq_s, h, w.Bent, 6 * h, w.PQ, 6 * h, w.bih, Q, 6 * h, h, false, stream))) return rc;
-  if ((rc = sgemm_nn(rel, seq_r, h, w.Brel, 3 * h, w.PQ, 6 * h, nullptr, Q, 3 * h, h, true, stream))) return rc;
-  if ((rc = sgemm_nn(glob, nullptr, h, w.Bglob, 6 * h, w.PT, 6 * h, nullptr, T, 6 * h, h, false, stream))) return rc;
+  // input projections.  The B operands are this call's transposed copies in the workspace, not the weights: they must
+  // not key the packed-weight cache (sgemm_nn's b_cacheable)
+  if ((rc = sgemm_nn(H2, readout, h, w.Brow, 6 * h, w.GI, 6 * h, nullptr, S, 6 * h, h, false, stream, false))) return rc;
+  if ((rc = sgemm_nn(ent, seq_s, h, w.Bent, 6 * h, w.PQ, 6 * h, w.bih, Q, 6 * h, h, false, stream, false))) return rc;
+  if ((rc = sgemm_nn(rel, seq_r, h, w.Brel, 3 * h, w.PQ, 6 * h, nullptr, Q, 3 * h, h, true, stream, false))) return rc;
+  if ((rc = sgemm_nn(glob, nullptr, h, w.Bglob, 6 * h, w.PT, 6 * h, nullptr, T, 6 * h, h, false, stream, false))) return rc;
 
   // recurrence over the packed time steps
   const int64_t hs_stride = Q * 2 * h;
@@ -461,10 +462,10 @@ int launch_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_g
     float* Hnext = w.Hs + (int64_t)(t + 1) * hs_stride;
     float* GH = w.GH + (int64_t)t * Q * 6 * h;
     if (t > 0) {
-      if ((rc = sgemm_nn(Hprev, nullptr, 2 * h, w.Whh, 6 * h, GH, 6 * h, nullptr, n_act, 3 * h, h, false, stream)))
+      if ((rc = sgemm_nn(Hprev, nullptr, 2 * h, w.Whh, 6 * h, GH, 6 * h, nullptr, n_act, 3 * h, h, false, stream, false)))
         return rc;
       if ((rc = sgemm_nn(Hprev + h, nullptr, 2 * h, w.Whh + 3 * h, 6 * h, GH + 3 * h, 6 * h, nullptr, n_act,
-                         3 * h, h, false, stream)))
+                         3 * h, h, false, stream, false)))
         return rc;
     }
     const int total = n_act * 2 * h;

@@ -275,7 +275,8 @@ int launch_selfloop_bwd(const float* H, const int32_t* h_index, const float* Wlo
   transpose_kernel<<<tg, dim3(32, 8), 0, stream>>>(Wloop, WloopT_ws, d_in, d_out);
   RENET_CHECK_LAUNCH("transpose_kernel");
   int rc;
-  if ((rc = sgemm_nn(dLoop, nullptr, d_out, WloopT_ws, d_in, dH, d_in, nullptr, N, d_in, d_out, false, stream))) return rc;
+  if ((rc = sgemm_nn(dLoop, nullptr, d_out, WloopT_ws, d_in, dH, d_in, nullptr, N, d_in, d_out, false, stream, false)))
+    return rc;
   return sgemm_tn(H, h_index, d_in, dLoop, d_out, dWloop, d_out, d_in, d_out, N, true, stream);
 }
 

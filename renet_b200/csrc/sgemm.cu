@@ -240,7 +240,7 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 int umma_gemm_nn_try(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
                      int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
-                     cudaStream_t stream);
+                     cudaStream_t stream, bool b_cacheable);
 
 // RENET_GEMM=ffma|umma selects the dense-GEMM engine (both are this library's own sm_90a kernels).
 static int g_gemm_mode = -1;
@@ -286,10 +286,10 @@ int sgemm_nn_ffma(const float* A, const int32_t* a_index, int64_t lda, const flo
 
 int sgemm_nn(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
              int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
-             cudaStream_t stream) {
+             cudaStream_t stream, bool b_cacheable) {
   if (M <= 0 || N <= 0) return RENET_OK;
   if (gemm_mode() == 1) {   // wgmma 3xTF32 path (umma_gemm.cu); returns 0 when the shape is not supported
-    const int r = umma_gemm_nn_try(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
+    const int r = umma_gemm_nn_try(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream, b_cacheable);
     if (r != 0) return r < 0 ? r : RENET_OK;
   }
   return sgemm_nn_ffma(A, a_index, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, false, stream);

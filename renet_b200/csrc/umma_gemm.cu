@@ -902,10 +902,10 @@ int umma_gemm_prepacked(const float* A, const int32_t* a_index, int64_t lda, con
 }
 
 // Returns 1 if the shape was taken by the tensor-core path (launch enqueued), 0 if the caller should fall back to the FFMA
-// kernel, negative on error.
+// kernel, negative on error.  b_cacheable: B is a weight whose packed image may be cached by address (sgemm_nn).
 int umma_gemm_nn_try(const float* A, const int32_t* a_index, int64_t lda, const float* B, int64_t ldb, float* C,
                      int64_t ldc, const float* bias, int64_t M, int32_t N, int32_t K, bool accumulate,
-                     cudaStream_t stream) {
+                     cudaStream_t stream, bool b_cacheable) {
   const bool aligned = ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C) |
                          reinterpret_cast<uintptr_t>(bias)) & 15) == 0;
   if (!aligned || !umma_shape_ok(N, K) || lda % 4 != 0 || ldc % 4 != 0 || M < 64) return 0;
@@ -914,7 +914,7 @@ int umma_gemm_nn_try(const float* A, const int32_t* a_index, int64_t lda, const 
   bool hit = false;
   const void* keys[4] = {B, reinterpret_cast<const void*>((intptr_t)ldb), reinterpret_cast<const void*>((intptr_t)N),
                          reinterpret_cast<const void*>((intptr_t)K)};
-  void* Bp = packed_cache_lookup(keys, 4, pb, &hit);
+  void* Bp = b_cacheable ? packed_cache_lookup(keys, 4, pb, &hit) : nullptr;
   int rc = 0;
   if (Bp == nullptr) {
     StreamBlock blk;

@@ -778,12 +778,13 @@ class RENetInference:
             out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
         return out
 
-    def _observed_histories(self, ents, history, name, graph_dict, global_emb):
+    def _observed_histories(self, ents, history, name, graph_dict, global_emb, before=None, caller='evaluate_observed'):
         """evaluate_observed's histories of one direction, checked: ((hist, hist_t, hid, ent_of), has) -- the distinct
         histories (lists, timestamp lists), each triple's history id (-1 when empty), the entity of each history, and which
         triples have one.  A history is identified by its entity and timestamps, since the entries of one (entity, timestamp)
         must be equal wherever they appear (ValueError otherwise); ids ascend with the entity, as _encode_queries needs.
-        ValueError for entry ids out of range and for timestamps missing from graph_dict or global_emb."""
+        ValueError for entry ids out of range, for timestamps missing from graph_dict or global_emb, and with ``before``
+        (one timestamp per triple) for a history timestamp not before its triple's.  ValueErrors name ``caller``."""
         lists, times = history
         R, E = self.num_rels, self.in_dim
         seen = {}                                        # (entity, t) -> the first entry seen, as int64 [k, 2]
@@ -791,25 +792,29 @@ class RENetInference:
         hid = np.full(len(ents), -1, dtype=np.int64)
         for i, (e, hl, ht) in enumerate(zip(ents.tolist(), lists, times)):
             if len(hl) != len(ht):
-                raise ValueError('evaluate_observed: %s[%d] has %d entries but %d timestamps' % (name, i, len(hl), len(ht)))
+                raise ValueError('%s: %s[%d] has %d entries but %d timestamps' % (caller, name, i, len(hl), len(ht)))
             if len(hl) == 0:
                 continue
             ts = tuple(int(t) for t in ht)
+            if before is not None and max(ts) >= before[i]:
+                # a forecast may only see the past: an entry at or after the query's timestamp may hold its answer
+                raise ValueError('%s: %s[%d] holds timestamp %d, not before its query\'s timestamp %d'
+                                 % (caller, name, i, max(ts), before[i]))
             for a, t in zip(hl, ts):
                 prev = seen.get((e, t))
                 if prev is None:
                     if t not in graph_dict:
-                        raise ValueError('evaluate_observed: %s[%d] refers to timestamp %d, which graph_dict lacks' % (name, i, t))
+                        raise ValueError('%s: %s[%d] refers to timestamp %d, which graph_dict lacks' % (caller, name, i, t))
                     if t not in global_emb:
-                        raise ValueError('evaluate_observed: %s[%d] refers to timestamp %d, which global_emb lacks' % (name, i, t))
+                        raise ValueError('%s: %s[%d] refers to timestamp %d, which global_emb lacks' % (caller, name, i, t))
                     v = np.asarray(a, dtype=np.int64).reshape(-1, 2)
                     if len(v) and (v[:, 0].min() < 0 or v[:, 0].max() >= R or v[:, 1].min() < 0 or v[:, 1].max() >= E):
-                        raise ValueError('evaluate_observed: %s[%d] holds ids outside [0, %d) x [0, %d) at timestamp %d'
-                                         % (name, i, R, E, t))
+                        raise ValueError('%s: %s[%d] holds ids outside [0, %d) x [0, %d) at timestamp %d'
+                                         % (caller, name, i, R, E, t))
                     seen[(e, t)] = (a, v)
                 elif prev[0] is not a and not np.array_equal(prev[1], np.asarray(a, dtype=np.int64).reshape(-1, 2)):
-                    raise ValueError('evaluate_observed: %s[%d] holds an entry of entity %d at timestamp %d that differs from '
-                                     'another history\'s entry of the same entity and timestamp' % (name, i, e, t))
+                    raise ValueError('%s: %s[%d] holds an entry of entity %d at timestamp %d that differs from '
+                                     'another history\'s entry of the same entity and timestamp' % (caller, name, i, e, t))
             hid[i] = keys.setdefault((e, ts), i)
         order = sorted(keys.items())                     # by entity, then timestamps
         rank = {first: j for j, (_, first) in enumerate(order)}
@@ -1036,20 +1041,9 @@ class RENetInference:
 
         A model on the host takes the same control flow with _encode_one per query, materialised logits and a stable
         sort (topk_excluding_torch)."""
-        from .decoder import TOPK_MAX_K
-        q = torch.as_tensor(queries)
-        if q.dim() != 2 or q.shape[1] != 3 or q.dtype.is_floating_point:
-            raise ValueError('forecast: queries must be integer rows (entity, relation, timestamp), got %s %s'
-                             % (tuple(q.shape), q.dtype))
-        q = q.cpu().long()
-        qn = q.numpy()
+        qn = self._forecast_queries(queries, k, 'forecast')
+        q = torch.from_numpy(qn)
         n = len(qn)
-        if not 1 <= k <= min(self.in_dim, TOPK_MAX_K):
-            raise ValueError('forecast: k = %d outside [1, %d]' % (k, min(self.in_dim, TOPK_MAX_K)))
-        if n and (qn[:, 0].min() < 0 or qn[:, 0].max() >= self.in_dim):
-            raise ValueError('forecast: entity ids outside [0, %d)' % self.in_dim)
-        if n and (qn[:, 1].min() < 0 or qn[:, 1].max() >= self.num_rels):
-            raise ValueError('forecast: relation ids outside [0, %d)' % self.num_rels)
         if n and (np.any(np.diff(qn[:, 2]) < 0) or qn[0, 2] < int(self.latest_time)):
             raise ValueError('forecast: timestamps must be non-decreasing and not before latest_time = %d'
                              % int(self.latest_time))
@@ -1106,6 +1100,96 @@ class RENetInference:
                     v, c = shard.allgather_slices(v, m), shard.allgather_slices(c, m)
                 values[i0:i1], ids[i0:i1] = v, c
                 i0 = i1
+        return values, ids
+
+    def _forecast_queries(self, queries, k, caller):
+        """The forecast calls' checks on ``queries`` (integer rows (entity, relation, timestamp), ids in range) and ``k``;
+        ValueErrors name ``caller``.  Returns the queries as a host int64 array [n, 3]."""
+        from .decoder import TOPK_MAX_K
+        q = torch.as_tensor(queries)
+        if q.dim() != 2 or q.shape[1] != 3 or q.dtype.is_floating_point:
+            raise ValueError('%s: queries must be integer rows (entity, relation, timestamp), got %s %s'
+                             % (caller, tuple(q.shape), q.dtype))
+        qn = q.cpu().long().numpy()
+        n = len(qn)
+        if not 1 <= k <= min(self.in_dim, TOPK_MAX_K):
+            raise ValueError('%s: k = %d outside [1, %d]' % (caller, k, min(self.in_dim, TOPK_MAX_K)))
+        if n and (qn[:, 0].min() < 0 or qn[:, 0].max() >= self.in_dim):
+            raise ValueError('%s: entity ids outside [0, %d)' % (caller, self.in_dim))
+        if n and (qn[:, 1].min() < 0 or qn[:, 1].max() >= self.num_rels):
+            raise ValueError('%s: relation ids outside [0, %d)' % (caller, self.num_rels))
+        return qn
+
+    def forecast_observed(self, queries, history, graph_dict, global_emb, k=10, subject=True, known=None,
+                          time_aware=False):
+        """The model's k most likely answers of each query over observed history: forecast's result for queries whose
+        histories the caller knows, as evaluate_observed encodes a test triple from its own history.
+
+        ``queries``: int64 [n, 3] rows (entity, relation, timestamp), in any order.  ``history`` = (lists, timestamp lists),
+        one entry per query: the entity's subject-side history for ``subject=True``, its object-side one otherwise, in the
+        format evaluate_observed takes (e.g. synthetic.observed_history of the known facts).  Every timestamp of a query's
+        history must be before the query's own timestamp.  ``graph_dict`` / ``global_emb``: the true graphs and global
+        embeddings of the timestamps those histories reference, as evaluate_observed takes them.
+
+        Returns forecast's result: (values float32 [n, k], entity ids int64 [n, k]) on the model's device, p = softmax over
+        all entities, descending, ties to the lower id.  ``subject=True`` scores the objects of (e, r, ?, t) from
+        [ent_e | s_h | rel_r], ``False`` the subjects of (?, r, e, t) with the inverse relation embeddings; an empty history
+        gives a zero s_h.  ``known``: triples whose answers are left out of the lists but not out of the normaliser, or
+        with ``time_aware=True`` quadruples, of which only the answers known at the query's own t are left out.  A row
+        with fewer than k admissible answers ends in id -1 and value 0.
+
+        Nothing rolls over, nothing is sampled and the global model is not called: the test-time state, graph_dict,
+        global_emb, latest_time and torch's RNG stay as they were.  The model scores in eval mode and its mode is restored.
+        The distinct (entity, relation, history) queries are encoded once by _encode_queries (each (entity, timestamp)
+        component built once), and the rows are scored OBSERVED_RANK_ROWS at a time by renet_decoder_topk with one
+        exclusion list per row from a FilterIndex / TimeFilterIndex built once per call; a row's top-k depends on that row
+        alone, so the chunk size changes no bit.  Every ValueError -- evaluate_observed's checks on the histories, forecast's
+        on ``queries`` and ``k``, a history timestamp not before its query's -- comes before any work.  A model on the host
+        takes the same flow through _encode_one, ``linear`` and topk_excluding_torch."""
+        qn = self._forecast_queries(queries, k, 'forecast_observed')
+        n = len(qn)
+        if len(history) != 2 or len(history[0]) != n or len(history[1]) != n:
+            raise ValueError('forecast_observed: history must be (lists, timestamp lists) of %d queries' % n)
+        if known is not None:
+            kt = torch.as_tensor(known)
+            if kt.dim() != 2 or kt.shape[1] < (4 if time_aware else 3):
+                raise ValueError('forecast_observed: known must be %s' % ('quadruples (s, r, o, t) with time_aware'
+                                                                          if time_aware else 'triples (s, r, o)'))
+        elif time_aware:
+            raise ValueError('forecast_observed: time_aware needs known quadruples (s, r, o, t)')
+        obs, has = self._observed_histories(qn[:, 0], history, 'history', graph_dict, global_emb, before=qn[:, 2],
+                                            caller='forecast_observed')
+        index = None
+        if known is not None:
+            index = TimeFilterIndex(known) if time_aware else FilterIndex(known)
+        dev = self.ent_embeds.device
+        direction = 'objects' if subject else 'subjects'
+        col = None
+        if index is not None:
+            col = index.col(direction)
+            if self.ent_embeds.is_cuda:
+                col = torch.from_numpy(col).to(dev)                  # once per call; each chunk sends its ranges
+        rel_embeds, _ = self._direction(subject)
+        values = torch.empty(n, k, device=dev)
+        ids = torch.empty(n, k, dtype=torch.long, device=dev)
+        modes = [(mod, mod.training) for mod in self.modules()]
+        self.eval()
+        try:
+            with torch.no_grad():
+                s_h = self._encode_queries(qn[:, 0], qn[:, 1], has, subject, history=obs, graphs=(graph_dict, global_emb))
+                for i0 in range(0, n, OBSERVED_RANK_ROWS):
+                    i1 = min(i0 + OBSERVED_RANK_ROWS, n)
+                    e, r = qn[i0:i1, 0], qn[i0:i1, 1]
+                    x = torch.cat((self.ent_embeds[torch.from_numpy(e).to(dev)], s_h[i0:i1],
+                                   rel_embeds[torch.from_numpy(r).to(dev)]), dim=1)
+                    exclude = None
+                    if index is not None:
+                        key = (e, r) + ((qn[i0:i1, 2],) if time_aware else ())
+                        exclude = (col,) + index.ranges(direction, *key)
+                    values[i0:i1], ids[i0:i1] = self._topk_rows(x, k, exclude)
+        finally:
+            for mod, mode in modes:
+                mod.training = mode
         return values, ids
 
     def _topk_rows(self, x, k, exclude):

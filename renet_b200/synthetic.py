@@ -109,6 +109,50 @@ def build_history(quads, history_len=10):
     return S, ST, O, OT
 
 
+def observed_history(facts, entities, timestamps, subject=True, history_len=10):
+    """The history window of each (entities[i], timestamps[i]) over the known quadruples ``facts``: the reference's
+    history of that entity at that time (get_history_graph.py:142-190), for any entity and time, not only those of a
+    stream's quadruples.  It holds the last ``history_len`` distinct timestamps before t at which the entity is the subject
+    of a fact (``subject=True``; its object otherwise), each entry an int64 array [k, 2] of (relation, other entity) in
+    the facts' order.  Returns (lists, timestamp lists), one per query, as RENet.evaluate_observed and
+    RENet.forecast_observed take them; for every quadruple of a time-sorted stream they equal build_history's.  The entry
+    of one (entity, timestamp) is one array object, shared by every window that holds it, as in the reference's pickles.
+
+    Vectorised: one stable sort of the facts by (entity, timestamp), whose runs are the entries, and one searchsorted per
+    query for its window of runs; only the runs some window holds become arrays."""
+    f = np.asarray(facts, dtype=np.int64)
+    if f.ndim != 2 or f.shape[1] < 4:
+        raise ValueError('observed_history: facts must be quadruples (s, r, o, t)')
+    ents = np.asarray(entities, dtype=np.int64).reshape(-1)
+    ts = np.asarray(timestamps, dtype=np.int64).reshape(-1)
+    if len(ents) != len(ts):
+        raise ValueError('observed_history: %d entities but %d timestamps' % (len(ents), len(ts)))
+    if history_len < 1:
+        raise ValueError('observed_history: history_len = %d, needs at least 1' % history_len)
+    ent, other = (f[:, 0], f[:, 2]) if subject else (f[:, 2], f[:, 0])
+    times, pos = np.unique(f[:, 3], return_inverse=True)
+    T = len(times) + 1                                   # a query's position among the timestamps is at most len(times)
+    key = ent * T + pos.reshape(-1)
+    order = np.argsort(key, kind='stable')
+    key = key[order]
+    pairs = np.stack((f[order, 1], other[order]), axis=1)
+    start = np.flatnonzero(np.concatenate(([True], key[1:] != key[:-1]))) if len(key) else np.zeros(0, np.int64)
+    stop = np.append(start[1:], len(key))
+    run_key = key[start]
+    # the runs of entity e before t: keys in [e * T, e * T + #timestamps < t), the last history_len of them
+    hi = np.searchsorted(run_key, ents * T + np.searchsorted(times, ts, 'left'), 'left')
+    lo = np.maximum(np.searchsorted(run_key, ents * T, 'left'), hi - history_len)
+    cover = np.zeros(len(start) + 1, dtype=np.int64)
+    np.add.at(cover, lo, 1)
+    np.add.at(cover, hi, -1)
+    entry = [None] * len(start)
+    for j in np.flatnonzero(np.cumsum(cover[:-1]) > 0).tolist():
+        entry[j] = pairs[start[j]:stop[j]]
+    run_t = times[run_key % T].tolist()
+    lists = [entry[a:b] for a, b in zip(lo.tolist(), hi.tolist())]
+    return lists, [run_t[a:b] for a, b in zip(lo.tolist(), hi.tolist())]
+
+
 class SyntheticTKG:
     """quads + graph_dict + histories + a global_emb stand-in, ready for RENet.forward."""
 
