@@ -197,6 +197,62 @@ class TimeFilterIndex:
         return self.dirs[direction][1]
 
 
+class RelationFilterIndex:
+    """The known relations of every entity, built once from known facts: for an entity e as a subject, the r of every known
+    (e, r, .); as an object, the r of every known (., r, e) -- the relations the filtered relation ranks leave out of a
+    query (e, ?).  With ``time_aware=True`` (quadruples) keyed by (entity, timestamp): only the relations known at the
+    query's own t.  Per side one int32 column array of the sorted distinct relations, grouped by key, and the keys sorted
+    ascending; ``ranges(subject, entity[, t])`` and ``col(subject)`` give the CSR lists the rank and top-k kernels take."""
+
+    def __init__(self, facts, time_aware=False):
+        f = np.asarray(torch.as_tensor(facts).cpu().numpy(), dtype=np.int64)
+        if f.ndim != 2 or f.shape[1] < (4 if time_aware else 3):
+            raise ValueError('RelationFilterIndex needs %s' % ('quadruples (s, r, o, t)' if time_aware else 'triples (s, r, o)'))
+        self.time_aware = time_aware
+        self.times = np.unique(f[:, 3]) if time_aware else np.zeros(0, dtype=np.int64)
+        self.T = max(len(self.times), 1)
+        pos = np.searchsorted(self.times, f[:, 3]) if time_aware else 0
+        self.sides = {}
+        for subject, fix in ((True, 0), (False, 2)):
+            key = f[:, fix] * self.T + pos
+            order = np.lexsort((f[:, 1], key))
+            k, r = key[order], f[order, 1]
+            keep = np.ones(len(k), dtype=bool)
+            keep[1:] = (k[1:] != k[:-1]) | (r[1:] != r[:-1])             # distinct (key, relation) pairs
+            self.sides[subject] = (k[keep], np.ascontiguousarray(r[keep], dtype=np.int32))
+
+    def ranges(self, subject, entity, t=None):
+        """(begin, end) int64 arrays: the known relations of entity[i] (at t[i] when time-aware) on the given side are
+        col(subject)[begin[i]:end[i]]; absent keys give empty ranges."""
+        keys, _ = self.sides[bool(subject)]
+        e = np.asarray(entity, dtype=np.int64)
+        ok = e >= 0
+        if self.time_aware:
+            t = np.broadcast_to(np.asarray(t, dtype=np.int64), e.shape)
+            if len(self.times) == 0:
+                z = np.zeros(e.shape, dtype=np.int64)
+                return z, z
+            pos = np.minimum(np.searchsorted(self.times, t), len(self.times) - 1)
+            ok &= self.times[pos] == t
+            k = np.where(ok, np.where(ok, e, 0) * self.T + pos, -1)
+        else:
+            k = np.where(ok, e, -1)
+        return np.searchsorted(keys, k, 'left'), np.searchsorted(keys, k, 'right')
+
+    def col(self, subject):
+        return self.sides[bool(subject)][1]
+
+
+def _relation_exclusions(index, ents, subject, *t):
+    """(col, begin, end) of per-row exclusion lists from a RelationFilterIndex: row i's list is the known relations of
+    ents[i] (at t[i] when time-aware) on the subject side where subject[i], else on the object side; col holds both sides."""
+    b_s, e_s = index.ranges(True, ents, *t)
+    b_o, e_o = index.ranges(False, ents, *t)
+    off = len(index.col(True))
+    col = np.concatenate((index.col(True), index.col(False)))
+    return col, np.where(subject, b_s, b_o + off), np.where(subject, e_s, e_o + off)
+
+
 def rank_counts_torch(z, label, exclude=None):
     """What renet_decoder_rank counts, on materialised logits z [M, N] with torch: int64 [M, 4] = (#z > z_l, #z == z_l,
     #p > p_l, #p == p_l), p = torch.sigmoid(z) with row m's excluded columns other than its label set to 0 (the last two
@@ -295,18 +351,19 @@ class RENetInference:
         R = self.num_rels
         return (self.rel_embeds[:R], False) if subject else (self.rel_embeds[R:], True)
 
-    def _encode_one(self, entity, r, history, history_t, subject, graph_dict=None, global_emb=None):
+    def _encode_one(self, entity, r, history, history_t, subject, graph_dict=None, global_emb=None, relation=False):
         """Final hidden state of `encoder` for ONE (entity, relation) history (aggregator.predict + encoder,
-        model.py:333-351), over the model's graph_dict / global_emb unless others are given."""
+        model.py:333-351), over the model's graph_dict / global_emb unless others are given.  ``relation=True``: the final
+        state s_q of `encoder_r` instead (aggregator.predict's inp_r, model.py:94-96,200-204), which does not depend on r."""
         rel_embeds, reverse = self._direction(subject)
         dev = self.ent_embeds.device
         e = torch.as_tensor(entity, device=dev).view(1)
         rr = torch.as_tensor(r, device=dev).view(1)
-        s_h, _, _ = self.aggregator.encode(([history], [history_t]), e, rr, self.ent_embeds, rel_embeds,
-                                           self.graph_dict if graph_dict is None else graph_dict,
-                                           self.global_emb if global_emb is None else global_emb, reverse, self.encoder,
-                                           self.encoder_r)
-        return s_h.view(-1)
+        s_h, s_q, _ = self.aggregator.encode(([history], [history_t]), e, rr, self.ent_embeds, rel_embeds,
+                                             self.graph_dict if graph_dict is None else graph_dict,
+                                             self.global_emb if global_emb is None else global_emb, reverse, self.encoder,
+                                             self.encoder_r)
+        return (s_q if relation else s_h).view(-1)
 
     def pred_r_rank2(self, s, r, subject=True):
         """model.py:168-213: joint distribution over (relation, other entity) for entity s[0]:
@@ -730,24 +787,9 @@ class RENetInference:
         whose length differs from the test data's, ids out of range, history timestamps missing from graph_dict or
         global_emb, and ``time_aware`` without quadruples -- all before any work.  A model on the host takes the same flow
         through _encode_one and materialised logits."""
-        test_data = torch.as_tensor(test_data)
-        if test_data.dim() != 2 or test_data.shape[1] < 4:
-            raise ValueError('evaluate_observed: test_data must be quadruples (s, r, o, t)')
-        quads = test_data.cpu().numpy().astype(np.int64)
+        quads, (s_obs, has_s), (o_obs, has_o) = self._observed_split(test_data, s_history, o_history, graph_dict, global_emb,
+                                                                     total_data, raw, time_aware, 'evaluate_observed')
         n = len(quads)
-        if time_aware:
-            _quadruples(total_data)
-        if (not raw or time_aware) and total_data is None:
-            raise ValueError('filtered evaluation needs total_data (all known triples)')
-        for name, hist in (('s_history', s_history), ('o_history', o_history)):
-            if len(hist) != 2 or len(hist[0]) != n or len(hist[1]) != n:
-                raise ValueError('evaluate_observed: %s must be (lists, timestamp lists) of %d test triples' % (name, n))
-        if n and (min(quads[:, 0].min(), quads[:, 2].min()) < 0 or max(quads[:, 0].max(), quads[:, 2].max()) >= self.in_dim):
-            raise ValueError('evaluate_observed: entity ids outside [0, %d)' % self.in_dim)
-        if n and (quads[:, 1].min() < 0 or quads[:, 1].max() >= self.num_rels):
-            raise ValueError('evaluate_observed: relation ids outside [0, %d)' % self.num_rels)
-        s_obs, has_s = self._observed_histories(quads[:, 0], s_history, 's_history', graph_dict, global_emb)
-        o_obs, has_o = self._observed_histories(quads[:, 2], o_history, 'o_history', graph_dict, global_emb)
         tfidx = TimeFilterIndex(_quadruples(total_data)) if time_aware else None
         fidx = FilterIndex(total_data) if not raw or time_aware else None
         protocols = {k: [] for k in PROTOCOLS}
@@ -770,6 +812,102 @@ class RENetInference:
                         r = r['raw' if raw else 'filtered']
                     ranks.append(r)
                     total_loss += float(np.sum(loss.astype(np.float64)))
+        finally:
+            for mod, mode in modes:
+                mod.training = mode
+        out = stream_metrics(ranks, total_loss)
+        if time_aware:
+            out['protocols'] = {k: stream_metrics(v, total_loss) for k, v in protocols.items()}
+        return out
+
+    def _observed_split(self, test_data, s_history, o_history, graph_dict, global_emb, total_data, raw, time_aware, caller):
+        """The checks of an observed-history evaluation, all before any work: (quads int64 [n, 4], (s_obs, has_s),
+        (o_obs, has_o)) with each direction's histories as _observed_histories returns them.  ValueErrors name ``caller``."""
+        test_data = torch.as_tensor(test_data)
+        if test_data.dim() != 2 or test_data.shape[1] < 4:
+            raise ValueError('%s: test_data must be quadruples (s, r, o, t)' % caller)
+        quads = test_data.cpu().numpy().astype(np.int64)
+        n = len(quads)
+        if time_aware:
+            _quadruples(total_data)
+        if (not raw or time_aware) and total_data is None:
+            raise ValueError('filtered evaluation needs total_data (all known triples)')
+        for name, hist in (('s_history', s_history), ('o_history', o_history)):
+            if len(hist) != 2 or len(hist[0]) != n or len(hist[1]) != n:
+                raise ValueError('%s: %s must be (lists, timestamp lists) of %d test triples' % (caller, name, n))
+        if n and (min(quads[:, 0].min(), quads[:, 2].min()) < 0 or max(quads[:, 0].max(), quads[:, 2].max()) >= self.in_dim):
+            raise ValueError('%s: entity ids outside [0, %d)' % (caller, self.in_dim))
+        if n and (quads[:, 1].min() < 0 or quads[:, 1].max() >= self.num_rels):
+            raise ValueError('%s: relation ids outside [0, %d)' % (caller, self.num_rels))
+        s = self._observed_histories(quads[:, 0], s_history, 's_history', graph_dict, global_emb, caller=caller)
+        o = self._observed_histories(quads[:, 2], o_history, 'o_history', graph_dict, global_emb, caller=caller)
+        return quads, s, o
+
+    def evaluate_relations_observed(self, test_data, s_history, o_history, graph_dict, global_emb, total_data=None, raw=False,
+                                    time_aware=False):
+        """The relation head over observed history: how well p(r | s, history) -- what ``encoder_r`` + ``linear_r`` learn
+        through training's 0.1-weighted relation loss (model.py:94-100) -- ranks the true relation of each test triple.
+        Arguments, checks and result dict are evaluate_observed's.
+
+        Per triple (s, r, o, t) two rows, each ranking the label r among all num_rels relations: the subject row
+        linear_r([ent_s | s_q]), s_q the final state of ``encoder_r`` over s's own history (aggregator.predict's inp_r,
+        reverse=False), and the object row linear_r([ent_o | o_q]) over o's object-side history (reverse=True), as
+        forward(subject=False) trains it; an empty history gives a zero state (pred_r_rank2, model.py:187-189).  Ranks use
+        the reference's tie rule: raw on the logits, filtered and time-aware filtered on the sigmoids with every other
+        relation known for the row's entity on its side -- (s, r', .) for the subject row, (., r', o) for the object row --
+        zeroed (RelationFilterIndex of ``total_data``, the time-aware one keyed at the row's own t).  ``ranks`` holds
+        [subject row, object row] per triple and ``loss`` the sum of both rows' relation cross-entropies.
+
+        Nothing rolls over, nothing is sampled and the global model is not called: the test-time state and torch's RNG are
+        left as they are.  The model scores in eval mode and its mode is restored.  s_q does not depend on r, so each
+        direction encodes each distinct (entity, history) once, through _encode_queries' chunks; the rows are ranked
+        OBSERVED_RANK_ROWS at a time by renet_decoder_rank_multi against ``linear_r``.  A model on the host takes the same
+        flow through _encode_one and materialised logits."""
+        from .decoder import ranks_from_counts
+        quads, (s_obs, has_s), (o_obs, has_o) = self._observed_split(test_data, s_history, o_history, graph_dict, global_emb,
+                                                                     total_data, raw, time_aware,
+                                                                     'evaluate_relations_observed')
+        n = len(quads)
+        indexes = []                                           # the static filter, then the time-aware one
+        if not raw or time_aware:
+            indexes.append(RelationFilterIndex(total_data))
+        if time_aware:
+            indexes.append(RelationFilterIndex(_quadruples(total_data), time_aware=True))
+        dev = self.ent_embeds.device
+        protocols = {k: [] for k in PROTOCOLS}
+        ranks, total_loss = [], 0.0
+        modes = [(mod, mod.training) for mod in self.modules()]
+        self.eval()
+        try:
+            with torch.no_grad():
+                graphs = (graph_dict, global_emb)
+                s_q = self._encode_queries(quads[:, 0], None, has_s, True, history=s_obs, graphs=graphs,
+                                           relation=True)
+                o_q = self._encode_queries(quads[:, 2], None, has_o, False, history=o_obs, graphs=graphs,
+                                           relation=True)
+                per = max(1, OBSERVED_RANK_ROWS // 2)
+                for i0 in range(0, n, per):
+                    i1 = min(i0 + per, n)
+                    q = quads[i0:i1]
+                    m = i1 - i0
+                    ents = np.concatenate((q[:, 0], q[:, 2]))
+                    x = torch.cat((self.ent_embeds[torch.from_numpy(ents).to(dev)], torch.cat((s_q[i0:i1], o_q[i0:i1]))),
+                                  dim=1)
+                    side = np.concatenate((np.ones(m, bool), np.zeros(m, bool)))
+                    t2 = np.concatenate((q[:, 3], q[:, 3]))
+                    excludes = [_relation_exclusions(ix, ents, side, *((t2,) if ix.time_aware else ())) for ix in indexes]
+                    loss_rows, counts = self._rank_rows(x, np.concatenate((q[:, 1], q[:, 1])), excludes, self.linear_r)
+                    rks = [ranks_from_counts(counts[:, 2 * j], counts[:, 2 * j + 1]).cpu().numpy()
+                           for j in range(len(excludes) + 1)]
+                    pair = [np.stack((rk[:m], rk[m:]), axis=1).reshape(-1) for rk in rks]    # [subject, object] per triple
+                    if time_aware:
+                        for k, rk in zip(PROTOCOLS, pair):
+                            protocols[k].append(rk)
+                        ranks.append(pair[0] if raw else pair[1])
+                    else:
+                        ranks.append(pair[-1])
+                    lr = loss_rows.cpu().numpy().astype(np.float32)
+                    total_loss += float(np.sum((lr[:m] + lr[m:]).astype(np.float64)))
         finally:
             for mod, mode in modes:
                 mod.training = mode
@@ -919,11 +1057,13 @@ class RENetInference:
         lr = loss_rows.cpu().numpy().astype(np.float32)
         return ranks, lr[loss_row[:n]] + lr[loss_row[n:]]
 
-    def _rank_rows(self, x, label, excludes):
-        """(loss_rows [M], counts [M, 2 + 2L]) of the rows of x against ``linear``: the raw (greater, equal) pair, then the
-        filtered pair against each of the L = 0-2 exclusion lists ``excludes``.  One renet_decoder_rank_multi call on the
-        GPU; on the host, row by row through ``linear`` as predict computes them, counted with torch once per list."""
+    def _rank_rows(self, x, label, excludes, linear=None):
+        """(loss_rows [M], counts [M, 2 + 2L]) of the rows of x against ``linear`` (the entity head's unless another is
+        given): the raw (greater, equal) pair, then the filtered pair against each of the L = 0-2 exclusion lists
+        ``excludes``.  One renet_decoder_rank_multi call on the GPU; on the host, row by row through ``linear`` as predict
+        computes them, counted with torch once per list."""
         from .decoder import decoder_rank_counts_multi
+        linear = self.linear if linear is None else linear
         dev = x.device
         lab = torch.from_numpy(np.ascontiguousarray(label, dtype=np.int64)).to(dev)
         if len(lab) == 0:
@@ -933,26 +1073,32 @@ class RENetInference:
                     torch.zeros(0, 2 + 2 * len(excludes), dtype=torch.int32 if x.is_cuda else torch.long, device=dev))
         if x.is_cuda:
             ex = [tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev) for a in e) for e in excludes]
-            return decoder_rank_counts_multi(x, self.linear.weight, self.linear.bias, lab, ex)
-        z = torch.stack([self.linear(row) for row in x])
+            return decoder_rank_counts_multi(x, linear.weight, linear.bias, lab, ex)
+        z = torch.stack([linear(row) for row in x])
         loss_rows = torch.stack([self.criterion(z[m].view(1, -1), lab[m].view(1)) for m in range(len(lab))])
         cs = [rank_counts_torch(z, lab, e) for e in excludes]
         return loss_rows, torch.cat([rank_counts_torch(z, lab)[:, :2]] + [ci[:, 2:] for ci in cs], dim=1)
 
-    def _encode_queries(self, ents, rels, has, subject, shard=None, history=None, graphs=None):
+    def _encode_queries(self, ents, rels, has, subject, shard=None, history=None, graphs=None, relation=False):
         """s_h [n, h] of the queries (ents[i], rels[i]); rows where ``has`` is False stay zero (predict's empty-history
         rule).  Query i's history is the current test-time history of ents[i], or with ``history`` = (hist, hist_t, hid,
         ent_of) the history hist[hid[i]] / hist_t[hid[i]], whose entity is ent_of[hid[i]] (= ents[i]), over ``graphs`` =
         (graph_dict, global_emb) instead of the model's.  Equal queries (history, relation) are encoded once.  On the GPU the
         distinct queries go through the device batcher in chunks, one isolation group per entity, so that each equals
         _encode_one's encoding of it alone; on the host, through _encode_one, one query per chunk.  With a ``shard`` chunk j
-        runs on rank j mod world and every rank all-gathers the encodings."""
+        runs on rank j mod world and every rank all-gathers the encodings.
+
+        ``relation=True``: the relation head's s_q [n, h] instead, the final state of ``encoder_r`` that the same fused pass
+        computes.  s_q does not depend on the relation (its inputs are [H2 | ent | global], model.py:94-96), so ``rels`` is
+        ignored and each distinct history is encoded once."""
         h, R = self.h_dim, self.num_rels
         dev = self.ent_embeds.device
         out = torch.zeros(len(ents), h, device=dev)
         sel = np.flatnonzero(has)
         if len(sel) == 0:
             return out
+        if relation:
+            rels = np.zeros(len(ents), dtype=np.int64)
         graph_dict, global_emb = (self.graph_dict, self.global_emb) if graphs is None else graphs
         if history is None:
             hist = self.s_hist_test if subject else self.o_hist_test
@@ -993,18 +1139,19 @@ class RENetInference:
         for j0, j1 in (chunks[c] for c in (range(len(chunks)) if shard is None else shard.units(len(chunks)))):
             if not self.ent_embeds.is_cuda:
                 hh, e, rr = int(q_h[j0]), int(q_e[j0]), int(q_r[j0])
-                parts.append(self._encode_one(e, rr, hist[hh], hist_t[hh], subject, graph_dict, global_emb)
+                parts.append(self._encode_one(e, rr, hist[hh], hist_t[hh], subject, graph_dict, global_emb, relation)
                              .view(1, h).to(out.dtype))
                 continue
             view, gs = _chunk_view(hist, hist_t, q_h[j0:j1], q_e[j0:j1], graph_dict)
             s_dev = torch.from_numpy(q_e[j0:j1]).to(dev)
             r_dev = torch.from_numpy(q_r[j0:j1]).to(dev)
-            sh, _, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, global_emb,
-                                               reverse, self.encoder, self.encoder_r)
+            sh, sq, hb = self.aggregator.encode(view, s_dev, r_dev, self.ent_embeds, rel_embeds, gs, global_emb,
+                                                reverse, self.encoder, self.encoder_r)
+            state = sq if relation else sh
             # the encoder returns the sequences length-sorted: row k is sample sample_order[k] of the view
             idx = hb.sample_order(dev)
-            part = torch.empty_like(sh)
-            part[idx] = sh
+            part = torch.empty_like(state)
+            part[idx] = state
             parts.append(part)
         if shard is not None:
             parts = shard.gather_units(parts, [j1 - j0 for j0, j1 in chunks], out[:0])
@@ -1041,82 +1188,139 @@ class RENetInference:
 
         A model on the host takes the same control flow with _encode_one per query, materialised logits and a stable
         sort (topk_excluding_torch)."""
-        qn = self._forecast_queries(queries, k, 'forecast')
+        return self._forecast_stream(self._forecast_queries(queries, k, 'forecast'), global_model, k, subject, known,
+                                     time_aware, process_group, 'forecast')
+
+    def forecast_relations(self, queries, global_model, k=10, subject=True, known=None, time_aware=False,
+                           process_group=None):
+        """The model's k most likely next relations of each entity, over its own test-time state: the relation head's
+        p(r | e, history) = softmax(linear_r([ent_e | s_q])), the distribution pred_r_rank2 weighs the roll-over's
+        candidates with (model.py:202-208).
+
+        ``queries``: int64 [n, 2] rows (entity, timestamp), timestamps non-decreasing and not before ``latest_time``.
+        ``subject=True`` asks which relation e takes part in next as a subject, (e, ?, ., t), from its subject-side
+        test-time history; ``False`` as an object, (., ?, e, t), from its object-side history.  Returns (values float32
+        [n, k], relation ids int64 [n, k]) on the model's device, p = softmax over all num_rels relations, descending, ties
+        to the lower id; an empty history gives a zero s_q (model.py:187-189).  ``known``: triples (or quadruples with
+        ``time_aware``) whose relations are left out of each entity's list -- every relation of a known (e, r, .) (or
+        (., r, e)), or only those known at the query's own t -- but not out of the softmax; a row with fewer than k
+        admissible relations ends in id -1 and value 0.
+
+        forecast's contract otherwise: each timestamp change rolls over through the same _roll_over, leaving the same
+        state and RNG stream as forecast; ``process_group`` shards the encoding chunks and top-k rows in the same way and
+        every rank returns the one-process result bit for bit.  s_q does not depend on the relation, so each distinct
+        entity of a run is encoded once, and the rows are scored by one renet_decoder_topk call against ``linear_r``."""
+        return self._forecast_stream(self._forecast_queries(queries, k, 'forecast_relations', relations=True), global_model,
+                                     k, subject, known, time_aware, process_group, 'forecast_relations')
+
+    def _forecast_stream(self, qn, global_model, k, subject, known, time_aware, process_group, caller):
+        """forecast (qn int64 [n, 3] of (entity, relation, timestamp)) or forecast_relations (qn [n, 2] of (entity,
+        timestamp)) over the test-time state, after _forecast_queries' checks; ValueErrors name ``caller``."""
+        relation = qn.shape[1] == 2
         q = torch.from_numpy(qn)
         n = len(qn)
-        if n and (np.any(np.diff(qn[:, 2]) < 0) or qn[0, 2] < int(self.latest_time)):
-            raise ValueError('forecast: timestamps must be non-decreasing and not before latest_time = %d'
-                             % int(self.latest_time))
+        if n and (np.any(np.diff(qn[:, -1]) < 0) or qn[0, -1] < int(self.latest_time)):
+            raise ValueError('%s: timestamps must be non-decreasing and not before latest_time = %d'
+                             % (caller, int(self.latest_time)))
         if time_aware and known is None:
-            raise ValueError('forecast: time_aware needs known quadruples (s, r, o, t)')
-        shard = self._eval_shard(process_group, 'forecast')
+            raise ValueError('%s: time_aware needs known quadruples (s, r, o, t)' % caller)
+        shard = self._eval_shard(process_group, caller)
         if shard is not None:
             import hashlib
             digest = int.from_bytes(hashlib.blake2b(np.ascontiguousarray(qn).tobytes(), digest_size=7).digest(), 'little')
             fp = [n, digest, int(self.latest_time), int(self.num_k), int(k), int(bool(subject)), int(bool(time_aware)),
                   -1 if known is None else len(known)]
             if not shard.same_everywhere(fp):
-                raise ValueError('forecast: the ranks of process_group were called with different queries, latest_time, '
-                                 'num_k, k or flags')
+                raise ValueError('%s: the ranks of process_group were called with different queries, latest_time, '
+                                 'num_k, k or flags' % caller)
         self._trim_test_histories()
-        index = None
-        if known is not None:
-            index = TimeFilterIndex(_quadruples(known)) if time_aware else FilterIndex(known)
-        dev = self.ent_embeds.device
-        direction = 'objects' if subject else 'subjects'
-        col = None
-        if index is not None:
-            col = index.col(direction)
-            if self.ent_embeds.is_cuda:
-                col = torch.from_numpy(col).to(dev)                  # once per call; each run sends its ranges
-        rel_embeds, _ = self._direction(subject)
+        index, col = self._forecast_index(known, time_aware, subject, relation, True)
         hist = self.s_hist_test if subject else self.o_hist_test
+        dev = self.ent_embeds.device
         values = torch.empty(n, k, device=dev)
         ids = torch.empty(n, k, dtype=torch.long, device=dev)
         with torch.no_grad():
             i0 = 0
             while i0 < n:
                 i1 = i0 + 1
-                while i1 < n and qn[i1, 2] == qn[i0, 2]:
+                while i1 < n and qn[i1, -1] == qn[i0, -1]:
                     i1 += 1
-                t = q[i0, 2]
+                t = q[i0, -1]
                 if self.latest_time != t:
                     self._roll_over(t, global_model, shard)
-                e, r = qn[i0:i1, 0], qn[i0:i1, 1]
+                e, r = qn[i0:i1, 0], (None if relation else qn[i0:i1, 1])      # the relation head takes no relation
                 has = np.asarray([len(hist[x]) != 0 for x in e], dtype=bool)
-                s_h = self._encode_queries(e, r, has, subject, shard)
-                x = torch.cat((self.ent_embeds[torch.from_numpy(e).to(dev)], s_h, rel_embeds[torch.from_numpy(r).to(dev)]),
-                              dim=1)
+                state = self._encode_queries(e, r, has, subject, shard, relation=relation)
+                x = self._forecast_rows(e, r, state, subject, relation)
                 # a row's top-k depends on that row alone (no split-K, no kernel choice by row count, per-row steps after
                 # the GEMM), so a shard scores a contiguous slice of the rows with the lists of its rows only
                 m = i1 - i0
                 lo, hi = (0, m) if shard is None else shard.slice(m)
-                exclude = None
-                if index is not None:
-                    key = (e[lo:hi], r[lo:hi]) + ((np.full(hi - lo, int(t)),) if time_aware else ())
-                    exclude = (col,) + index.ranges(direction, *key)
-                v, c = self._topk_rows(x[lo:hi], k, exclude)
+                exclude = self._forecast_exclude(index, col, subject, relation, e[lo:hi], None if relation else r[lo:hi],
+                                                 np.full(hi - lo, int(t)) if time_aware else None)
+                v, c = self._topk_rows(x[lo:hi], k, exclude, self.linear_r if relation else None)
                 if shard is not None:
                     v, c = shard.allgather_slices(v, m), shard.allgather_slices(c, m)
                 values[i0:i1], ids[i0:i1] = v, c
                 i0 = i1
         return values, ids
 
-    def _forecast_queries(self, queries, k, caller):
-        """The forecast calls' checks on ``queries`` (integer rows (entity, relation, timestamp), ids in range) and ``k``;
-        ValueErrors name ``caller``.  Returns the queries as a host int64 array [n, 3]."""
+    def _forecast_index(self, known, time_aware, subject, relation, check_quadruples=False):
+        """(index, col) of a forecast's known facts: a FilterIndex / TimeFilterIndex (a RelationFilterIndex for the relation
+        head) and its column array for the queried side, on the model's device when it is a GPU (sent once per call; each
+        chunk sends its ranges), or (None, None) without ``known``."""
+        if known is None:
+            return None, None
+        if time_aware and check_quadruples:
+            known = _quadruples(known)
+        if relation:
+            index = RelationFilterIndex(known, time_aware)
+            col = index.col(subject)
+        else:
+            index = TimeFilterIndex(known) if time_aware else FilterIndex(known)
+            col = index.col('objects' if subject else 'subjects')
+        if self.ent_embeds.is_cuda:
+            col = torch.from_numpy(col).to(self.ent_embeds.device)
+        return index, col
+
+    def _forecast_rows(self, e, r, state, subject, relation):
+        """The decoder rows of forecast queries with entities e and relations r (host arrays) and their encoder states:
+        [ent_e | s_h | rel_r] for the entity head (inverse relation embeddings for subject=False), [ent_e | s_q] for the
+        relation head."""
+        dev = self.ent_embeds.device
+        ent = self.ent_embeds[torch.from_numpy(e).to(dev)]
+        if relation:
+            return torch.cat((ent, state), dim=1)
+        rel_embeds, _ = self._direction(subject)
+        return torch.cat((ent, state, rel_embeds[torch.from_numpy(r).to(dev)]), dim=1)
+
+    def _forecast_exclude(self, index, col, subject, relation, e, r, t):
+        """(col, begin, end) of forecast rows with entities e, relations r and, time-aware, timestamps t (else None), or
+        None without an index."""
+        if index is None:
+            return None
+        tt = () if t is None else (t,)
+        if relation:
+            return (col,) + index.ranges(subject, e, *tt)
+        return (col,) + index.ranges('objects' if subject else 'subjects', e, r, *tt)
+
+    def _forecast_queries(self, queries, k, caller, relations=False):
+        """The forecast calls' checks on ``queries`` (integer rows (entity, relation, timestamp), ids in range; with
+        ``relations``, rows (entity, timestamp)) and ``k`` (at most the number of answers: entities, or relations with
+        ``relations``); ValueErrors name ``caller``.  Returns the queries as a host int64 array [n, 3] ([n, 2])."""
         from .decoder import TOPK_MAX_K
         q = torch.as_tensor(queries)
-        if q.dim() != 2 or q.shape[1] != 3 or q.dtype.is_floating_point:
-            raise ValueError('%s: queries must be integer rows (entity, relation, timestamp), got %s %s'
-                             % (caller, tuple(q.shape), q.dtype))
+        cols, what = (2, '(entity, timestamp)') if relations else (3, '(entity, relation, timestamp)')
+        if q.dim() != 2 or q.shape[1] != cols or q.dtype.is_floating_point:
+            raise ValueError('%s: queries must be integer rows %s, got %s %s' % (caller, what, tuple(q.shape), q.dtype))
         qn = q.cpu().long().numpy()
         n = len(qn)
-        if not 1 <= k <= min(self.in_dim, TOPK_MAX_K):
-            raise ValueError('%s: k = %d outside [1, %d]' % (caller, k, min(self.in_dim, TOPK_MAX_K)))
+        top = min(self.num_rels if relations else self.in_dim, TOPK_MAX_K)
+        if not 1 <= k <= top:
+            raise ValueError('%s: k = %d outside [1, %d]' % (caller, k, top))
         if n and (qn[:, 0].min() < 0 or qn[:, 0].max() >= self.in_dim):
             raise ValueError('%s: entity ids outside [0, %d)' % (caller, self.in_dim))
-        if n and (qn[:, 1].min() < 0 or qn[:, 1].max() >= self.num_rels):
+        if not relations and n and (qn[:, 1].min() < 0 or qn[:, 1].max() >= self.num_rels):
             raise ValueError('%s: relation ids outside [0, %d)' % (caller, self.num_rels))
         return qn
 
@@ -1146,57 +1350,74 @@ class RENetInference:
         alone, so the chunk size changes no bit.  Every ValueError -- evaluate_observed's checks on the histories, forecast's
         on ``queries`` and ``k``, a history timestamp not before its query's -- comes before any work.  A model on the host
         takes the same flow through _encode_one, ``linear`` and topk_excluding_torch."""
-        qn = self._forecast_queries(queries, k, 'forecast_observed')
+        return self._forecast_from_history(self._forecast_queries(queries, k, 'forecast_observed'), history, graph_dict,
+                                           global_emb, k, subject, known, time_aware, 'forecast_observed')
+
+    def forecast_relations_observed(self, queries, history, graph_dict, global_emb, k=10, subject=True, known=None,
+                                    time_aware=False):
+        """The model's k most likely next relations of each entity over observed history: forecast_relations' result for
+        queries whose histories the caller knows, with forecast_observed's arguments and guarantees.
+
+        ``queries``: int64 [n, 2] rows (entity, timestamp), in any order.  ``history``: one window per query, the entity's
+        subject-side history for ``subject=True`` and its object-side one otherwise (e.g. synthetic.observed_history of the
+        known facts), every timestamp before the query's own.  Returns (values float32 [n, k], relation ids int64 [n, k]),
+        p = softmax(linear_r([ent_e | s_q])) over all num_rels relations, descending, ties to the lower id; an empty history
+        gives a zero s_q.  ``known`` (triples, or quadruples with ``time_aware``) leaves the entity's known relations on
+        that side out of the list but not out of the softmax; a row with fewer than k admissible relations ends in id -1
+        and value 0.
+
+        Nothing rolls over, nothing is sampled, the global model is not called, and the state, RNG and module mode are
+        left as they were.  Each distinct (entity, history) is encoded once by _encode_queries, and the rows are scored
+        OBSERVED_RANK_ROWS at a time by renet_decoder_topk against ``linear_r``.  Every ValueError comes before any work."""
+        return self._forecast_from_history(self._forecast_queries(queries, k, 'forecast_relations_observed', relations=True),
+                                           history, graph_dict, global_emb, k, subject, known, time_aware,
+                                           'forecast_relations_observed')
+
+    def _forecast_from_history(self, qn, history, graph_dict, global_emb, k, subject, known, time_aware, caller):
+        """forecast_observed (qn int64 [n, 3] of (entity, relation, timestamp)) or forecast_relations_observed (qn [n, 2] of
+        (entity, timestamp)) after _forecast_queries' checks; ValueErrors name ``caller``."""
+        relation = qn.shape[1] == 2
         n = len(qn)
         if len(history) != 2 or len(history[0]) != n or len(history[1]) != n:
-            raise ValueError('forecast_observed: history must be (lists, timestamp lists) of %d queries' % n)
+            raise ValueError('%s: history must be (lists, timestamp lists) of %d queries' % (caller, n))
         if known is not None:
             kt = torch.as_tensor(known)
             if kt.dim() != 2 or kt.shape[1] < (4 if time_aware else 3):
-                raise ValueError('forecast_observed: known must be %s' % ('quadruples (s, r, o, t) with time_aware'
-                                                                          if time_aware else 'triples (s, r, o)'))
+                raise ValueError('%s: known must be %s' % (caller, 'quadruples (s, r, o, t) with time_aware'
+                                                           if time_aware else 'triples (s, r, o)'))
         elif time_aware:
-            raise ValueError('forecast_observed: time_aware needs known quadruples (s, r, o, t)')
-        obs, has = self._observed_histories(qn[:, 0], history, 'history', graph_dict, global_emb, before=qn[:, 2],
-                                            caller='forecast_observed')
-        index = None
-        if known is not None:
-            index = TimeFilterIndex(known) if time_aware else FilterIndex(known)
+            raise ValueError('%s: time_aware needs known quadruples (s, r, o, t)' % caller)
+        obs, has = self._observed_histories(qn[:, 0], history, 'history', graph_dict, global_emb, before=qn[:, -1],
+                                            caller=caller)
+        index, col = self._forecast_index(known, time_aware, subject, relation)
         dev = self.ent_embeds.device
-        direction = 'objects' if subject else 'subjects'
-        col = None
-        if index is not None:
-            col = index.col(direction)
-            if self.ent_embeds.is_cuda:
-                col = torch.from_numpy(col).to(dev)                  # once per call; each chunk sends its ranges
-        rel_embeds, _ = self._direction(subject)
         values = torch.empty(n, k, device=dev)
         ids = torch.empty(n, k, dtype=torch.long, device=dev)
         modes = [(mod, mod.training) for mod in self.modules()]
         self.eval()
         try:
             with torch.no_grad():
-                s_h = self._encode_queries(qn[:, 0], qn[:, 1], has, subject, history=obs, graphs=(graph_dict, global_emb))
+                rels = None if relation else qn[:, 1]                           # the relation head takes no relation
+                state = self._encode_queries(qn[:, 0], rels, has, subject, history=obs, graphs=(graph_dict, global_emb),
+                                             relation=relation)
                 for i0 in range(0, n, OBSERVED_RANK_ROWS):
                     i1 = min(i0 + OBSERVED_RANK_ROWS, n)
-                    e, r = qn[i0:i1, 0], qn[i0:i1, 1]
-                    x = torch.cat((self.ent_embeds[torch.from_numpy(e).to(dev)], s_h[i0:i1],
-                                   rel_embeds[torch.from_numpy(r).to(dev)]), dim=1)
-                    exclude = None
-                    if index is not None:
-                        key = (e, r) + ((qn[i0:i1, 2],) if time_aware else ())
-                        exclude = (col,) + index.ranges(direction, *key)
-                    values[i0:i1], ids[i0:i1] = self._topk_rows(x, k, exclude)
+                    e, r = qn[i0:i1, 0], (None if relation else rels[i0:i1])
+                    x = self._forecast_rows(e, r, state[i0:i1], subject, relation)
+                    exclude = self._forecast_exclude(index, col, subject, relation, e, r,
+                                                     qn[i0:i1, -1] if time_aware else None)
+                    values[i0:i1], ids[i0:i1] = self._topk_rows(x, k, exclude, self.linear_r if relation else None)
         finally:
             for mod, mode in modes:
                 mod.training = mode
         return values, ids
 
-    def _topk_rows(self, x, k, exclude):
-        """(values [M, k], ids int64 [M, k]) of the rows of x against ``linear`` with the exclusion lists ``exclude`` =
-        (col, begin, end) or None: one renet_decoder_topk call on the GPU; on the host, row by row through ``linear`` as
-        predict computes them, then topk_excluding_torch."""
+    def _topk_rows(self, x, k, exclude, linear=None):
+        """(values [M, k], ids int64 [M, k]) of the rows of x against ``linear`` (the entity head's unless another is given)
+        with the exclusion lists ``exclude`` = (col, begin, end) or None: one renet_decoder_topk call on the GPU; on the
+        host, row by row through ``linear`` as predict computes them, then topk_excluding_torch."""
         from .decoder import decoder_topk
+        linear = self.linear if linear is None else linear
         dev = x.device
         if len(x) == 0:                  # a shard without rows: the empty results keep the dtypes the all-gather needs
             return torch.zeros(0, k, device=dev), torch.zeros(0, k, dtype=torch.long, device=dev)
@@ -1205,7 +1426,7 @@ class RENetInference:
             if exclude is not None:
                 ex = (exclude[0],) + tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev)
                                            for a in exclude[1:])
-            return decoder_topk(x, self.linear.weight, self.linear.bias, k, ex)
-        z = torch.stack([self.linear(row) for row in x])
+            return decoder_topk(x, linear.weight, linear.bias, k, ex)
+        z = torch.stack([linear(row) for row in x])
         return topk_excluding_torch(z, k, exclude)
 
