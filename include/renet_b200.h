@@ -237,10 +237,18 @@ int renet_scatter_add_rows(const float* src, const int32_t* index, float* dst,
  *   seq_len, seq_start [Q] (device, int32);  host_batch_sizes [max_len] (HOST: number of
  *   sequences active at step t -- what pack_padded_sequence computes, Aggregator.py:160-165);
  *   w_ih4 [3h,4h], w_hh4 [3h,h], b_ih4, b_hh4 [3h] : encoder;  *_3 : encoder_r ([3h,3h] ...)
- *   hn4, hn3 [Q,h] out.   workspace: renet_gru_workspace_bytes(S, Q, T, h) bytes; its contents
+ *   hn4, hn3 [Q,h] out.   workspace: renet_gru_workspace_bytes_len(S, Q, T, h, max_len) bytes; its contents
  *   after the call are what renet_gru_bwd needs (saved activations).
+ *
+ *   History length: the workspaces keep every step's recurrent pre-activations and hidden states, so they grow with
+ *   max_len.  The *_bytes_len entries size a call of max_len steps: at max_len <= 16 they equal the entries without
+ *   _len (which keep their signatures and always return the 16-step size), above 16 they grow by about
+ *   8h x 4 B x Q per step forward and 6h x 4 B x Q per step backward.  Every GRU entry refuses a workspace smaller than
+ *   its max_len needs (RENET_ERR_INVALID_ARG) before it launches anything.  Up to 64 steps the recurrence is one
+ *   persistent cooperative kernel; longer calls run it step by step.
  * ---------------------------------------------------------------------------------------------- */
 int64_t renet_gru_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32_t h);
+int64_t renet_gru_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len);
 int renet_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
                   const float* ent, const float* rel, const int32_t* seq_s, const int32_t* seq_r,
                   const int32_t* seq_len, const int32_t* seq_start,
@@ -257,6 +265,7 @@ int renet_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_gl
  * readout); d_ent [*,h], d_rel [*,h], d_glob [T,h] (may be NULL) and the eight parameter gradients
  * are ACCUMULATED (+=), like .grad. */
 int64_t renet_gru_bwd_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32_t h);
+int64_t renet_gru_bwd_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len);
 int renet_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
                   const float* ent, const float* rel, const int32_t* seq_s, const int32_t* seq_r,
                   const int32_t* seq_len, const int32_t* seq_start,
@@ -283,6 +292,7 @@ int renet_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_gl
  * the mask and statistical otherwise.  row_seq [S]: sequence of every row.  Needs the tensor-core GEMM engine.
  * ---------------------------------------------------------------------------------------------- */
 int64_t renet_gru_dropout_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32_t h);
+int64_t renet_gru_dropout_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len);
 int renet_gru_fwd_dropout(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
                           const float* ent, const float* rel, const int32_t* row_seq, const int32_t* seq_s,
                           const int32_t* seq_r, const int32_t* seq_len, const int32_t* seq_start,
@@ -292,6 +302,7 @@ int renet_gru_fwd_dropout(const float* H2, const int32_t* readout, const int32_t
                           float* hn4, float* hn3, int64_t S, int64_t Q, int64_t T, int32_t h, float p, uint64_t seed,
                           void* workspace, int64_t workspace_bytes, void* stream);
 int64_t renet_gru_bwd_dropout_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32_t h);
+int64_t renet_gru_bwd_dropout_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len);
 int renet_gru_bwd_dropout(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
                           const float* ent, const float* rel, const int32_t* row_seq, const int32_t* seq_s,
                           const int32_t* seq_r, const int32_t* seq_len, const int32_t* seq_start,
@@ -310,7 +321,7 @@ int renet_dropout_mask(uint64_t seed, uint64_t offset, int64_t n, float p, float
  * nn.GRU(h_dim, h_dim), global_model.py:25,49; hn3 / the *_3 gradients are then scratch / NULL).  Rows are sequence-major
  * (sequence q owns rows seq_start[q] .. +seq_len[q]-1), sequences sorted by length descending, h0 = 0.  Input projection =
  * two tensor-core GEMMs, recurrence = the kernel of renet_gru_fwd.  k4 <= 4h, k3 <= 3h, multiples of 4.  Workspaces:
- * renet_gru_dropout_workspace_bytes(S, Q, 1, h) / renet_gru_bwd_dropout_workspace_bytes(S, Q, 1, h).
+ * renet_gru_dropout_workspace_bytes_len(S, Q, 1, h, max_len) / renet_gru_bwd_dropout_workspace_bytes_len(S, Q, 1, h, max_len).
  * Backward: dX4 [S,k4] (dX3) written, parameter gradients accumulated. */
 int renet_gru_dense_fwd(const float* X4, int32_t k4, const float* X3, int32_t k3, const int32_t* seq_len,
                         const int32_t* seq_start, const int32_t* host_batch_sizes, int32_t max_len,

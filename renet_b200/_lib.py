@@ -46,6 +46,10 @@ SIGNATURES = {
     'renet_gru_dropout_workspace_bytes': (_i64, [_i64, _i64, _i64, _i32]),
     'renet_gru_fwd_dropout': (ctypes.c_int, [_vp] * 12 + [_i32] + [_vp] * 10 + [_i64, _i64, _i64, _i32, ctypes.c_float, ctypes.c_uint64, _vp, _i64, _vp]),
     'renet_gru_bwd_dropout_workspace_bytes': (_i64, [_i64, _i64, _i64, _i32]),
+    'renet_gru_workspace_bytes_len': (_i64, [_i64, _i64, _i64, _i32, _i32]),
+    'renet_gru_bwd_workspace_bytes_len': (_i64, [_i64, _i64, _i64, _i32, _i32]),
+    'renet_gru_dropout_workspace_bytes_len': (_i64, [_i64, _i64, _i64, _i32, _i32]),
+    'renet_gru_bwd_dropout_workspace_bytes_len': (_i64, [_i64, _i64, _i64, _i32, _i32]),
     'renet_gru_bwd_dropout': (ctypes.c_int, [_vp] * 12 + [_i32] + [_vp] * 18 + [_i64, _i64, _i64, _i64, _i32, ctypes.c_float, ctypes.c_uint64, _vp, _vp, _i64, _vp]),
     'renet_dropout_mask': (ctypes.c_int, [ctypes.c_uint64, ctypes.c_uint64, _i64, ctypes.c_float, _vp, _vp]),
     'renet_gru_dense_fwd': (ctypes.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32] + [_vp] * 10 + [_i64, _i64, _i32, _vp, _i64, _vp]),

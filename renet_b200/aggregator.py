@@ -213,9 +213,9 @@ class RGCNAggregator(nn.Module):
         sub = g.readout_sub(hb.readout, reverse)       # layer 2 runs on the read-out sub-graph (Aggregator.py:140)
         H = torch.empty(g.N + hb.S, h, device=dev)     # H1 [N] | H2 compact [S]
         hn = torch.zeros(2, B, h, device=dev)          # rows >= Q stay zero: samples without history
-        nbytes = int(L.renet_gru_workspace_bytes(hb.S, Q, T, h))
-        ws = torch.empty(nbytes // 4 + 4, dtype=torch.float32, device=dev)
         bs = hb.batch_sizes
+        nbytes = int(L.renet_gru_workspace_bytes_len(hb.S, Q, T, h, len(bs)))
+        ws = torch.empty(nbytes // 4 + 4, dtype=torch.float32, device=dev)
         l1, l2 = self.rgcn1, self.rgcn2
         hot = g.hot_rel(reverse)
         rc = L.renet_encode_fwd(P(ent_embeds), P(g.node_ent), P(g.row_ptr), P(g.col_src), P(g.col_type(reverse)),

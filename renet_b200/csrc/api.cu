@@ -39,7 +39,7 @@ int launch_selfloop_bwd(const float* H, const int32_t* h_index, const float* Wlo
                         float* dWloop, float* WloopT_ws, int64_t N, int d_in, int d_out, cudaStream_t stream);
 int launch_scatter_add_rows(const float* src, const int32_t* index, float* dst, int64_t n_rows, int d,
                             cudaStream_t stream);
-int64_t gru_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout = false);
+int64_t gru_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout = false, int max_len = 0);
 int launch_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
                    const float* ent, const float* rel, const int32_t* seq_s, const int32_t* seq_r,
                    const int32_t* seq_len, const int32_t* seq_start, const int32_t* host_batch_sizes,
@@ -48,7 +48,7 @@ int launch_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_g
                    float* hn3, int64_t S, int64_t Q, int64_t T, int h, float* ws_base, cudaStream_t stream, float p_drop = 0.f,
                    uint64_t seed = 0, const int32_t* row_seq = nullptr, const float* ext_X4 = nullptr, int k4 = 0,
                    const float* ext_X3 = nullptr, int k3 = 0, int phase = 0);
-int64_t gru_bwd_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout = false);
+int64_t gru_bwd_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout = false, int max_len = 0);
 int launch_dropout_mask(uint64_t seed, uint64_t offset, int64_t n, float p, float* out, cudaStream_t stream);
 int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
                    const float* ent, const float* rel, const int32_t* seq_s, const int32_t* seq_r,
@@ -372,6 +372,9 @@ int renet_scatter_add_rows(const float* src, const int32_t* index, float* dst, i
 int64_t renet_gru_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32_t h) {
   return gru_workspace_floats(S, Q, T, h) * (int64_t)sizeof(float);
 }
+int64_t renet_gru_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len) {
+  return gru_workspace_floats(S, Q, T, h, false, max_len) * (int64_t)sizeof(float);
+}
 
 int renet_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
                   const float* ent, const float* rel, const int32_t* seq_s, const int32_t* seq_r,
@@ -386,7 +389,9 @@ int renet_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_gl
                       host_batch_sizes && w_ih4 && w_hh4 && b_ih4 && b_hh4 && w_ih3 && w_hh3 && b_ih3 && b_hh3 &&
                       hn4 && hn3 && workspace,
                   "renet_gru_fwd: null pointer");
-  RENET_CHECK_ARG(workspace_bytes >= renet_gru_workspace_bytes(S, Q, T, h), "renet_gru_fwd: workspace too small");
+  RENET_CHECK_ARG(workspace_bytes >= renet_gru_workspace_bytes_len(S, Q, T, h, max_len),
+                  "renet_gru_fwd: workspace of %lld bytes too small for max_len %d (needs %lld)", (long long)workspace_bytes,
+                  max_len, (long long)renet_gru_workspace_bytes_len(S, Q, T, h, max_len));
   RENET_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "renet_gru_fwd: workspace must be 16-byte aligned");
   return launch_gru_fwd(H2, readout, row_glob, glob, ent, rel, seq_s, seq_r, seq_len, seq_start, host_batch_sizes,
                         max_len, w_ih4, w_hh4, b_ih4, b_hh4, w_ih3, w_hh3, b_ih3, b_hh3, hn4, hn3, S, Q, T, h,
@@ -395,6 +400,9 @@ int renet_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_gl
 
 int64_t renet_gru_bwd_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32_t h) {
   return gru_bwd_workspace_floats(S, Q, T, h) * (int64_t)sizeof(float);
+}
+int64_t renet_gru_bwd_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len) {
+  return gru_bwd_workspace_floats(S, Q, T, h, false, max_len) * (int64_t)sizeof(float);
 }
 
 int renet_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
@@ -412,8 +420,9 @@ int renet_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_gl
                       d_rel && dw_ih4 && dw_hh4 && db_ih4 && db_hh4 && dw_ih3 && dw_hh3 && db_ih3 && db_hh3 &&
                       fwd_workspace && bwd_workspace,
                   "renet_gru_bwd: null pointer");
-  RENET_CHECK_ARG(bwd_workspace_bytes >= renet_gru_bwd_workspace_bytes(S, Q, T, h),
-                  "renet_gru_bwd: workspace too small");
+  RENET_CHECK_ARG(bwd_workspace_bytes >= renet_gru_bwd_workspace_bytes_len(S, Q, T, h, max_len),
+                  "renet_gru_bwd: workspace of %lld bytes too small for max_len %d (needs %lld)", (long long)bwd_workspace_bytes,
+                  max_len, (long long)renet_gru_bwd_workspace_bytes_len(S, Q, T, h, max_len));
   RENET_CHECK_ARG((reinterpret_cast<uintptr_t>(bwd_workspace) & 15) == 0, "renet_gru_bwd: workspace must be 16-byte aligned");
   return launch_gru_bwd(H2, readout, row_glob, glob, ent, rel, seq_s, seq_r, seq_len, seq_start, host_batch_sizes,
                         max_len, w_ih4, w_hh4, w_ih3, w_hh3, dhn4, dhn3, dH2, d_ent, d_rel, d_glob, dw_ih4, dw_hh4,
@@ -426,6 +435,12 @@ int64_t renet_gru_dropout_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32
 }
 int64_t renet_gru_bwd_dropout_workspace_bytes(int64_t S, int64_t Q, int64_t T, int32_t h) {
   return gru_bwd_workspace_floats(S, Q, T, h, true) * (int64_t)sizeof(float);
+}
+int64_t renet_gru_dropout_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len) {
+  return gru_workspace_floats(S, Q, T, h, true, max_len) * (int64_t)sizeof(float);
+}
+int64_t renet_gru_bwd_dropout_workspace_bytes_len(int64_t S, int64_t Q, int64_t T, int32_t h, int32_t max_len) {
+  return gru_bwd_workspace_floats(S, Q, T, h, true, max_len) * (int64_t)sizeof(float);
 }
 
 int renet_gru_fwd_dropout(const float* H2, const int32_t* readout, const int32_t* row_glob, const float* glob,
@@ -441,7 +456,9 @@ int renet_gru_fwd_dropout(const float* H2, const int32_t* readout, const int32_t
   RENET_CHECK_ARG(H2 && readout && row_glob && glob && ent && rel && row_seq && seq_s && seq_r && seq_len && seq_start &&
                       host_batch_sizes && w_ih4 && w_hh4 && b_ih4 && b_hh4 && w_ih3 && w_hh3 && b_ih3 && b_hh3 && hn4 &&
                       hn3 && workspace, "renet_gru_fwd_dropout: null pointer");
-  RENET_CHECK_ARG(workspace_bytes >= renet_gru_dropout_workspace_bytes(S, Q, T, h), "renet_gru_fwd_dropout: workspace too small");
+  RENET_CHECK_ARG(workspace_bytes >= renet_gru_dropout_workspace_bytes_len(S, Q, T, h, max_len),
+                  "renet_gru_fwd_dropout: workspace of %lld bytes too small for max_len %d (needs %lld)", (long long)workspace_bytes,
+                  max_len, (long long)renet_gru_dropout_workspace_bytes_len(S, Q, T, h, max_len));
   RENET_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 127) == 0, "renet_gru_fwd_dropout: workspace must be 128-byte aligned");
   return launch_gru_fwd(H2, readout, row_glob, glob, ent, rel, seq_s, seq_r, seq_len, seq_start, host_batch_sizes, max_len,
                         w_ih4, w_hh4, b_ih4, b_hh4, w_ih3, w_hh3, b_ih3, b_hh3, hn4, hn3, S, Q, T, h, (float*)workspace,
@@ -464,8 +481,9 @@ int renet_gru_bwd_dropout(const float* H2, const int32_t* readout, const int32_t
                       host_batch_sizes && w_ih4 && w_hh4 && w_ih3 && w_hh3 && dhn4 && dhn3 && dH2 && d_ent && d_rel && dw_ih4 &&
                       dw_hh4 && db_ih4 && db_hh4 && dw_ih3 && dw_hh3 && db_ih3 && db_hh3 && fwd_workspace && bwd_workspace,
                   "renet_gru_bwd_dropout: null pointer");
-  RENET_CHECK_ARG(bwd_workspace_bytes >= renet_gru_bwd_dropout_workspace_bytes(S, Q, T, h),
-                  "renet_gru_bwd_dropout: workspace too small");
+  RENET_CHECK_ARG(bwd_workspace_bytes >= renet_gru_bwd_dropout_workspace_bytes_len(S, Q, T, h, max_len),
+                  "renet_gru_bwd_dropout: workspace of %lld bytes too small for max_len %d (needs %lld)",
+                  (long long)bwd_workspace_bytes, max_len, (long long)renet_gru_bwd_dropout_workspace_bytes_len(S, Q, T, h, max_len));
   return launch_gru_bwd(H2, readout, row_glob, glob, ent, rel, seq_s, seq_r, seq_len, seq_start, host_batch_sizes, max_len, w_ih4,
                         w_hh4, w_ih3, w_hh3, dhn4, dhn3, dH2, d_ent, d_rel, d_glob, dw_ih4, dw_hh4, db_ih4, db_hh4, dw_ih3,
                         dw_hh3, db_ih3, db_hh3, N, S, Q, T, h, (const float*)fwd_workspace, (float*)bwd_workspace,
@@ -482,7 +500,9 @@ int renet_gru_dense_fwd(const float* X4, int32_t k4, const float* X3, int32_t k3
   RENET_CHECK_ARG(X4 && seq_len && seq_start && host_batch_sizes && w_ih4 && w_hh4 && b_ih4 && b_hh4 && hn4 && hn3 && workspace,
                   "renet_gru_dense_fwd: null pointer");
   RENET_CHECK_ARG(X3 == nullptr || (w_ih3 && w_hh3 && b_ih3 && b_hh3), "renet_gru_dense_fwd: second encoder needs its weights");
-  RENET_CHECK_ARG(workspace_bytes >= renet_gru_dropout_workspace_bytes(S, Q, 1, h), "renet_gru_dense_fwd: workspace too small");
+  RENET_CHECK_ARG(workspace_bytes >= renet_gru_dropout_workspace_bytes_len(S, Q, 1, h, max_len),
+                  "renet_gru_dense_fwd: workspace of %lld bytes too small for max_len %d (needs %lld)", (long long)workspace_bytes,
+                  max_len, (long long)renet_gru_dropout_workspace_bytes_len(S, Q, 1, h, max_len));
   RENET_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 127) == 0, "renet_gru_dense_fwd: workspace must be 128-byte aligned");
   return launch_gru_fwd(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, seq_len, seq_start,
                         host_batch_sizes, max_len, w_ih4, w_hh4, b_ih4, b_hh4, w_ih3, w_hh3, b_ih3, b_hh3, hn4, hn3, S, Q, 1, h,
@@ -501,7 +521,9 @@ int renet_gru_dense_bwd(const float* X4, int32_t k4, const float* X3, int32_t k3
                       db_ih4 && db_hh4 && fwd_workspace && bwd_workspace, "renet_gru_dense_bwd: null pointer");
   RENET_CHECK_ARG(X3 == nullptr || (w_ih3 && w_hh3 && dX3 && dw_ih3 && dw_hh3 && db_ih3 && db_hh3),
                   "renet_gru_dense_bwd: second encoder needs its weights and gradient buffers");
-  RENET_CHECK_ARG(bwd_workspace_bytes >= renet_gru_bwd_dropout_workspace_bytes(S, Q, 1, h), "renet_gru_dense_bwd: workspace too small");
+  RENET_CHECK_ARG(bwd_workspace_bytes >= renet_gru_bwd_dropout_workspace_bytes_len(S, Q, 1, h, max_len),
+                  "renet_gru_dense_bwd: workspace of %lld bytes too small for max_len %d (needs %lld)",
+                  (long long)bwd_workspace_bytes, max_len, (long long)renet_gru_bwd_dropout_workspace_bytes_len(S, Q, 1, h, max_len));
   return launch_gru_bwd(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, seq_len, seq_start,
                         host_batch_sizes, max_len, w_ih4, w_hh4, w_ih3, w_hh3, dhn4, dhn3, nullptr, nullptr, nullptr, nullptr,
                         dw_ih4, dw_hh4, db_ih4, db_hh4, dw_ih3, dw_hh3, db_ih3, db_hh3, 0, S, Q, 1, h,
@@ -541,7 +563,7 @@ int renet_encode_fwd(const float* ent, const int32_t* node_ent, const int32_t* r
   ForkLease lease{(cudaStream_t)stream};
   const bool gru_args_ok = S > 0 && Q > 0 && readout && row_glob && glob && rel && seq_s && seq_r && seq_len && seq_start &&
                            host_batch_sizes && w_ih4 && w_hh4 && b_ih4 && b_hh4 && w_ih3 && w_hh3 && b_ih3 && b_hh3 && hn4 && hn3 &&
-                           workspace && workspace_bytes >= renet_gru_workspace_bytes(S, Q, T, h) &&
+                           workspace && workspace_bytes >= renet_gru_workspace_bytes_len(S, Q, T, h, max_len) &&
                            (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && max_len >= 0 && T >= 0;
   bool forked = false;
   if (gru_args_ok) {

@@ -255,12 +255,14 @@ GruWs carve(float* base, int64_t S, int64_t Q, int64_t T, int h, int max_len, bo
   return w;
 }
 
-constexpr int kMaxLenWs = 16;  // workspace is sized for sequences up to this long (reference: 10)
+// Steps the per-step buffers (GH, Hs; dGH in backward) are carved for: never fewer than 16 (the reference uses 10), so
+// every call up to 16 steps has one workspace layout, and max_len above that.  Forward and backward carve the same L.
+inline int ws_len(int max_len) { return max_len > 16 ? max_len : 16; }
 
 }  // namespace
 
-int64_t gru_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout) {
-  return carve(nullptr, S, Q, T, h, kMaxLenWs, dropout).total_floats;
+int64_t gru_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout, int max_len) {
+  return carve(nullptr, S, Q, T, h, ws_len(max_len), dropout).total_floats;
 }
 
 int launch_gru_recur(const float* GI, const float* PQ, const float* PT, const float* bhh, const int32_t* row_glob,
@@ -300,12 +302,8 @@ int launch_gru_fwd(const float* H2, const int32_t* readout, const int32_t* row_g
   // GRU: the global model's GRU(h,h), global_model.py:25,49); readout / ent / rel / glob / row_glob are not used
   const bool dense = ext_X4 != nullptr;
   if (!dense) { k4 = 4 * h; k3 = 3 * h; }
-  if (max_len > kMaxLenWs) {
-    set_error("renet_gru_fwd: max_len %d exceeds the supported %d", max_len, kMaxLenWs);
-    return RENET_ERR_INVALID_ARG;
-  }
   const bool dropout = p_drop > 0.f || dense;
-  GruWs w = carve(ws_base, S, Q, T, h, kMaxLenWs, dropout);
+  GruWs w = carve(ws_base, S, Q, T, h, ws_len(max_len), dropout);
   {
     const bool splittable = gemm_mode() == 1 && h % 4 == 0 && (3 * h) % 200 == 0 && (reinterpret_cast<uintptr_t>(ws_base) & 127) == 0 &&
                             !dropout;
@@ -606,12 +604,12 @@ struct GruBwdWs {
   int64_t total_floats;
 };
 
-GruBwdWs carve_bwd(float* base, int64_t S, int64_t Q, int64_t T, int h, bool dropout = false) {
+GruBwdWs carve_bwd(float* base, int64_t S, int64_t Q, int64_t T, int h, int max_len, bool dropout = false) {
   GruBwdWs w;
   int64_t off = 0;
   auto take = [&](int64_t n) { float* p = base ? base + off : nullptr; off += align4(n); return p; };
   w.dGI = take(S * 6 * h);
-  w.dGH = take((int64_t)kMaxLenWs * Q * 6 * h);          // every step's recurrent-gate gradients (one dW_hh GEMM over all steps)
+  w.dGH = take((int64_t)ws_len(max_len) * Q * 6 * h);          // every step's recurrent-gate gradients (one dW_hh GEMM over all steps)
   w.dPQ = take(Q * 6 * h);
   w.dPT = take(T * 6 * h);
   w.dHa = take(Q * 2 * h);
@@ -638,8 +636,8 @@ GruBwdWs carve_bwd(float* base, int64_t S, int64_t Q, int64_t T, int h, bool dro
 
 }  // namespace
 
-int64_t gru_bwd_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout) {
-  return carve_bwd(nullptr, S, Q, T, h, dropout).total_floats;
+int64_t gru_bwd_workspace_floats(int64_t S, int64_t Q, int64_t T, int h, bool dropout, int max_len) {
+  return carve_bwd(nullptr, S, Q, T, h, max_len, dropout).total_floats;
 }
 
 int launch_scatter_add_rows(const float* src, const int32_t* index, float* dst, int64_t n_rows, int d,
@@ -658,20 +656,15 @@ int launch_gru_bwd(const float* H2, const int32_t* readout, const int32_t* row_g
   const bool dense = ext_X4 != nullptr;
   if (!dense) { k4 = 4 * h; k3 = 3 * h; }
   const bool dropout = p_drop > 0.f || dense;
-  GruWs f = carve(const_cast<float*>(fwd_ws), S, Q, T, h, kMaxLenWs, dropout);
-  GruBwdWs b = carve_bwd(bwd_ws, S, Q, T, h, dropout);
+  GruWs f = carve(const_cast<float*>(fwd_ws), S, Q, T, h, ws_len(max_len), dropout);
+  GruBwdWs b = carve_bwd(bwd_ws, S, Q, T, h, max_len, dropout);
   if (dense) {
     row_glob = reinterpret_cast<const int32_t*>(f.zrow);
     if (ext_X3 == nullptr) { w_ih3 = w_ih4; w_hh3 = w_hh4; }
   }
   int rc;
-  // checked before anything is written: a rejected call used to have zeroed dH2 already
   int last = 0;
   while (last < max_len && host_batch_sizes[last] > 0) ++last;
-  if (last > kMaxLenWs) {
-    set_error("renet_gru_bwd: max_len %d exceeds the supported %d", last, kMaxLenWs);
-    return RENET_ERR_INVALID_ARG;
-  }
   RENET_CHECK_CUDA(cudaMemsetAsync(b.dbias, 0, 12 * h * sizeof(float), stream));
   RENET_CHECK_CUDA(cudaMemsetAsync(b.dWhh, 0, (int64_t)h * 6 * h * sizeof(float), stream));
   RENET_CHECK_CUDA(cudaMemsetAsync(b.dPT, 0, T * 6 * h * sizeof(float), stream));

@@ -27,7 +27,7 @@ constexpr int R_A_BYTES = 128 * 128;      // one 32-wide K chunk of the 128-row 
 constexpr int R_B_PLANE = RN * 128;       // 12288
 constexpr int R_MAX_CHUNKS = 7;           // h <= 224
 constexpr int R_SMEM = R_MAX_CHUNKS * 2 * R_B_PLANE + 2 * R_A_BYTES + 1024 + 128;
-constexpr int R_MAX_LEN = 16;
+constexpr int R_MAX_LEN = 64;             // longest call the kernel takes: its per-step active counts go by value (256 B)
 
 struct StepCounts { int n[R_MAX_LEN]; };
 

@@ -104,9 +104,9 @@ class _DenseGruFn(torch.autograd.Function):
         Q = seq_len_dev.numel()
         dev = X.device
         hn = torch.zeros(2, Q, h, device=dev)
-        nbytes = int(L.renet_gru_dropout_workspace_bytes(S, Q, 1, h))
-        ws = torch.empty(nbytes // 4 + 32, dtype=torch.float32, device=dev)
         bs = np.ascontiguousarray(batch_sizes, dtype=np.int32)
+        nbytes = int(L.renet_gru_dropout_workspace_bytes_len(S, Q, 1, h, len(bs)))
+        ws = torch.empty(nbytes // 4 + 32, dtype=torch.float32, device=dev)
         rc = L.renet_gru_dense_fwd(P(X), k, None, 0, P(seq_len_dev), P(seq_start_dev), bs.ctypes.data_as(_lib.ctypes.c_void_p),
                                    len(bs), P(w_ih), P(w_hh), P(b_ih), P(b_hh), None, None, None, None, P(hn[0]), P(hn[1]), S, Q,
                                    h, P(ws), nbytes, _lib.stream())
@@ -128,9 +128,9 @@ class _DenseGruFn(torch.autograd.Function):
         dX = torch.empty_like(X)
         dw_ih, dw_hh = torch.zeros_like(w_ih), torch.zeros_like(w_hh)
         db_ih, db_hh = torch.zeros(3 * h, device=dev), torch.zeros(3 * h, device=dev)
-        nbytes = int(L.renet_gru_bwd_dropout_workspace_bytes(S, Q, 1, h))
-        bws = torch.empty(nbytes // 4 + 32, dtype=torch.float32, device=dev)
         bs = ctx.bs
+        nbytes = int(L.renet_gru_bwd_dropout_workspace_bytes_len(S, Q, 1, h, len(bs)))
+        bws = torch.empty(nbytes // 4 + 32, dtype=torch.float32, device=dev)
         rc = L.renet_gru_dense_bwd(P(X), k, None, 0, P(seq_len_dev), P(seq_start_dev), bs.ctypes.data_as(_lib.ctypes.c_void_p),
                                    len(bs), P(w_ih), P(w_hh), None, None, P(dhn), P(zero), P(dX), None, P(dw_ih), P(dw_hh),
                                    P(db_ih), P(db_hh), None, None, None, None, S, Q, h, P(ws), P(bws), nbytes, _lib.stream())

@@ -34,7 +34,7 @@ class _FusedGruFn(torch.autograd.Function):
         bs = hb.batch_sizes      # host int32 numpy
         if p_drop > 0.0:
             # training with input dropout (Aggregator.py:157-158): masked inputs materialised in the workspace, Philox masks
-            nbytes = int(L.renet_gru_dropout_workspace_bytes(S, Q, T, h))
+            nbytes = int(L.renet_gru_dropout_workspace_bytes_len(S, Q, T, h, len(bs)))
             ws = torch.empty(nbytes // 4 + 32, dtype=torch.float32, device=dev)
             rc = L.renet_gru_fwd_dropout(_lib.ptr(H2), _lib.ptr(readout), _lib.ptr(hb.row_glob), _lib.ptr(glob),
                                          _lib.ptr(ent), _lib.ptr(rel), _lib.ptr(hb.row_seq), _lib.ptr(seq_s), _lib.ptr(seq_r),
@@ -46,7 +46,7 @@ class _FusedGruFn(torch.autograd.Function):
                                          _lib.stream())
             _lib.check(rc, 'renet_gru_fwd_dropout')
         else:
-            nbytes = int(L.renet_gru_workspace_bytes(S, Q, T, h))
+            nbytes = int(L.renet_gru_workspace_bytes_len(S, Q, T, h, len(bs)))
             ws = torch.empty(nbytes // 4 + 4, dtype=torch.float32, device=dev)
             rc = L.renet_gru_fwd(_lib.ptr(H2), _lib.ptr(readout), _lib.ptr(hb.row_glob), _lib.ptr(glob),
                                  _lib.ptr(ent), _lib.ptr(rel), _lib.ptr(seq_s), _lib.ptr(seq_r),

@@ -20,7 +20,7 @@ def fused_gru_backward(ctx, dhn4, dhn3):
     grads = [z(w_ih4), z(w_hh4), z(b_ih4), z(b_hh4), z(w_ih3), z(w_hh3), z(b_ih3), z(b_hh3)]
     bs = hb.batch_sizes
     if ctx.p_drop > 0.0:
-        nbytes = int(L.renet_gru_bwd_dropout_workspace_bytes(S, Q, T, h))
+        nbytes = int(L.renet_gru_bwd_dropout_workspace_bytes_len(S, Q, T, h, len(bs)))
         bws = torch.empty(nbytes // 4 + 32, dtype=torch.float32, device=dev)
         dH2.zero_()                                          # the scatter of the masked input gradients accumulates
         rc = L.renet_gru_bwd_dropout(_lib.ptr(H2), _lib.ptr(ctx.readout), _lib.ptr(hb.row_glob), _lib.ptr(glob), _lib.ptr(ent),
@@ -32,7 +32,7 @@ def fused_gru_backward(ctx, dhn4, dhn3):
                                      h, ctx.p_drop, ctx.seed, _lib.ptr(ws), _lib.ptr(bws), nbytes, _lib.stream())
         _lib.check(rc, 'renet_gru_bwd_dropout')
         return (dH2, d_ent, d_rel, d_glob, *grads, None, None, None, None, None, None)
-    nbytes = int(L.renet_gru_bwd_workspace_bytes(S, Q, T, h))
+    nbytes = int(L.renet_gru_bwd_workspace_bytes_len(S, Q, T, h, len(bs)))
     bws = torch.empty(nbytes // 4 + 4, dtype=torch.float32, device=dev)
     rc = L.renet_gru_bwd(_lib.ptr(H2), _lib.ptr(ctx.readout), _lib.ptr(hb.row_glob), _lib.ptr(glob), _lib.ptr(ent),
                          _lib.ptr(rel), _lib.ptr(seq_s), _lib.ptr(seq_r), _lib.ptr(hb.graph.seq_len_dev),

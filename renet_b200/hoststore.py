@@ -21,6 +21,7 @@ from . import _lib
 from .graph import BatchedHistoryGraph, PendingCount, _Frame, as_history_graph
 from .utils import HistoryBatch
 
+#: smallest batch_sizes capacity the batchers are given; a store whose longest history is longer gets that length
 MAX_LEN = 16
 
 
@@ -139,6 +140,7 @@ class HistoryStore:
         self.subjects = np.asarray(subjects, dtype=np.int64)
         lens = np.fromiter((len(h) for h in hist), dtype=np.int64, count=n)
         self.samp_off = np.concatenate(([0], np.cumsum(lens))).astype(np.int64)
+        self.max_len = max(MAX_LEN, int(lens.max()) if n else 0)      # batch_sizes capacity of every batch of this store
         total = int(self.samp_off[-1])
         arrays = [a for h in hist for a in h]
         flat_t = np.fromiter((int(t) for ht in hist_t for t in ht), dtype=np.int64, count=total)
@@ -262,12 +264,12 @@ def assemble_view_raw(view, out, sort=True):
     hs, gs = view.store, view.store.gs
     B = len(view.sample_idx)
     s_idx = np.empty(B, dtype=np.int64)
-    bsz = np.zeros(MAX_LEN, dtype=np.int32)
+    bsz = np.zeros(hs.max_len, dtype=np.int32)
     sizes = np.zeros(10, dtype=np.int64)
     rc = L.renet_host_assemble_batch(
         len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(gs.src), _p(gs.dst), _p(gs.type_s),
         _p(gs.type_o), _p(hs.samp_off), _p(hs.samp_entry), _p(hs.ent_graph), _p(hs.ent_srow), _p(hs.ent_off), _p(hs.nbr_row),
-        _p(view.sample_idx), B, int(sort), _p(s_idx), _p(out), out.size, _p(bsz), MAX_LEN, _p(sizes))
+        _p(view.sample_idx), B, int(sort), _p(s_idx), _p(out), out.size, _p(bsz), hs.max_len, _p(sizes))
     return _result(rc, 'renet_host_assemble_batch', False, sizes, s_idx, bsz, out)
 
 
@@ -291,13 +293,13 @@ def plan_view_raw(view, out, sort=True):
     hs, gs = view.store, view.store.gs
     B = len(view.sample_idx)
     s_idx = np.empty(B, dtype=np.int64)
-    bsz = np.zeros(MAX_LEN, dtype=np.int32)
+    bsz = np.zeros(hs.max_len, dtype=np.int32)
     sizes = np.zeros(10, dtype=np.int64)
     groups = _p(view.groups) if view.groups is not None else None
     rc = L.renet_host_plan_batch_grouped(
         len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(hs.samp_off), _p(hs.samp_entry), _p(hs.ent_graph),
         _p(hs.ent_srow), _p(hs.ent_off), _p(hs.nbr_row), _p(view.sample_idx), groups, B, int(sort), _p(s_idx), _p(out),
-        out.size, _p(bsz), MAX_LEN, _p(sizes))
+        out.size, _p(bsz), hs.max_len, _p(sizes))
     return _result(rc, 'renet_host_plan_batch', True, sizes, s_idx, bsz, out)
 
 
@@ -341,18 +343,18 @@ class NativeLoader:
         hs, gs = view.store, view.store.gs
         B = len(view.sample_idx)
         job = dict(view=view, out=out, sort=sort, device_edges=device_edges, s_idx=np.empty(B, dtype=np.int64),
-                   bsz=np.zeros(MAX_LEN, dtype=np.int32), sizes=np.zeros(10, dtype=np.int64))
+                   bsz=np.zeros(hs.max_len, dtype=np.int32), sizes=np.zeros(10, dtype=np.int64))
         if device_edges:
             t = self.L.renet_loader_submit_plan(
                 self.h, len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(hs.samp_off), _p(hs.samp_entry),
                 _p(hs.ent_graph), _p(hs.ent_srow), _p(hs.ent_off), _p(hs.nbr_row), _p(view.sample_idx), B, int(sort),
-                _p(job['s_idx']), _p(out), out.size, _p(job['bsz']), MAX_LEN, _p(job['sizes']))
+                _p(job['s_idx']), _p(out), out.size, _p(job['bsz']), hs.max_len, _p(job['sizes']))
         else:
             t = self.L.renet_loader_submit_assemble(
                 self.h, len(gs.times), _p(gs.node_off), _p(gs.node_ent), _p(gs.edge_off), _p(gs.src), _p(gs.dst), _p(gs.type_s),
                 _p(gs.type_o), _p(hs.samp_off), _p(hs.samp_entry), _p(hs.ent_graph), _p(hs.ent_srow), _p(hs.ent_off),
                 _p(hs.nbr_row), _p(view.sample_idx), B, int(sort), _p(job['s_idx']), _p(out), out.size, _p(job['bsz']),
-                MAX_LEN, _p(job['sizes']))
+                hs.max_len, _p(job['sizes']))
         if t < 0:
             raise RuntimeError('renet_loader_submit failed')
         job['ticket'] = t

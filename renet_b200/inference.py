@@ -25,6 +25,13 @@ from .graph import get_big_graph
 ROLLOVER_SEQ_BUDGET = 16384
 
 
+def _seq_budget(max_len):
+    """Sequences per encode chunk for histories of up to ``max_len`` steps: ROLLOVER_SEQ_BUDGET up to 16 steps, and
+    16 / max_len of it above, so that the GRU's per-step buffers (8h floats per sequence and step) stay within their
+    16-step size."""
+    return ROLLOVER_SEQ_BUDGET if max_len <= 16 else max(1, ROLLOVER_SEQ_BUDGET * 16 // max_len)
+
+
 #: distinct (entity, timestamp) components evaluate_stream_batched batches per chunk are bounded by their summed node and
 #: candidate-edge counts: the plan's mark_off / cand_off are int32, and 2^28 keeps them far from overflow
 EVAL_PLAN_BUDGET = 1 << 28
@@ -431,8 +438,8 @@ class RENetInference:
         return ents, wts
 
     def _topk_chunks(self, n):
-        """[c0, c1) of pred_r_topk's chunks of n entities: ROLLOVER_SEQ_BUDGET // R entities each."""
-        per = max(1, ROLLOVER_SEQ_BUDGET // self.num_rels)
+        """[c0, c1) of pred_r_topk's chunks of n entities: _seq_budget(seq_len) // R entities each."""
+        per = max(1, _seq_budget(self.seq_len) // self.num_rels)
         return [(c0, min(c0 + per, n)) for c0 in range(0, n, per)]
 
     def _topk_chunk(self, ce, wc, k, subject, capacity=None):
@@ -1120,12 +1127,13 @@ class RENetInference:
             for t in set().union(*ent_times.values()):
                 g = graph_dict[t]
                 sizes[t] = g.number_of_nodes() + g.number_of_edges()
+            budget = _seq_budget(max(self.seq_len, max(len(hist_t[hh]) for hh in np.unique(q_h))))
             chunks, j0 = [], 0
             while j0 < len(keys):
                 # a chunk: whole entities, within both budgets; an entity's components are the distinct timestamps of its
                 # histories
                 cost, j1 = 0, j0
-                while j1 < len(keys) and j1 - j0 < ROLLOVER_SEQ_BUDGET:
+                while j1 < len(keys) and j1 - j0 < budget:
                     e = q_e[j1]
                     if j1 == j0 or e != q_e[j1 - 1]:
                         c = sum(sizes[t] for t in ent_times[e])
