@@ -290,13 +290,19 @@ def bwd_kernels(which, loop, indexed, det):
 CHUNK = 16384
 
 
-def ref_forward(g, X, h_index, W, norm, loop):
-    """(pre-activation reference, S) [n_dst, 200] in float64"""
-    src, dst, et = (torch.from_numpy(a).to(DEV) for a in (g.src, g.dst, g.et))
+def _edges(g):
+    """g's src, dst, type as int64 device tensors (g may hold numpy arrays or device tensors)"""
+    return (torch.as_tensor(a, device=DEV).long() for a in (g.src, g.dst, g.et))
+
+
+def ref_forward(g, X, h_index, W, norm, loop, chunk=CHUNK):
+    """(pre-activation reference, S) [n_dst, 200] in float64; chunk: edges per pass (a pass holds ~ 1.6 KB of float64
+    messages per edge)"""
+    src, dst, et = _edges(g)
     rows = h_index.long()[src] if h_index is not None else src
     acc = torch.zeros(2, g.n_dst, 100, 2, dtype=torch.float64, device=DEV)
-    for a in range(0, g.E, CHUNK):                 # block b / in i / out j at b*4 + i*2 + j
-        b = slice(a, a + CHUNK)
+    for a in range(0, g.E, chunk):                 # block b / in i / out j at b*4 + i*2 + j
+        b = slice(a, a + chunk)
         x, w = X[rows[b]].double().view(-1, 100, 2), W[et[b]].double().view(-1, 100, 2, 2)
         acc[0].index_add_(0, dst[b], torch.einsum('ebi,ebij->ebj', x, w))
         acc[1].index_add_(0, dst[b], torch.einsum('ebi,ebij->ebj', x.abs(), w.abs()))
@@ -310,15 +316,15 @@ def ref_forward(g, X, h_index, W, norm, loop):
     return acc[0], acc[1].abs()
 
 
-def ref_backward(g, X, h_index, W, norm, P):
+def ref_backward(g, X, h_index, W, norm, P, chunk=CHUNK):
     """(dH, S_dH [n_src, 200], dW, S_dW [R2, 400]) in float64, without the self-loop part and the base"""
-    src, dst, et = (torch.from_numpy(a).to(DEV) for a in (g.src, g.dst, g.et))
+    src, dst, et = _edges(g)
     rows = h_index.long()[src] if h_index is not None else src
     G = P.double() * norm.double()[:, None]
     dH = torch.zeros(2, g.n_src, 100, 2, dtype=torch.float64, device=DEV)
     dW = torch.zeros(2, g.R2, 400, dtype=torch.float64, device=DEV)
-    for a in range(0, g.E, CHUNK):
-        b = slice(a, a + CHUNK)
+    for a in range(0, g.E, chunk):
+        b = slice(a, a + chunk)
         x, w = X[rows[b]].double().view(-1, 100, 2), W[et[b]].double().view(-1, 100, 2, 2)
         gg = G[dst[b]].view(-1, 100, 2)
         dH[0].index_add_(0, src[b], torch.einsum('ebij,ebj->ebi', w, gg))
@@ -329,19 +335,25 @@ def ref_backward(g, X, h_index, W, norm, P):
     return dH[0], dH[1], dW[0], dW[1]
 
 
+def bar_ratio(got, ref, S, n):
+    """(per row: the largest err / ((n + 4) 2^-24 S) over the row's elements, |got - ref|); n: int64 device tensor"""
+    unit = U * (n.double() + 4)[:, None] * S
+    err = (got.double() - ref).abs()
+    ratio = torch.where(unit > 0, err / unit.clamp_min(1e-300), torch.where(err > 0, float('inf'), 0.0).double())
+    return ratio.max(1).values, err
+
+
 def check_rows(label, case, what, got, ref, S, n_terms, exact_to=None):
     """per-row bar; rows with n_terms == 0 must equal exact_to bit for bit"""
-    n = torch.from_numpy(np.asarray(n_terms, dtype=np.int64)).to(DEV)
+    n = torch.as_tensor(n_terms, device=DEV).long() if torch.is_tensor(n_terms) else torch.from_numpy(
+        np.asarray(n_terms, dtype=np.int64)).to(DEV)
     assert torch.isfinite(got).all(), (case, what, 'not finite')
     if exact_to is not None:
         z = (n == 0).nonzero().flatten()
         bad = (got[z] != exact_to[z]).any(1).nonzero().flatten()
         assert bad.numel() == 0, '%s %s: row %d has no edges and is not bit-equal to its self-loop row / base' % (
             case, what, int(z[bad[0]]))
-    unit = U * (n.double() + 4)[:, None] * S
-    err = (got.double() - ref).abs()
-    ratio = torch.where(unit > 0, err / unit.clamp_min(1e-300), torch.where(err > 0, float('inf'), 0.0).double())
-    per_row = ratio.max(1).values
+    per_row, err = bar_ratio(got, ref, S, n)
     worst = float(per_row.max())
     row = int(per_row.argmax())
     if worst > WORST.get(label, (-1.0,))[0]:
