@@ -40,6 +40,8 @@ const char* renet_last_error(void);
 /* Number of kernels this library has launched on this process so far (for bench.py's
  * "gpu_launches" claim). */
 int64_t renet_launch_count(void);
+/* Number of those launches that asked for programmatic dependent launch (RENET_PDL, DESIGN §4). */
+int64_t renet_pdl_launch_count(void);
 
 /* Dense-GEMM engine used for the self-loop and GRU projections: 0 = FFMA (fp32 CUDA cores),
  * 1 = wgmma 3xTF32 (tensor cores, fp32-accurate split).  Both are this library's own kernels.

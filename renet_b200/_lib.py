@@ -18,6 +18,7 @@ SIGNATURES = {
     'renet_version': (ctypes.c_int, []),
     'renet_last_error': (ctypes.c_char_p, []),
     'renet_launch_count': (_i64, []),
+    'renet_pdl_launch_count': (_i64, []),
     'renet_set_gemm_engine': (ctypes.c_int, [ctypes.c_int]),
     'renet_get_gemm_engine': (ctypes.c_int, []),
     'renet_set_deterministic': (ctypes.c_int, [ctypes.c_int]),
@@ -158,6 +159,10 @@ def require_cuda(*tensors):
 
 def launch_count():
     return int(lib().renet_launch_count())
+
+
+def pdl_launch_count():
+    return int(lib().renet_pdl_launch_count())
 
 
 # ---- packed-weight cache (renet_set_weight_generation) -----------------------------------------------------------------

@@ -2,11 +2,13 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include <atomic>
+#include <map>
 #include <mutex>
 #include <string.h>
 #include <vector>
 
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace renet {
 
@@ -20,6 +22,44 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+// ---- programmatic dependent launch (launch.cuh) ----------------------------------------------------------------------
+static std::atomic<int64_t> g_pdl_launches{0};
+void count_pdl_launch() { g_pdl_launches.fetch_add(1, std::memory_order_relaxed); }
+bool pdl_allowed() {
+  const char* e = getenv("RENET_PDL");
+  return !(e && e[0] == '0');
+}
+namespace {
+std::mutex g_pdl_mu;
+// (device, stream) -> what the last early-triggering library launch on it writes
+std::map<std::pair<int, cudaStream_t>, std::vector<DevSpan>> g_pdl_records;
+std::pair<int, cudaStream_t> pdl_key(cudaStream_t s) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  return {dev, s};
+}
+bool overlap(const DevSpan& a, const DevSpan& b) {
+  const uintptr_t a0 = reinterpret_cast<uintptr_t>(a.p), b0 = reinterpret_cast<uintptr_t>(b.p);
+  return a.bytes > 0 && b.bytes > 0 && a0 < b0 + (uintptr_t)b.bytes && b0 < a0 + (uintptr_t)a.bytes;
+}
+}  // namespace
+bool pdl_disjoint(cudaStream_t stream, std::initializer_list<DevSpan> pre_wait) {
+  if (!pdl_allowed()) return false;
+  const auto key = pdl_key(stream);
+  std::lock_guard<std::mutex> lk(g_pdl_mu);
+  const auto it = g_pdl_records.find(key);
+  if (it == g_pdl_records.end()) return true;
+  for (const DevSpan& r : pre_wait)
+    for (const DevSpan& w : it->second)
+      if (overlap(r, w)) return false;
+  return true;
+}
+void pdl_record(cudaStream_t stream, std::initializer_list<DevSpan> writes) {
+  const auto key = pdl_key(stream);
+  std::lock_guard<std::mutex> lk(g_pdl_mu);
+  g_pdl_records[key].assign(writes.begin(), writes.end());
+}
 static thread_local int g_last_gemm_kernel = 0;
 void note_gemm_kernel(int kernel) { g_last_gemm_kernel = kernel; }
 int last_gemm_kernel() { return g_last_gemm_kernel; }
@@ -193,6 +233,7 @@ extern "C" {
 int renet_version(void) { return 100; /* 0.1.0 */ }
 const char* renet_last_error(void) { return g_err; }
 int64_t renet_launch_count(void) { return g_launches.load(); }
+int64_t renet_pdl_launch_count(void) { return g_pdl_launches.load(); }
 int renet_set_gemm_engine(int engine) { return set_gemm_mode(engine); }
 int renet_get_gemm_engine(void) { return gemm_mode(); }
 int renet_set_deterministic(int on) { return set_deterministic(on); }

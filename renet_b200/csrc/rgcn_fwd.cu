@@ -148,14 +148,17 @@ static int launch_stream_cfg(const float* H, const int32_t* h_index, const float
                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_done = true;
   }
-  // (Programmatic stream serialisation behind the self-loop GEMM is not used: with a CUDA event recorded between the two
-  // kernels it once made a GDELT-shaped launch orders of magnitude slower, an interaction that was never pinned down.
-  // Plain stream order it is; the kernel's griddepcontrol.wait is a no-op then.)
-  long long* dbg = g_stream_dbg;
-  rgcn_gather_stream_kernel<RELU, HAS_LOOP, INDEXED, false, Cfg><<<kNumSMs, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(
-      H, h_index, W, row_ptr, col_src, col_type, norm, Hout, N, R2, hot_rel, n_hot, E_hint, dbg);
-  RENET_CHECK_LAUNCH("rgcn_gather_stream_kernel");
-  return RENET_OK;
+  // Programmatic dependent launch (launch.cuh, DESIGN §4): the prologue before the kernel's griddepcontrol.wait (partition
+  // search, row_ptr slice, relation ranking, resident relation rows, first index blocks) runs under the previous kernel's
+  // tail when that kernel writes none of these pre-wait inputs.  norm is read after the wait; it is listed all the same,
+  // so a norm the previous kernel writes keeps the plain order.
+  const int64_t e4 = (int64_t)E_hint * 4, n4 = ((int64_t)N + 1) * 4;
+  return launch_pdl("rgcn_gather_stream_kernel",
+                    {{row_ptr, n4}, {col_src, e4}, {col_type, e4}, {h_index, INDEXED ? (int64_t)N * 4 : 0},
+                     {norm, (int64_t)N * 4}, {W, (int64_t)R2 * 1600}, {hot_rel, hot_rel ? (int64_t)n_hot * 4 : 0}},
+                    {{Hout, (int64_t)N * 800}}, rgcn_gather_stream_kernel<RELU, HAS_LOOP, INDEXED, false, Cfg>,
+                    dim3(kNumSMs), dim3(Cfg::kThreads), Cfg::kSmemBytes, stream, H, h_index, W, row_ptr, col_src, col_type,
+                    norm, Hout, N, R2, hot_rel, n_hot, E_hint, g_stream_dbg);
 }
 
 template <bool RELU, bool HAS_LOOP, bool INDEXED>

@@ -36,6 +36,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "launch.cuh"
 #include "umma.cuh"
 
 namespace renet {
@@ -537,11 +538,13 @@ rgcn_gather_stream_kernel(const float* __restrict__ X, const int32_t* __restrict
       st_bulk_g2s(ring + slot * kStSlot, X + (int64_t)(int)src * 200, 800, bar);
     }
   };
-  // Everything above read graph structure, weights and the relation ranking only; from here on the kernel touches what
-  // the previous kernel in the stream produced (the self-loop rows in Hout; layer 2's input rows).  A launcher that uses
-  // programmatic stream serialisation gets the prologue overlapped with that kernel's tail; in plain stream order (what
-  // the library does, see rgcn_fwd.cu) this wait returns immediately.
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  // Everything above read graph structure (row_ptr, col_a, col_type, x_index), the weights W and hot_rel only: the
+  // pre-wait inputs the forward launcher declares (rgcn_fwd.cu), which the previous kernel in the stream must not write
+  // (DESIGN §4).  From here on the kernel touches what that kernel produced (the self-loop rows in Hout; layer 2's input
+  // rows), and only now may the next kernel start: trigger after wait.  The backward is launched in plain stream order
+  // (the wait returns at once) and does not trigger early.
+  pdl_wait();
+  if constexpr (!BWD) pdl_trigger();
   if constexpr (kHub > 0) {
     if (warp == 2) {                   // the hub rows, on 8 group barriers (every barrier gets its arrival)
       if (lane < kStHotGroups)

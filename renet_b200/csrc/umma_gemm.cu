@@ -17,6 +17,7 @@
 //   * umma_gemm_resident_kernel: the whole B panel (K <= 224) resident in shared memory, A fed to wgmma from registers;
 //     umma_gemm_dedup runs it over the distinct rows of an index and copies the rows out.
 #include "common.cuh"
+#include "launch.cuh"
 #include <mutex>
 #include <vector>
 
@@ -76,6 +77,8 @@ __global__ void __launch_bounds__(256)
 umma_pack_b_kernel(const float* __restrict__ B, int64_t sk, int64_t sn, int N, int K, uint8_t* __restrict__ Bp,
                    int n_chunks, int tile_offset) {
   // logical B[k][n] = B[k*sk + n*sn]  (row-major [K,N]: sk = ldb, sn = 1; a [N,K] weight read transposed: sk = 1, sn = ld)
+  pdl_wait();                          // nothing before the wait: only the launch latency hides under the previous kernel
+  pdl_trigger();
   const int nt = blockIdx.x, kc = blockIdx.y;
   const int n0 = nt * UN, k0 = kc * P_BK;
   const int tile_n = min(UN, N - n0);
@@ -530,28 +533,32 @@ __global__ void __launch_bounds__(R_THREADS, 1)
 umma_gemm_resident_kernel(const float* __restrict__ A, const int32_t* __restrict__ a_index, int64_t lda,
                           const uint8_t* __restrict__ Bp, float* __restrict__ C, int64_t ldc, const float* __restrict__ bias,
                           int64_t M, const int32_t* __restrict__ m_dev, int N, int K, int n_chunks, int accumulate,
-                          int64_t batch_a, int64_t batch_bp, int64_t batch_c, int n_panels, long long* dbg) {
+                          int64_t batch_a, int64_t batch_bp, int64_t batch_c, int n_panels, int panel_before_wait,
+                          long long* dbg) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t sb = raw + ((1024 - (raw & 1023)) & 1023);       // swizzle atoms need 1024-byte alignment
   const uint32_t bar0 = sb + R_MAX_CHUNKS * R_CHUNK;
   const int tid = threadIdx.x;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
-  if (m_dev != nullptr) M = *m_dev;
   // panel p owns the CTAs [p*G/P, (p+1)*G/P) (G >= P: at least one each)
   const int G = gridDim.x, b = blockIdx.x;
   const int p = (int)(((int64_t)(b + 1) * n_panels - 1) / G);
   const int cta0 = (int)((int64_t)p * G / n_panels), ncta = (int)((int64_t)(p + 1) * G / n_panels) - cta0;
-  const int64_t n_rt = (M + 63) / 64;
-  const int64_t t_begin = (int64_t)(b - cta0) * n_rt / ncta, t_end = (int64_t)(b - cta0 + 1) * n_rt / ncta;
-  // with a device row count (or rows < CTAs) a CTA may have no tile: it must not issue copies it would never wait for
-  if (t_begin == t_end) return;
+  int64_t t_begin, t_end;
+  auto split_tiles = [&]() {
+    const int64_t n_rt = (M + 63) / 64;
+    t_begin = (int64_t)(b - cta0) * n_rt / ncta;
+    t_end = (int64_t)(b - cta0 + 1) * n_rt / ncta;
+  };
+  split_tiles();
+  // rows < CTAs: a CTA may have no tile, and it must not issue copies it would never wait for.  With a device row count
+  // (M is an upper bound until the wait) any CTA may still get one
+  const bool may_work = m_dev != nullptr || t_begin != t_end;
   const int n_tiles = (N + UN - 1) / UN;
   const int half = p & 1, nt = (p >> 1) % n_tiles, zb = (p >> 1) / n_tiles;
   GemmStamps ts(dbg, wg);
-  if (tid == 0) {
-    for (int c = 0; c < n_chunks; ++c) mbar_init(bar0 + 8 * c, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  auto copy_panel = [&]() {
     const uint8_t* src = Bp + zb * batch_bp + (size_t)nt * n_chunks * P_B_CHUNK + half * P_BH_BYTES;
     for (int c = 0; c < n_chunks; ++c) {
       const uint32_t bar = bar0 + 8 * c, dst = sb + c * R_CHUNK;
@@ -560,7 +567,29 @@ umma_gemm_resident_kernel(const float* __restrict__ A, const int32_t* __restrict
       bulk_copy_g2s(dst + P_BH_BYTES, src + (size_t)c * P_B_CHUNK + P_B_BYTES, P_BH_BYTES, bar);
       mbar_arrive(bar);
     }
+  };
+  if (tid == 0 && may_work) {
+    for (int c = 0; c < n_chunks; ++c) mbar_init(bar0 + 8 * c, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    // the packed panel is a weight image: before the wait unless the previous kernel writes it (the launcher knows:
+    // a new weight generation packed it in this call)
+    if (panel_before_wait) copy_panel();
   }
+  // what the previous kernel produced (*m_dev, A and a_index, C when accumulating) is read after the wait; every CTA
+  // reaches it (DESIGN §4)
+  pdl_wait();
+  pdl_trigger();
+  if (!may_work) return;
+  if (m_dev != nullptr) {
+    M = *m_dev;
+    split_tiles();
+    if (t_begin == t_end) {                                       // no tile after all: the copies land before the CTA exits
+      if (tid == 0 && panel_before_wait)
+        for (int c = 0; c < n_chunks; ++c) mbar_wait(bar0 + 8 * c, 0);
+      return;
+    }
+  }
+  if (tid == 0 && !panel_before_wait) copy_panel();
   __syncthreads();                                                // the barriers are initialised
 
   const int wt = tid & 127, lane = tid & 31, tig = lane & 3;
@@ -663,6 +692,8 @@ __global__ void __launch_bounds__(256)
 dedup_insert_kernel(const int32_t* __restrict__ a_index, int64_t M, unsigned long long* __restrict__ table, int bits,
                     uint32_t epoch, int32_t* __restrict__ slot_row, int32_t* __restrict__ uniq, int32_t* __restrict__ link,
                     int32_t* __restrict__ count) {
+  pdl_wait();                          // nothing before the wait (count was zeroed by the previous call's expand)
+  pdl_trigger();
   const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= M) return;
   const uint32_t v = (uint32_t)__ldg(a_index + n);
@@ -690,6 +721,8 @@ dedup_insert_kernel(const int32_t* __restrict__ a_index, int64_t M, unsigned lon
 __global__ void __launch_bounds__(256)
 dedup_expand_kernel(const float* __restrict__ P, const int32_t* __restrict__ slot_row, const int32_t* __restrict__ link,
                     float* __restrict__ C, int64_t ldc, int64_t M, int N, int32_t* __restrict__ count) {
+  pdl_wait();                          // nothing before the wait
+  pdl_trigger();
   if (blockIdx.x == 0 && threadIdx.x == 0) *count = 0;
   const int64_t n = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (n >= M) return;
@@ -764,9 +797,9 @@ bool umma_shape_ok(int N, int K) { return (K % 4 == 0) && (N % 8 == 0) && N > 0 
 // Pack logical B[k][n] = B[k*sk + n*sn] (K x N) into tiles [tile_offset, tile_offset + ceil(N/200)) of Bp.
 int umma_pack_b(const float* B, int64_t sk, int64_t sn, int N, int K, void* Bp, int tile_offset, cudaStream_t stream) {
   const int n_tiles = (N + UN - 1) / UN, n_chunks = (K + P_BK - 1) / P_BK;
-  umma_pack_b_kernel<<<dim3(n_tiles, n_chunks, 7), 256, 0, stream>>>(B, sk, sn, N, K, (uint8_t*)Bp, n_chunks, tile_offset);
-  RENET_CHECK_LAUNCH("umma_pack_b_kernel");
-  return RENET_OK;
+  return launch_pdl("umma_pack_b_kernel", {}, {{Bp, (int64_t)(tile_offset + n_tiles) * n_chunks * P_B_CHUNK}},
+                    umma_pack_b_kernel, dim3(n_tiles, n_chunks, 7), dim3(256), 0, stream, B, sk, sn, N, K, (uint8_t*)Bp,
+                    n_chunks, tile_offset);
 }
 
 // The resident-panel kernel serves EPI 0 products without split-K whose panels fit shared memory and the grid.
@@ -788,15 +821,21 @@ static int launch_resident(const float* A, const int32_t* a_index, int64_t lda, 
   // every panel gets at least one CTA; a CTA never holds more than one panel
   const int64_t n_work = (int64_t)n_panels * ((M + 63) / 64);
   const unsigned grid = (unsigned)(n_work < kNumSMs ? n_work : kNumSMs);
+  // The panel copies go before the kernel's griddepcontrol.wait unless the previous kernel writes the packed image (its
+  // pack ran in this call); its other inputs are read after the wait, so the launch itself always qualifies for PDL
+  const int64_t bp_bytes = (int64_t)(batch - 1) * batch_bp + umma_packed_bytes(N, K);
+  const int early = pdl_disjoint(stream, {{Bp, bp_bytes}}) ? 1 : 0;
+  const DevSpan c_span = {C, ((int64_t)(batch - 1) * batch_c + (M - 1) * ldc + N) * 4};
+  int rc;
   if (a_index)
-    umma_gemm_resident_kernel<true><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
-                                                                        m_dev, N, K, n_chunks, accumulate, batch_a, batch_bp,
-                                                                        batch_c, n_panels, g_gemm_dbg);
+    rc = launch_pdl("umma_gemm_resident_kernel", {}, {c_span}, umma_gemm_resident_kernel<true>, dim3(grid), dim3(R_THREADS),
+                    R_SMEM, stream, A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M, m_dev, N, K, n_chunks,
+                    (int)accumulate, batch_a, batch_bp, batch_c, n_panels, early, g_gemm_dbg);
   else
-    umma_gemm_resident_kernel<false><<<grid, R_THREADS, R_SMEM, stream>>>(A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M,
-                                                                         m_dev, N, K, n_chunks, accumulate, batch_a, batch_bp,
-                                                                         batch_c, n_panels, g_gemm_dbg);
-  RENET_CHECK_LAUNCH("umma_gemm_resident_kernel");
+    rc = launch_pdl("umma_gemm_resident_kernel", {}, {c_span}, umma_gemm_resident_kernel<false>, dim3(grid), dim3(R_THREADS),
+                    R_SMEM, stream, A, a_index, lda, (const uint8_t*)Bp, C, ldc, bias, M, m_dev, N, K, n_chunks,
+                    (int)accumulate, batch_a, batch_bp, batch_c, n_panels, early, g_gemm_dbg);
+  if (rc) return rc;
   note_gemm_kernel(RENET_GEMM_RESIDENT);
   return RENET_OK;
 }
@@ -861,12 +900,14 @@ static int umma_gemm_dedup(const float* A, const int32_t* a_index, int64_t lda, 
   int32_t* slot_row = reinterpret_cast<int32_t*>(P + M * N);
   int32_t* uniq = slot_row + slots;
   int32_t* link = uniq + M;
-  dedup_insert_kernel<<<(unsigned)((M + 255) / 256), 256, 0, stream>>>(a_index, M, table, bits, epoch, slot_row, uniq, link,
-                                                                       count);
-  RENET_CHECK_LAUNCH("dedup_insert_kernel");
+  const DevSpan keys_span = {keys.p, keys.bytes}, rows_span = {rows.p, rows.bytes};
+  if ((rc = launch_pdl("dedup_insert_kernel", {}, {keys_span, rows_span}, dedup_insert_kernel, dim3((unsigned)((M + 255) / 256)),
+                       dim3(256), 0, stream, a_index, M, table, bits, epoch, slot_row, uniq, link, count)))
+    return rc;
   if ((rc = launch_resident(A, uniq, lda, Bp, P, N, bias, M, count, N, K, false, 1, 0, 0, 0, stream))) return rc;
-  dedup_expand_kernel<<<(unsigned)((M + 7) / 8), 256, 0, stream>>>(P, slot_row, link, C, ldc, M, N, count);
-  RENET_CHECK_LAUNCH("dedup_expand_kernel");
+  if ((rc = launch_pdl("dedup_expand_kernel", {}, {{C, ((M - 1) * ldc + N) * 4}, {count, 4}}, dedup_expand_kernel,
+                       dim3((unsigned)((M + 7) / 8)), dim3(256), 0, stream, P, slot_row, link, C, ldc, M, N, count)))
+    return rc;
   note_gemm_kernel(RENET_GEMM_DEDUP);
   return RENET_OK;
 }
